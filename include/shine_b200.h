@@ -1,5 +1,5 @@
 /*
- * shine_b200.h — C ABI of the B200-native (sm_100a) implementation of SHINE-mapping's per-point SDF
+ * shine_b200.h — C ABI of the H100-native (sm_90a) implementation of SHINE-mapping's per-point SDF
  * training step.  Plain C: raw device pointers + sizes + a cudaStream_t passed as void*; no torch types.
  *
  * The reference (PRBonn/SHINE_mapping @ 0fbaf8a) is 100 % Python and has NO FFI boundary for this path:
@@ -42,7 +42,7 @@ extern "C" {
 #define SHINE_FLAG_REDUCTION_SUM 1u   /* loss_reduction == "sum" (shine_incre.py:77-78); default mean   */
 #define SHINE_FLAG_WEIGHTED 2u        /* loss_weight_on (utils/loss.py:18-19): per-sample weight applied */
 #define SHINE_FLAG_TF32X1 4u          /* decoder contractions in plain TF32 (default: 3xTF32 ~ fp32)     */
-#define SHINE_FLAG_TCGEN05 8u         /* shine_sdf_infer / shine_sdf_bce_step: decoder on tcgen05.mma with TMEM accumulators
+#define SHINE_FLAG_TCGEN05 8u         /* shine_sdf_infer / shine_sdf_bce_step: decoder on warpgroup MMAs (wgmma)
                                          (128-point tiles, warp-specialised gather / epilogue warps) instead of
                                          warp-level mma.sync                                                  */
 #define SHINE_FLAG_MORTON_ORDERED 16u  /* shine_sdf_bce_step: the batch is in Morton order of its coordinates (the order the

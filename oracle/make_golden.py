@@ -1,10 +1,11 @@
 """Mint tests/golden/*.npz from the UNMODIFIED reference classes.  *** TEST INFRASTRUCTURE ***
 
-Runs only in the build container (needs /root/reference; kaolin is replaced by oracle/kaolin_shim).  Imports the
+Runs only where the reference checkout is available (SHINE_REFERENCE, default /root/reference; kaolin is replaced by
+oracle/kaolin_shim).  Imports the
 reference's own `FeatureOctree`, `Decoder`, `sdf_bce_loss`, `dataSampler`, `SHINEConfig` verbatim and drives
 them exactly like the loop body of shine_batch.py:123-209 on the CPU; the inputs and every output are frozen so
 that the oracle restatement (tests/test_oracle_golden.py) and the CUDA path (tests/test_gpu_parity.py) can be
-checked against the reference itself on the GPU box, where /root/reference does not exist.
+checked against the reference itself without the reference checkout.
 
     python oracle/make_golden.py            # rewrites tests/golden/*.npz
 """
@@ -167,6 +168,49 @@ def make_eikonal(name, feat_levels, n_azimuth, n_batch, seed, poly=True, weight_
           f"({os.path.getsize(path) / 1e6:.2f} MB)")
 
 
+# the make_case() cases of tests/test_reference_live.py: (levels, frames, poly)
+LIVE_CASES = [(2, 1, True), (4, 2, True), (3, 2, False)]
+
+
+def make_live_cases(name="ref_live_cases"):
+    """The reference's indices, prediction, loss and table gradients on the seeded parity cases of
+    tests/test_reference_live.py (tests/parity_utils.make_case), one key prefix per case."""
+    SHINEConfig, FeatureOctree, Decoder, _, sdf_bce_loss = import_reference()
+    sys.path.insert(0, ROOT)
+    from tests.parity_utils import make_case
+    out = {}
+    for levels, frames, poly in LIVE_CASES:
+        case = make_case(n_points=1200, n_batch=1000, feat_levels=levels, seed=77 + levels, n_frames=frames, poly=poly)
+        c = SHINEConfig(); c.device = "cpu"
+        c.tree_level_world, c.tree_level_feat, c.leaf_vox_size, c.poly_int_on = 12, levels, 0.2, poly
+        c.calculate_world_scale()
+        octree, dec = FeatureOctree(c), Decoder(c)
+        for fr in case["frames"]:
+            octree.update(torch.from_numpy(fr), False)
+        with torch.no_grad():
+            for p, t in zip(octree.hier_features, case["tables"]):
+                p.copy_(torch.from_numpy(t))
+        sd = dec.state_dict()
+        for k, v in case["dec"].items():
+            sd[k] = torch.from_numpy(v)
+        dec.load_state_dict(sd)
+        coord, label = torch.from_numpy(case["coord"]), torch.from_numpy(case["label"])
+        pred = dec.sdf(octree.query_feature(coord))
+        loss = sdf_bce_loss(pred, label, case["cfg"]["sigma"], None, False, "mean")
+        loss.backward()
+        key = f"l{levels}_f{frames}_p{int(poly)}_"
+        out[key + "coord"] = case["coord"]
+        out[key + "pred"] = pred.detach().numpy()
+        out[key + "loss"] = np.array(float(loss))
+        for i, idx in enumerate(octree.hierarchical_indices):
+            out[key + f"indices_{i}"] = idx.numpy().astype(np.int32)
+        for i, p in enumerate(octree.hier_features):
+            out[key + f"tgrad_{i}"] = p.grad.numpy()
+    path = os.path.join(ROOT, "tests", "golden", name + ".npz")
+    np.savez_compressed(path, **out)
+    print(f"{name}: {len(LIVE_CASES)} cases -> {path} ({os.path.getsize(path) / 1e6:.2f} MB)")
+
+
 if __name__ == "__main__":
     if not os.path.isdir(REF):
         sys.exit(f"{REF} not found: goldens can only be minted where the reference is mounted")
@@ -176,3 +220,4 @@ if __name__ == "__main__":
     make("ref_incre_l3_sum_weighted_linear", feat_levels=3, n_frames=2, n_azimuth=10, n_batch=1200, seed=44,
          poly=False, weighted=True, reduction="sum")
     make_eikonal("ref_eikonal_l3", feat_levels=3, n_azimuth=10, n_batch=1000, seed=45)
+    make_live_cases()

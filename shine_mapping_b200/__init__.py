@@ -1,4 +1,4 @@
-"""shine_mapping_b200 — B200-native (sm_100a) implementation of SHINE-mapping's per-point SDF training step
+"""shine_mapping_b200 — H100-native (sm_90a) implementation of SHINE-mapping's per-point SDF training step
 behind the reference's own `FeatureOctree` / `Decoder` / `sdf_bce_loss` surfaces (see DESIGN.md)."""
 from .config import SHINEConfig
 from .decoder import Decoder

@@ -1,7 +1,7 @@
 """ctypes binding of the C ABI in include/shine_b200.h (csrc/libshine_b200.so).
 
 There is no fallback: if the library is missing or a call fails, an exception is raised.  The library is
-built in-tree by `__graft_entry__.build()` (nvcc, sm_100a).
+built in-tree by `__graft_entry__.build()` (nvcc, sm_90a).
 """
 from __future__ import annotations
 
@@ -150,7 +150,7 @@ def lib() -> C.CDLL:
     if _lib is None:
         if not os.path.exists(LIB_PATH):
             raise ShineB200Error(
-                f"{LIB_PATH} is missing: build the sm_100a kernels first (python -c 'import __graft_entry__ as g; "
+                f"{LIB_PATH} is missing: build the sm_90a kernels first (python -c 'import __graft_entry__ as g; "
                 "g.build()').  shine_mapping_b200 has no CPU or eager fallback for the hot path.")
         handle = C.CDLL(LIB_PATH)
         for name, (restype, argtypes) in SYMBOLS.items():
@@ -175,7 +175,7 @@ def check(rc: int, what: str) -> None:
 def require_cuda(t: torch.Tensor, what: str) -> None:
     if not t.is_cuda:
         raise ShineB200Error(
-            f"{what}: tensor is on {t.device}; the hot path runs only as sm_100a CUDA kernels (no CPU fallback)")
+            f"{what}: tensor is on {t.device}; the hot path runs only as sm_90a CUDA kernels (no CPU fallback)")
 
 
 def ptr(t):

@@ -1,4 +1,4 @@
-// shine_b200.cu — hand-written sm_100a kernels + the C ABI of include/shine_b200.h.
+// shine_b200.cu — hand-written sm_90a kernels + the C ABI of include/shine_b200.h.
 //
 // Hot path (reference PRBonn/SHINE_mapping, shine_batch.py:123-209):
 //   FeatureOctree.query_feature  (model/feature_octree.py:199-244)   Morton hash walk + 8-corner blend, L levels
@@ -13,7 +13,7 @@
 // That "row-half" layout converts to / from the mma A-fragment / C-fragment layouts with two
 // shfl.xor(1) each (see to_afrag / from_cfrag), so activations never touch shared memory in the forward.
 //
-// Built with: nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 (see __graft_entry__.build()).
+// Built with: nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 (see __graft_entry__.build()).
 
 #include <cuda_runtime.h>
 #include <math.h>
@@ -21,10 +21,9 @@
 
 #include "shine_b200.h"
 
-// tuning switches (defaults = the best measured on B200; every alternative is in profiles/r01_summary.md)
-// Front-end of the fused kernel (A/B on B200, profiles/r02_summary.md): reading key + 4 corner rows as one 32-byte
-// sector per level (every lane probes every level) wins for inference (0.140 -> 0.132 ms) but costs the training
-// kernel 12 % more instructions (0.296 -> 0.333 ms); the level-split key probe + ids load is kept there.
+// tuning switches.  Front-end of the fused kernel: reading key + 4 corner rows as one 32-byte sector per level (every
+// lane probes every level) is used for inference; the training kernel keeps the level-split key probe + ids load, which
+// issues fewer instructions.
 #ifndef SHINE_SECTOR_PROBE_TRAIN
 #define SHINE_SECTOR_PROBE_TRAIN 0
 #endif
@@ -33,9 +32,6 @@
 #endif
 #ifndef SHINE_CPASYNC_PREFETCH
 #define SHINE_CPASYNC_PREFETCH 0  // 1: next tile's inputs via cp.async to shared memory; 0: register prefetch (timing-neutral)
-#endif
-#ifndef SHINE_DW3_TMEM
-#define SHINE_DW3_TMEM 1      // 1: output-layer weight-gradient accumulators parked in TMEM; 0: registers
 #endif
 #ifndef SHINE_GATHER_GROUP
 #define SHINE_GATHER_GROUP 2  // levels whose first-probe sectors are in flight together (register pressure vs parallelism)
@@ -56,7 +52,14 @@
 #define SHINE_EXPERIMENT_NO_RED 0
 #endif
 #ifndef SHINE_TRAIN_MINB
-#define SHINE_TRAIN_MINB 2    // min resident blocks/SM of the training kernel (register cap 65536/(256*MINB))
+#define SHINE_TRAIN_MINB 2    // min resident blocks/SM of the training kernels (register cap 65536/(256*MINB))
+#endif
+// The per-point training kernels with decoder gradients keep 56 accumulators per lane live through the whole tile: at 2
+// blocks/SM (128 registers) they spill ~0.5 KB per thread, at 1 block/SM (255) they do not, and on H100 the spill-free
+// build is faster (C2 batch in the order drawn, kernel: 0.460 vs 0.564 ms).  The grouped kernel timed on Morton-ordered batches
+// spills ~0.3 KB at 2 blocks/SM and is still faster there than at 1 (0.228 vs 0.252 ms): it keeps SHINE_TRAIN_MINB.
+#ifndef SHINE_TRAIN_DECGRAD_MINB
+#define SHINE_TRAIN_DECGRAD_MINB 1
 #endif
 #ifndef SHINE_INFER_MINB
 #define SHINE_INFER_MINB 3
@@ -320,24 +323,9 @@ __device__ __forceinline__ void from_cfrag(const float (&c)[4], int odd, float (
     else      { v[0] = r0;   v[1] = r1;   v[2] = c[2]; v[3] = c[3]; }
 }
 
-// ------------------------------------------------------------------------------------------------------
-// Tensor Memory as accumulator parking space.  The decoder-gradient accumulators (56 fp32 per lane: dW2 32,
-// dW1 8, db2 8, db1 8) are only touched in the wgrad section of a tile; between tiles they live in TMEM
-// (tcgen05.st / tcgen05.ld -> SASS STTM / LDTM) instead of pinning registers through the gather and MLP phases.
-// Warp w of the block owns TMEM lanes 32*(w&3).. and columns 64*(w>>2)..+55 of the block's 128-column allocation.
-// ------------------------------------------------------------------------------------------------------
-// register view: dW2[2][4][4] (cols 0..31), dW1[2][4] (32..39), db2[4][2] (40..47), db1[4][2] (48..55), dw3[4][2] (56..63)
+// decoder-gradient accumulators of a lane (mma.sync C fragments): dW2[2][4][4], dW1[2][4], and the per-column partial
+// sums of db2, db1, dw3 ([4][2]: columns 8j + 2t + q)
 #define SHINE_ACC_DECL float dW2[2][4][4], dW1[2][4], db2p[4][2], db1p[4][2], dw3p[4][2]
-#define SHINE_ACC_LOAD(ta)                                                                             \
-    do {                                                                                               \
-        tmem_ld32((ta), &dW2[0][0][0]); tmem_ld8((ta) + 32, &dW1[0][0]); tmem_ld8((ta) + 40, &db2p[0][0]); \
-        tmem_ld8((ta) + 48, &db1p[0][0]); tmem_ld8((ta) + 56, &dw3p[0][0]); tmem_wait_ld();              \
-    } while (0)
-#define SHINE_ACC_STORE(ta)                                                                            \
-    do {                                                                                               \
-        tmem_st32((ta), &dW2[0][0][0]); tmem_st8((ta) + 32, &dW1[0][0]); tmem_st8((ta) + 40, &db2p[0][0]); \
-        tmem_st8((ta) + 48, &db1p[0][0]); tmem_st8((ta) + 56, &dw3p[0][0]); tmem_wait_st();              \
-    } while (0)
 
 // ------------------------------------------------------------------------------------------------------
 // the fused kernel: hash walk + gather + blend + MLP (+ BCE loss) (+ full backward with scatter-add)
@@ -489,7 +477,8 @@ __device__ __forceinline__ void grouped_scatter(const StepParams& P, int L, int 
 }
 
 template <int NTF, bool TRAIN, bool DEC_GRAD, int LMAX, bool GROUPED = false>
-__global__ void __launch_bounds__(256, TRAIN ? SHINE_TRAIN_MINB : SHINE_INFER_MINB) sdf_fused_kernel(const __grid_constant__ StepParams P) {
+__global__ void __launch_bounds__(256, !TRAIN ? SHINE_INFER_MINB : (DEC_GRAD && !GROUPED) ? SHINE_TRAIN_DECGRAD_MINB : SHINE_TRAIN_MINB)
+sdf_fused_kernel(const __grid_constant__ StepParams P) {
     static_assert(!GROUPED || TRAIN, "the grouped scatter belongs to the training kernels");
     static_assert(SmemPlan::kStagePerWarp >= SmemPlan::kDecGradFloats, "a warp's staging area holds its partial decoder gradient");
     extern __shared__ __align__(16) float smem[];
@@ -517,40 +506,18 @@ __global__ void __launch_bounds__(256, TRAIN ? SHINE_TRAIN_MINB : SHINE_INFER_MI
         smem[SmemPlan::W3 + tid] = P.dec.w3[tid];
     }
     if (tid == 0) smem[SmemPlan::B3] = P.dec.b3 ? P.dec.b3[0] : 0.f;
-    // Tensor-Memory parking areas of this warp (lanes 32*(warp&3).., column group warp>>2):
-    //   tpark: per-tile state that must survive the MLP phase (blend factors tx,ty,tz of every level + slot indices)
-    //   tacc : decoder-gradient accumulators (DEC_GRAD only)
-    constexpr int kPark = LMAX <= 4 ? 16 : 32;                           // blend factors + slots parked per lane
+    constexpr int kPark = LMAX <= 4 ? 16 : 32;                           // blend factors of every level, per lane
     constexpr int kIdPark = 4 * LMAX;                                    // this lane's 4 corner rows of every level
-    constexpr int kColsPerGroup = DEC_GRAD ? 128 : (kPark + kIdPark);    // 56 acc (+pad to 64) + park + ids
-    constexpr int kTmemCols = TRAIN ? 2 * kColsPerGroup : 0;             // 256 (dec grads) / 32 / 64, power of two
-    uint32_t tacc = 0, tpark = 0;
-    if (TRAIN) {
-        if (warp == 0) {   // one warp allocates for the block (2 blocks/SM x 256 columns = the SM's 512)
-            const uint32_t sa = (uint32_t)__cvta_generic_to_shared(smu + SmemPlan::B3 + 1);
-            asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(sa), "n"(kTmemCols > 0 ? kTmemCols : 32) : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-        }
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    }
     __syncthreads();
-    if (TRAIN) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        tacc = smu[SmemPlan::B3 + 1] + ((uint32_t)(32 * (warp & 3)) << 16) + (uint32_t)kColsPerGroup * (uint32_t)(warp >> 2);
-        tpark = tacc + (DEC_GRAD ? 64u : 0u);
+    SHINE_ACC_DECL;
+#pragma unroll
+    for (int a = 0; a < 2; ++a) {
+#pragma unroll
+        for (int b = 0; b < 4; ++b) { dW2[a][b][0] = dW2[a][b][1] = dW2[a][b][2] = dW2[a][b][3] = 0.f; }
+        dW1[a][0] = dW1[a][1] = dW1[a][2] = dW1[a][3] = 0.f;
     }
-    if (DEC_GRAD) {
-        SHINE_ACC_DECL;
 #pragma unroll
-        for (int a = 0; a < 2; ++a) {
-#pragma unroll
-            for (int b = 0; b < 4; ++b) { dW2[a][b][0] = dW2[a][b][1] = dW2[a][b][2] = dW2[a][b][3] = 0.f; }
-            dW1[a][0] = dW1[a][1] = dW1[a][2] = dW1[a][3] = 0.f;
-        }
-#pragma unroll
-        for (int j = 0; j < 4; ++j) { db2p[j][0] = db2p[j][1] = db1p[j][0] = db1p[j][1] = dw3p[j][0] = dw3p[j][1] = 0.f; }
-        SHINE_ACC_STORE(tacc);
-    }
+    for (int j = 0; j < 4; ++j) { db2p[j][0] = db2p[j][1] = db1p[j][0] = db1p[j][1] = dw3p[j][0] = dw3p[j][1] = 0.f; }
 
     constexpr bool kSectorProbe = TRAIN ? (SHINE_SECTOR_PROBE_TRAIN != 0) : (SHINE_SECTOR_PROBE_INFER != 0);
     constexpr bool kSlotPrefetch = TRAIN && !kSectorProbe && (SHINE_SLOT_PREFETCH != 0) && (SHINE_CPASYNC_PREFETCH == 0);
@@ -560,14 +527,8 @@ __global__ void __launch_bounds__(256, TRAIN ? SHINE_TRAIN_MINB : SHINE_INFER_MI
     const float up = (TRAIN && P.d_loss) ? __ldg(P.d_loss) : 1.0f;
     const float gscale = P.loss_scale * up;
 
-    // decoder-gradient accumulators: dW2/dW1/db2/db1/dw3 are parked in TMEM (SHINE_ACC_*); only db3 stays in a register
     float db3p = 0.f;
     float loss_acc = 0.f;
-#if !SHINE_DW3_TMEM
-    float dw3r[4][2];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) { dw3r[j][0] = dw3r[j][1] = 0.f; }
-#endif
 
     float* stage = smem + SmemPlan::STAGE + warp * SmemPlan::kStagePerWarp;   // only touched when DEC_GRAD
     float* stA = stage;                       // [16][kWS]
@@ -749,7 +710,7 @@ __global__ void __launch_bounds__(256, TRAIN ? SHINE_TRAIN_MINB : SHINE_INFER_MI
 
 #endif
         float feat[4];
-        float pk[kPark];      // [3i..3i+2] = tx,ty,tz of level i (parked in TMEM over the MLP phase)
+        float pk[kPark];      // [3i..3i+2] = tx,ty,tz of level i (kept over the MLP phase for the scatter)
         float idp[kIdPark];   // [4i..4i+3] = rows of this lane's corners (z bit == half) of level i, -1 on a miss
         uint32_t hitmask = 0;
         if constexpr (kSectorProbe) {
@@ -921,11 +882,6 @@ __global__ void __launch_bounds__(256, TRAIN ? SHINE_TRAIN_MINB : SHINE_INFER_MI
             continue;
         }
 #endif
-        if (TRAIN && !GROUPED) {
-            if (kPark == 16) tmem_st16(tpark, pk); else tmem_st32(tpark, pk);
-            if (kIdPark == 16) tmem_st16(tpark + kPark, idp); else tmem_st32(tpark + kPark, idp);
-            tmem_wait_st();
-        }
         if (!TRAIN && P.mask) {
             bool present = false;
 #pragma unroll
@@ -1043,17 +999,13 @@ __global__ void __launch_bounds__(256, TRAIN ? SHINE_TRAIN_MINB : SHINE_INFER_MI
         const float dpx = __shfl_xor_sync(kFull, dpo, 1);
         const float dp0 = odd ? dpx : dpo, dp8 = odd ? dpo : dpx;
         float dh2[4][4];
-        float db2t[4][2], db1t[4][2], dw3t[4][2];   // this tile's partials, folded into the TMEM accumulators in the wgrad section
+        float db2t[4][2], db1t[4][2], dw3t[4][2];   // this tile's partials, folded into the accumulators in the wgrad section
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             dh2[j][0] = h2[j][0] > 0.f ? dp0 * w3a[j] : 0.f; dh2[j][1] = h2[j][1] > 0.f ? dp0 * w3b[j] : 0.f;
             dh2[j][2] = h2[j][2] > 0.f ? dp8 * w3a[j] : 0.f; dh2[j][3] = h2[j][3] > 0.f ? dp8 * w3b[j] : 0.f;
             if (DEC_GRAD) {
-#if SHINE_DW3_TMEM
                 dw3t[j][0] = dp0 * h2[j][0] + dp8 * h2[j][2];  dw3t[j][1] = dp0 * h2[j][1] + dp8 * h2[j][3];
-#else
-                dw3r[j][0] += dp0 * h2[j][0] + dp8 * h2[j][2]; dw3r[j][1] += dp0 * h2[j][1] + dp8 * h2[j][3];
-#endif
                 db2t[j][0] = dh2[j][0] + dh2[j][2];            db2t[j][1] = dh2[j][1] + dh2[j][3];
                 *reinterpret_cast<float2*>(stA + g * kWS + 8 * j + 2 * t) = make_float2(dh2[j][0], dh2[j][1]);
                 *reinterpret_cast<float2*>(stA + (g + 8) * kWS + 8 * j + 2 * t) = make_float2(dh2[j][2], dh2[j][3]);
@@ -1109,15 +1061,11 @@ __global__ void __launch_bounds__(256, TRAIN ? SHINE_TRAIN_MINB : SHINE_INFER_MI
 
         // ---- backward: decoder weight grads (contraction over the tile's 16 points) -------------------
         if (DEC_GRAD) {
-            SHINE_ACC_DECL;
-            SHINE_ACC_LOAD(tacc);
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
                 db2p[j][0] += db2t[j][0]; db2p[j][1] += db2t[j][1];
                 db1p[j][0] += db1t[j][0]; db1p[j][1] += db1t[j][1];
-#if SHINE_DW3_TMEM
                 dw3p[j][0] += dw3t[j][0]; dw3p[j][1] += dw3t[j][1];
-#endif
             }
             __syncwarp();
             // dW2[n2][k1] += sum_rows dh2[row][n2] * h1[row][k1]
@@ -1150,7 +1098,6 @@ __global__ void __launch_bounds__(256, TRAIN ? SHINE_TRAIN_MINB : SHINE_INFER_MI
                 mma3x2<NTF>(dW1[0], dW1[1], a0, a1, bh, bl, bh, bl);
             }
             __syncwarp();
-            SHINE_ACC_STORE(tacc);
         }
 
         // ---- backward: scatter-add into the corner-feature tables (index_put_ accumulate) -------------
@@ -1164,10 +1111,8 @@ __global__ void __launch_bounds__(256, TRAIN ? SHINE_TRAIN_MINB : SHINE_INFER_MI
         }
         float dx[4];
         from_cfrag(dxc, odd, dx);
-        float qk[kPark], qid[kIdPark];
-        if (kPark == 16) tmem_ld16(tpark, qk); else tmem_ld32(tpark, qk);
-        if (kIdPark == 16) tmem_ld16(tpark + kPark, qid); else tmem_ld32(tpark + kPark, qid);
-        tmem_wait_ld();
+        const float (&qk)[kPark] = pk;
+        const float (&qid)[kIdPark] = idp;
 #pragma unroll
         for (int i = 0; i < LMAX; ++i) {
             // the 8 corner rows: this lane kept the 4 with z bit == half, its partner (lane ^ 2) the other 4
@@ -1214,8 +1159,6 @@ __global__ void __launch_bounds__(256, TRAIN ? SHINE_TRAIN_MINB : SHINE_INFER_MI
         if (lane == 0 && loss_acc != 0.f) atomicAdd(P.loss, loss_acc * P.loss_scale);
     }
     if (DEC_GRAD) {
-        SHINE_ACC_DECL;
-        SHINE_ACC_LOAD(tacc);
         // every warp writes its complete partial gradient vector [gw1 256 | gb1 32 | gw2 1024 | gb2 32 | gw3 32 | gb3 1]
         // into its own staging area (each element has exactly one owner lane: plain stores, no shared-memory atomics),
         // then the block sums the eight vectors and issues one global atomic per non-zero element
@@ -1236,11 +1179,7 @@ __global__ void __launch_bounds__(256, TRAIN ? SHINE_TRAIN_MINB : SHINE_INFER_MI
         for (int j = 0; j < 4; ++j) {
 #pragma unroll
             for (int q = 0; q < 2; ++q) {
-#if SHINE_DW3_TMEM
                 float a = db1p[j][q], b = db2p[j][q], c = dw3p[j][q];
-#else
-                float a = db1p[j][q], b = db2p[j][q], c = dw3r[j][q];
-#endif
 #pragma unroll
                 for (int o = 4; o < 32; o <<= 1) {
                     a += __shfl_xor_sync(kFull, a, o); b += __shfl_xor_sync(kFull, b, o); c += __shfl_xor_sync(kFull, c, o);
@@ -1271,26 +1210,18 @@ __global__ void __launch_bounds__(256, TRAIN ? SHINE_TRAIN_MINB : SHINE_INFER_MI
             if (dst) atomicAdd(dst, v);
         }
     }
-    if (TRAIN) {
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncthreads();
-        if (warp == 0) {
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(smu[SmemPlan::B3 + 1]), "n"(kTmemCols > 0 ? kTmemCols : 32) : "memory");
-        }
-    }
 }
 
 
 // ------------------------------------------------------------------------------------------------------
-// tcgen05 inference kernel (SHINE_FLAG_TCGEN05): query_feature -> Decoder.sdf with the decoder on the 5th-gen
-// tensor cores.  One thread per point: it walks the hash, gathers its 8 x L rows with 256-bit loads and blends all
-// 8 channels, then the block's 128 feature vectors become the A operand (M = 128 points) of
-//     D1[128x32] = X[128x8] * W1^T      (tcgen05.mma kind::tf32, 3xTF32: hi*hi + lo*hi + hi*lo)
+// Warpgroup-MMA inference kernel (SHINE_FLAG_TCGEN05): query_feature -> Decoder.sdf with the decoder on wgmma.
+// Two threads per point walk the hash, gather the 8 x L rows and blend all 8 channels; the block's 128 feature vectors
+// become the A operand (M = 128 points, two m64 instructions) of
+//     D1[128x32] = X[128x8] * W1^T      (wgmma kind tf32, 3xTF32: hi*hi + lo*hi + hi*lo)
 //     D2[128x32] = relu(D1+b1)[128x32] * W2^T
 // with operands in shared memory (canonical K-major, no swizzle: 8-row x 16-byte core matrices, LBO = 128 B between
-// the two K-chunks of one MMA, SBO = stride of an 8-row group) and accumulators in Tensor Memory; every thread reads
-// its own row of D back with tcgen05.ld (TMEM lane = point) for bias / ReLU / the 32->1 output layer.
+// the two K-chunks of one MMA, SBO = stride of an 8-row group) and the accumulators in registers (mma.sync C-fragment
+// layout); bias / ReLU / the 32->1 output layer work on the fragments, a row's dot product is summed over its lane quad.
 // ------------------------------------------------------------------------------------------------------
 
 struct TcPlan {                                   // byte offsets in dynamic shared memory
@@ -1303,20 +1234,17 @@ struct TcPlan {                                   // byte offsets in dynamic sha
     static constexpr int W2H = W1L + 1024;        // W2  hi  [4 groups][8 chunks][8][16 B]         = 4 KB
     static constexpr int W2L = W2H + 4096;
     static constexpr int VEC = W2L + 4096;        // b1[32] b2[32] w3[32] b3 (floats)
-    static constexpr int BAR = VEC + 100 * 4;     // mbarrier (8 B), tmem base (4 B)
-    static constexpr int BYTES = BAR + 16;
+    static constexpr int BYTES = VEC + 100 * 4;
 };
 
 template <int LMAX>
 __global__ void __launch_bounds__(128, 5) sdf_infer_tc_kernel(const __grid_constant__ StepParams P) {
     extern __shared__ __align__(128) unsigned char tsm[];
-    const int tid = threadIdx.x, warp = tid >> 5;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const uint32_t sbase = (uint32_t)__cvta_generic_to_shared(tsm);
     float* vec = reinterpret_cast<float*>(tsm + TcPlan::VEC);
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tsm + TcPlan::BAR + 8);
-    const uint32_t bar = sbase + TcPlan::BAR;
 
-    // ---- prologue: weights (hi/lo) into the canonical UMMA layout, TMEM allocation, mbarrier -------------------
+    // ---- prologue: weights (hi/lo) into the canonical K-major layout ---------------------------------------
     for (int i = tid; i < kH * kF; i += 128) {
         const int n = i / kF, k = i % kF;
         uint32_t hi, lo; split_tf32(P.dec.w1[i], hi, lo);
@@ -1336,23 +1264,8 @@ __global__ void __launch_bounds__(128, 5) sdf_infer_tc_kernel(const __grid_const
         vec[32 + tid] = P.dec.b2 ? P.dec.b2[tid] : 0.f;
         vec[64 + tid] = P.dec.w3[tid];
     }
-    if (tid == 0) {
-        vec[96] = P.dec.b3 ? P.dec.b3[0] : 0.f;
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar) : "memory");
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 64;" ::"r"(sbase + TcPlan::BAR + 8) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+    if (tid == 0) vec[96] = P.dec.b3 ? P.dec.b3[0] : 0.f;
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem = *tmem_slot;
-    const uint32_t trow = tmem + ((uint32_t)(32 * warp) << 16);          // this warp's 32 TMEM lanes
-    // instruction descriptor: D=F32, A=B=TF32, both K-major, N=32 (>>3), M=128 (>>4)
-    constexpr uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((32u >> 3) << 17) | ((128u >> 4) << 24);
 
     const bool poly = P.oct.poly_interp != 0;
     const int L = P.oct.num_levels;
@@ -1360,14 +1273,13 @@ __global__ void __launch_bounds__(128, 5) sdf_infer_tc_kernel(const __grid_const
 #pragma unroll
     for (int i = 1; i < LMAX; ++i)
         if (i < L && P.oct.lv[i].level != P.oct.lv[0].level - i) consecutive = false;
-    uint32_t phase = 0;
-    const int rg = tid >> 3, r0 = tid & 7;                                   // 8-row group / row within it
+    const int g = lane >> 2, t = lane & 3;                                // accumulator fragment: rows g, g+8; cols 2t, 2t+1
     const int num_tiles = (int)((P.n + 127) / 128);
 
     const int half = tid & 1;                                              // gather: two adjacent lanes per point
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         // ---- hash walk + gather + blend with two lanes per point (levels split for probing, corners split by z bit so
-        //      the pair's two LDG.256 of one instruction hit z-neighbour rows = usually one 128-byte line); two passes of
+        //      the pair's row loads of one instruction hit z-neighbour rows = usually one 128-byte line); two passes of
         //      64 points fill the 128-row A tile ----
 #pragma unroll 1
         for (int pass = 0; pass < 2; ++pass) {
@@ -1433,78 +1345,82 @@ __global__ void __launch_bounds__(128, 5) sdf_infer_tc_kernel(const __grid_const
             *reinterpret_cast<uint4*>(tsm + TcPlan::A1H + off) = make_uint4(h4[0], h4[1], h4[2], h4[3]);
             *reinterpret_cast<uint4*>(tsm + TcPlan::A1L + off) = make_uint4(l4[0], l4[1], l4[2], l4[3]);
         }
-        const int64_t p = (int64_t)tile * 128 + tid;          // epilogues: one thread per row of the tile
-        const bool valid = p < P.n;
-
-        // ---- layer 1 on the tensor core ----------------------------------------------------------------------------
+        // ---- layer 1 on the tensor core (rows 0..63 and 64..127: SBO 256 B -> 8 groups = 2048 B) -------------------
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
         __syncthreads();
-        if (tid == 0) {
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint64_t ah = umma_desc(sbase + TcPlan::A1H, 128, 256), al = umma_desc(sbase + TcPlan::A1L, 128, 256);
-            const uint64_t bh = umma_desc(sbase + TcPlan::W1H, 128, 256), bl = umma_desc(sbase + TcPlan::W1L, 128, 256);
-            umma_tf32(tmem, al, bh, idesc, 0u);
-            umma_tf32(tmem, ah, bl, idesc, 1u);
-            umma_tf32(tmem, ah, bh, idesc, 1u);
-            asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-        }
-        mbar_wait(bar, phase); phase ^= 1u;
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        float hv[32];
-        tmem_ld32(trow, hv);
-        tmem_wait_ld();
-
-        // ---- bias + ReLU, layer 2 ------------------------------------------------------------------------------
+        float d[2][16];
+        wgmma_fence();
         {
-            const int off = rg * 1024 + r0 * 16;
+            const uint64_t bh = wgmma_desc(sbase + TcPlan::W1H, 128, 256), bl = wgmma_desc(sbase + TcPlan::W1L, 128, 256);
 #pragma unroll
-            for (int c = 0; c < 8; ++c) {
-                const float4 bb = *reinterpret_cast<const float4*>(vec + 4 * c);
-                uint32_t h0, h1, h2, h3, l0, l1, l2, l3;
-                split_fast(fmaxf(hv[4 * c + 0] + bb.x, 0.f), h0, l0); split_fast(fmaxf(hv[4 * c + 1] + bb.y, 0.f), h1, l1);
-                split_fast(fmaxf(hv[4 * c + 2] + bb.z, 0.f), h2, l2); split_fast(fmaxf(hv[4 * c + 3] + bb.w, 0.f), h3, l3);
-                *reinterpret_cast<uint4*>(tsm + TcPlan::A2H + off + 128 * c) = make_uint4(h0, h1, h2, h3);
-                *reinterpret_cast<uint4*>(tsm + TcPlan::A2L + off + 128 * c) = make_uint4(l0, l1, l2, l3);
+            for (int h = 0; h < 2; ++h) {
+                const uint64_t ah = wgmma_desc(sbase + TcPlan::A1H + 2048 * h, 128, 256);
+                const uint64_t al = wgmma_desc(sbase + TcPlan::A1L + 2048 * h, 128, 256);
+                wgmma_n32(d[h], al, bh, 0u);
+                wgmma_n32(d[h], ah, bl, 1u);
+                wgmma_n32(d[h], ah, bh, 1u);
+            }
+        }
+        wgmma_commit();
+        wgmma_wait_all();
+        __syncthreads();                                   // every warp's MMAs are done with X before H1 overwrites it
+
+        // ---- bias + ReLU -> H1 (hi/lo), layer 2 ----------------------------------------------------------------------
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+#pragma unroll
+            for (int rr = 0; rr < 2; ++rr) {
+                const int row = 64 * h + 16 * warp + g + 8 * rr;
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const int col = 8 * j + 2 * t;
+                    uint32_t h0, h1, l0, l1;
+                    split_fast(fmaxf(d[h][4 * j + 2 * rr] + vec[col], 0.f), h0, l0);
+                    split_fast(fmaxf(d[h][4 * j + 2 * rr + 1] + vec[col + 1], 0.f), h1, l1);
+                    const int off = (row >> 3) * 1024 + (col >> 2) * 128 + (row & 7) * 16 + (col & 3) * 4;
+                    *reinterpret_cast<uint2*>(tsm + TcPlan::A2H + off) = make_uint2(h0, h1);
+                    *reinterpret_cast<uint2*>(tsm + TcPlan::A2L + off) = make_uint2(l0, l1);
+                }
             }
         }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
         __syncthreads();
-        if (tid == 0) {
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+        wgmma_fence();
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
 #pragma unroll
             for (int kk = 0; kk < 4; ++kk) {
-                const uint64_t ah = umma_desc(sbase + TcPlan::A2H + 256 * kk, 128, 1024), al = umma_desc(sbase + TcPlan::A2L + 256 * kk, 128, 1024);
-                const uint64_t bh = umma_desc(sbase + TcPlan::W2H + 256 * kk, 128, 1024), bl = umma_desc(sbase + TcPlan::W2L + 256 * kk, 128, 1024);
-                umma_tf32(tmem + 32, al, bh, idesc, kk > 0 ? 1u : 0u);
-                umma_tf32(tmem + 32, ah, bl, idesc, 1u);
-                umma_tf32(tmem + 32, ah, bh, idesc, 1u);
+                const uint64_t ah = wgmma_desc(sbase + TcPlan::A2H + 8192 * h + 256 * kk, 128, 1024);
+                const uint64_t al = wgmma_desc(sbase + TcPlan::A2L + 8192 * h + 256 * kk, 128, 1024);
+                const uint64_t bh = wgmma_desc(sbase + TcPlan::W2H + 256 * kk, 128, 1024);
+                const uint64_t bl = wgmma_desc(sbase + TcPlan::W2L + 256 * kk, 128, 1024);
+                wgmma_n32(d[h], al, bh, kk > 0 ? 1u : 0u);
+                wgmma_n32(d[h], ah, bl, 1u);
+                wgmma_n32(d[h], ah, bh, 1u);
             }
-            asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
         }
-        mbar_wait(bar, phase); phase ^= 1u;
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        tmem_ld32(trow + 32, hv);
-        tmem_wait_ld();
+        wgmma_commit();
+        wgmma_wait_all();
 
-        // ---- bias + ReLU + 32 -> 1 output layer ----------------------------------------------------------------------
-        float pr = vec[96];
+        // ---- bias + ReLU + 32 -> 1 output layer: 8 columns per lane, the row's sum over the lane quad -----------------
 #pragma unroll
-        for (int c = 0; c < 8; ++c) {
-            const float4 bb = *reinterpret_cast<const float4*>(vec + 32 + 4 * c);
-            const float4 ww = *reinterpret_cast<const float4*>(vec + 64 + 4 * c);
-            pr = fmaf(fmaxf(hv[4 * c + 0] + bb.x, 0.f), ww.x, pr); pr = fmaf(fmaxf(hv[4 * c + 1] + bb.y, 0.f), ww.y, pr);
-            pr = fmaf(fmaxf(hv[4 * c + 2] + bb.z, 0.f), ww.z, pr); pr = fmaf(fmaxf(hv[4 * c + 3] + bb.w, 0.f), ww.w, pr);
+        for (int h = 0; h < 2; ++h) {
+#pragma unroll
+            for (int rr = 0; rr < 2; ++rr) {
+                float pr = 0.f;
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const int col = 8 * j + 2 * t;
+                    pr = fmaf(fmaxf(d[h][4 * j + 2 * rr] + vec[32 + col], 0.f), vec[64 + col], pr);
+                    pr = fmaf(fmaxf(d[h][4 * j + 2 * rr + 1] + vec[33 + col], 0.f), vec[65 + col], pr);
+                }
+                pr += __shfl_xor_sync(kFull, pr, 1);
+                pr += __shfl_xor_sync(kFull, pr, 2);
+                const int64_t p = (int64_t)tile * 128 + 64 * h + 16 * warp + g + 8 * rr;
+                if (t == 0 && p < P.n) P.pred[p] = pr + vec[96];
+            }
         }
-        if (valid) P.pred[p] = pr;
-    }
-
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 0) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 64;" ::"r"(tmem) : "memory");
+        __syncthreads();                                   // H1 has been read by every warp's MMAs before the next gather
     }
 }
 
@@ -1708,7 +1624,6 @@ int launch_infer_tc_t(const StepParams& P, cudaStream_t st) {
         const int by_regs = fa.numRegs > 0 ? 65536 / (fa.numRegs * 128) : 1;
         const int by_smem = (227 * 1024) / (TcPlan::BYTES + 1024);
         int q = by_regs < by_smem ? by_regs : by_smem;
-        if (q > 8) q = 8;                      // 8 x 64 TMEM columns = all 512
         per_sm_cached = q < 1 ? 1 : q;
     }
     const int tiles = (int)((P.n + 127) / 128);
@@ -1784,7 +1699,7 @@ int shine_abi_version(void) { return SHINE_ABI_VERSION; }
 const char* shine_error_string(int code) {
     if (code == SHINE_OK) return "ok";
     if (code == SHINE_ERR_INVALID_ARG) return "shine_b200: invalid argument";
-    if (code == SHINE_ERR_UNSUPPORTED) return "shine_b200: unsupported configuration for the sm_100a kernels";
+    if (code == SHINE_ERR_UNSUPPORTED) return "shine_b200: unsupported configuration for the sm_90a kernels";
     if (code > 0) return cudaGetErrorString((cudaError_t)code);
     return "shine_b200: unknown error";
 }

@@ -160,11 +160,11 @@ struct BlendD {   // weights of model/feature_octree.py:186-193 and their deriva
 __device__ __forceinline__ float4 ldg_f4(const float* p) {
     return __ldg(reinterpret_cast<const float4*>(p));
 }
-// one instruction per full 32-byte feature row (sm_100a LDG.E.ENL2.256)
+// a full 32-byte feature row as two 16-byte non-coherent loads (the widest global load of sm_90a); the pair lands in
+// one sector
 __device__ __forceinline__ void ldg_row8(const float* p, float (&v)[8]) {
-    asm volatile("ld.global.nc.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]), "=f"(v[4]), "=f"(v[5]), "=f"(v[6]), "=f"(v[7])
-                 : "l"(p));
+    asm volatile("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]) : "l"(p));
+    asm volatile("ld.global.nc.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v[4]), "=f"(v[5]), "=f"(v[6]), "=f"(v[7]) : "l"(p + 4));
 }
 __device__ __forceinline__ int4 ldg_i4(const int32_t* p) {
     return __ldg(reinterpret_cast<const int4*>(p));
@@ -227,9 +227,9 @@ struct SlotSector { unsigned long long key; int32_t maxdisp; int32_t ids[4]; };
 __device__ __forceinline__ SlotSector ldg_sector(const HashSlot* slots, uint32_t s, int half) {
     uint32_t w[8];
     const void* p = reinterpret_cast<const char*>(slots + s) + 32 * half;
-    asm volatile("ld.global.nc.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]), "=r"(w[4]), "=r"(w[5]), "=r"(w[6]), "=r"(w[7])
-                 : "l"(p));
+    asm volatile("ld.global.nc.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]) : "l"(p));
+    asm volatile("ld.global.nc.v4.b32 {%0,%1,%2,%3}, [%4];"
+                 : "=r"(w[4]), "=r"(w[5]), "=r"(w[6]), "=r"(w[7]) : "l"(reinterpret_cast<const char*>(p) + 16));
     SlotSector r;
     r.key = ((unsigned long long)w[1] << 32) | w[0];
     r.maxdisp = (int32_t)w[3];
@@ -284,16 +284,16 @@ __device__ __forceinline__ void split_fast(float x, uint32_t& hi, uint32_t& lo) 
     hi = __float_as_uint(x) & g_tf32_mask;
     lo = __float_as_uint(x - __uint_as_float(hi));
 }
-// Packed fp32 pairs (sm_100a FFMA2 / FMUL2 / FADD2: two IEEE fp32 operations per lane per instruction; a scalar
-// operand broadcasts for free).  Same rounding as the scalar forms: results are bit-identical, the instruction count halves.
-typedef unsigned long long f2_t;
-__device__ __forceinline__ f2_t f2_pack(float a, float b) { f2_t r; asm("mov.b64 %0, {%1,%2};" : "=l"(r) : "f"(a), "f"(b)); return r; }
-__device__ __forceinline__ void f2_unpack(f2_t r, float& a, float& b) { asm("mov.b64 {%0,%1}, %2;" : "=f"(a), "=f"(b) : "l"(r)); }
-__device__ __forceinline__ f2_t f2_fma(f2_t a, f2_t b, f2_t c) { f2_t d; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c)); return d; }
-__device__ __forceinline__ f2_t f2_mul(f2_t a, f2_t b) { f2_t d; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
-__device__ __forceinline__ f2_t f2_add(f2_t a, f2_t b) { f2_t d; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
-__device__ __forceinline__ f2_t f2_sub(f2_t a, f2_t b) { f2_t d; asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
-// split_fast of two values: 2 LOP3 + 1 FADD2
+// fp32 pairs.  Every operation rounds once, like its scalar form (the _rn intrinsics keep the compiler from contracting
+// a multiply and an add into one FMA), so the results are those of the element-wise scalar code.
+typedef float2 f2_t;
+__device__ __forceinline__ f2_t f2_pack(float a, float b) { return make_float2(a, b); }
+__device__ __forceinline__ void f2_unpack(f2_t r, float& a, float& b) { a = r.x; b = r.y; }
+__device__ __forceinline__ f2_t f2_fma(f2_t a, f2_t b, f2_t c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
+__device__ __forceinline__ f2_t f2_mul(f2_t a, f2_t b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ f2_t f2_add(f2_t a, f2_t b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ f2_t f2_sub(f2_t a, f2_t b) { return make_float2(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y)); }
+// split_fast of two values
 __device__ __forceinline__ void split_fast2(float a, float b, uint32_t& ha, uint32_t& hb, uint32_t& la, uint32_t& lb) {
     ha = __float_as_uint(a) & g_tf32_mask; hb = __float_as_uint(b) & g_tf32_mask;
     float x, y;
@@ -330,7 +330,7 @@ __device__ __forceinline__ void mma3(float (&d)[4], const AFrag<NTF>& a, uint2 b
     mma_tf32(d, a.hi, bh.x, bh.y);
 }
 
-// acc[q] = fma(w3, r3[q], fma(w2, r2[q], fma(w1, r1[q], fma(w0, r0[q], acc[q])))) for the 8 channels, two per FFMA2
+// acc[q] = fma(w3, r3[q], fma(w2, r2[q], fma(w1, r1[q], fma(w0, r0[q], acc[q])))) for the 8 channels
 __device__ __forceinline__ void blend4(float (&acc)[8], const float (&r0)[8], const float (&r1)[8], const float (&r2)[8],
                                        const float (&r3)[8], float w0, float w1, float w2, float w3) {
     const f2_t p0 = f2_pack(w0, w0), p1 = f2_pack(w1, w1), p2 = f2_pack(w2, w2), p3 = f2_pack(w3, w3);
@@ -368,47 +368,35 @@ __device__ __forceinline__ void mma3x2(float (&d0)[4], float (&d1)[4], const AFr
 }
 
 // ------------------------------------------------------------------------------------------------------
-// Tensor Memory load / store (tcgen05.ld / tcgen05.st -> SASS LDTM / STTM), 32 lanes x 32-bit columns per warp
+// wgmma (sm_90a warpgroup MMA, kind tf32, fp32 accumulate) with shared-memory descriptors, mbarrier wait
 // ------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-                 : "=f"(v[0]),"=f"(v[1]),"=f"(v[2]),"=f"(v[3]),"=f"(v[4]),"=f"(v[5]),"=f"(v[6]),"=f"(v[7]),"=f"(v[8]),"=f"(v[9]),"=f"(v[10]),"=f"(v[11]),"=f"(v[12]),"=f"(v[13]),"=f"(v[14]),"=f"(v[15]),"=f"(v[16]),"=f"(v[17]),"=f"(v[18]),"=f"(v[19]),"=f"(v[20]),"=f"(v[21]),"=f"(v[22]),"=f"(v[23]),"=f"(v[24]),"=f"(v[25]),"=f"(v[26]),"=f"(v[27]),"=f"(v[28]),"=f"(v[29]),"=f"(v[30]),"=f"(v[31]) : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                 : "=f"(v[0]),"=f"(v[1]),"=f"(v[2]),"=f"(v[3]),"=f"(v[4]),"=f"(v[5]),"=f"(v[6]),"=f"(v[7]),"=f"(v[8]),"=f"(v[9]),"=f"(v[10]),"=f"(v[11]),"=f"(v[12]),"=f"(v[13]),"=f"(v[14]),"=f"(v[15]) : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float* v) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=f"(v[0]),"=f"(v[1]),"=f"(v[2]),"=f"(v[3]),"=f"(v[4]),"=f"(v[5]),"=f"(v[6]),"=f"(v[7]) : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const float* v) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};"
-                 :: "r"(taddr), "f"(v[0]),"f"(v[1]),"f"(v[2]),"f"(v[3]),"f"(v[4]),"f"(v[5]),"f"(v[6]),"f"(v[7]),"f"(v[8]),"f"(v[9]),"f"(v[10]),"f"(v[11]),"f"(v[12]),"f"(v[13]),"f"(v[14]),"f"(v[15]),"f"(v[16]),"f"(v[17]),"f"(v[18]),"f"(v[19]),"f"(v[20]),"f"(v[21]),"f"(v[22]),"f"(v[23]),"f"(v[24]),"f"(v[25]),"f"(v[26]),"f"(v[27]),"f"(v[28]),"f"(v[29]),"f"(v[30]),"f"(v[31]) : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const float* v) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};"
-                 :: "r"(taddr), "f"(v[0]),"f"(v[1]),"f"(v[2]),"f"(v[3]),"f"(v[4]),"f"(v[5]),"f"(v[6]),"f"(v[7]),"f"(v[8]),"f"(v[9]),"f"(v[10]),"f"(v[11]),"f"(v[12]),"f"(v[13]),"f"(v[14]),"f"(v[15]) : "memory");
-}
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const float* v) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};"
-                 :: "r"(taddr), "f"(v[0]),"f"(v[1]),"f"(v[2]),"f"(v[3]),"f"(v[4]),"f"(v[5]),"f"(v[6]),"f"(v[7]) : "memory");
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// ------------------------------------------------------------------------------------------------------
-// tcgen05.mma (kind::tf32) with shared-memory descriptors, mbarrier wait
-// ------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint64_t umma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+// Operand layout: K-major without swizzle, core matrices of 8 rows x 16 bytes; LBO = byte distance of the two core
+// matrices that make up the K = 8 of one instruction, SBO = byte distance of consecutive 8-row groups.
+__device__ __forceinline__ uint64_t wgmma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     return (uint64_t)((smem_addr >> 4) & 0x3FFF) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) |
-           ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32) | (1ull << 46);      // version 1 (Blackwell), SWIZZLE_NONE
+           ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32);                     // base offset 0, no swizzle
 }
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t a, uint64_t b, uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// D[64 x 32] (+)= A[64 x 8] B[32 x 8]^T.  Accumulator fragment of thread (warp w, lane l) of the warpgroup: d[4j + r] is row
+// 16w + l/4 + 8(r >> 1), column 8j + 2(l % 4) + (r & 1) — four m16n8 C fragments side by side.
+__device__ __forceinline__ void wgmma_n32(float (&d)[16], uint64_t a, uint64_t b, uint32_t accumulate) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, {%5, %5, %5, %5}, p;\n\t}\n"
-        ::"r"(d_tmem), "l"(a), "l"(b), "r"(idesc), "r"(accumulate), "r"(0u) : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(a), "l"(b), "r"(accumulate));
+}
+// D[64 x 8] (+)= A[64 x 8] B[8 x 8]^T (one m16n8 C fragment per warp)
+__device__ __forceinline__ void wgmma_n8(float (&d)[4], uint64_t a, uint64_t b, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %6, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n8k8.f32.tf32.tf32 {%0,%1,%2,%3}, %4, %5, p, 1, 1;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+        : "l"(a), "l"(b), "r"(accumulate));
 }
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     uint32_t done = 0;
@@ -467,7 +455,7 @@ inline int sm_count() {
     const int dev = current_device();
     if (cached[dev] == 0) {
         int n = 0;
-        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
         cached[dev] = n;
     }
     return cached[dev];

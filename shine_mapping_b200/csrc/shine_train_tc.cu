@@ -1,28 +1,28 @@
-// shine_train_tc.cu — the training step with the decoder on the 5th-generation tensor cores (tcgen05.mma, accumulators
-// in Tensor Memory), warp-specialised.  Same contract as sdf_fused_kernel<TRAIN> (reference shine_batch.py:123-209);
-// selected with SHINE_FLAG_TCGEN05 on shine_sdf_bce_step.
+// shine_train_tc.cu — the training step with the decoder on the warpgroup tensor-core instructions (wgmma, sm_90a),
+// warp-specialised.  Same contract as sdf_fused_kernel<TRAIN> (reference shine_batch.py:123-209); selected with
+// SHINE_FLAG_TCGEN05 on shine_sdf_bce_step.
 //
 // Why: in the mma.sync kernel every warp re-reads the decoder weights and stages the weight-gradient operands through
-// the LSU for each 16-point tile, and its time tracks its instruction count (ncu: 115 M warp instructions, 0.39 IPC per
-// scheduler whatever the variant).  Here the 2 lanes-per-point gather / scatter warps do nothing but gather and scatter,
-// and the decoder runs as 128-point tcgen05 tiles whose operands the tensor core reads from shared memory itself.
+// the LSU for each 16-point tile.  Here the 2 lanes-per-point gather / scatter warps do nothing but gather and scatter,
+// and the decoder runs as 128-point wgmma tiles whose operands the tensor core reads from shared memory itself.
 //
 // One CTA per SM, 20 warps:
 //   warps 0-15  gather/scatter (GS), two groups of 8.  Group g owns the rounds r = g, g+2, ... of this CTA; a round is a
 //               tile of 128 points, warp w of the group owns rows 16w..16w+15 (lane layout of the mma.sync kernel:
-//               2 lanes per point, z-split corners, LDG.256 rows).  Per round: hash walk + gather + blend -> X rows
-//               (hi/lo tf32) into the round's operand buffer, corner rows + blend factors parked in TMEM, arrive on
-//               x_full; later wait dx_full, read dL/dfeature rows, scatter-add (red.v4) into the tables.
-//   warps 16-19 decoder epilogue (EP), one thread per row of the tile; thread 0 also issues the MMAs.  Per round:
+//               2 lanes per point, z-split corners, 32-byte rows).  Per round: hash walk + gather + blend -> X rows
+//               (hi/lo tf32) into the round's operand buffer, arrive on x_full; later wait dx_full, read dL/dfeature
+//               rows, walk the hash again (the slots are L2-resident by then) and scatter-add (red.v4) into the tables.
+//   warps 16-19 decoder epilogue (EP), one warpgroup; it issues the MMAs (two m64 halves per 128-row tile) and after
+//               each one stages the accumulators through shared memory so that thread i works on row i of the tile:
 //               D1 = X W1^T            -> +b1, ReLU (mask kept), H1 hi/lo -> smem
 //               D2 = H1 W2^T           -> +b2, ReLU, pred, BCE loss, dL/dpred, dH2 hi/lo -> smem, dW3/db3 in registers
 //               D3 = dH2 W2            -> ReLU mask, dH1 hi/lo -> smem
-//               D4 = dH1 W1 (tensor core)  ||  dW2 += dH2^T H1, dW1 += dH1^T X, bias sums: mma.sync by the four warps,
-//                                              fragments read straight from the operand tiles (tcgen05 has no unswizzled
-//                                              MN-major layout for tf32: profiles/r02_umma_mn_major_probe.txt)
+//               D4 = dH1 W1 (wgmma, in flight)  ||  dW2 += dH2^T H1, dW1 += dH1^T X, bias sums: mma.sync by the four
+//                                                   warps, fragments read straight from the operand tiles (tf32 wgmma
+//                                                   operands must be K-major)
 //               D4 -> dX rows -> smem, arrive dx_full.
-//   The gather warps run one round ahead per group (4 X / dX slots, 2 TMEM parking sets per warp), so they only wait for
-//   the decoder when it is the bottleneck.  All contractions are 3xTF32 (hi*hi + lo*hi + hi*lo, fp32 accumulate).
+//   The gather warps run one round ahead per group (4 X / dX slots), so they only wait for the decoder when it is the
+//   bottleneck.  All contractions are 3xTF32 (hi*hi + lo*hi + hi*lo, fp32 accumulate).
 //
 // Shared-memory operand layout (no swizzle): an activation matrix [128 points][C columns] is stored as core matrices of
 // 8 points x 16 bytes (4 columns): offset(pt, c) = (pt>>3)*S_pt + (c>>2)*128 + (pt&7)*16 + (c&3)*4 — the canonical
@@ -37,6 +37,7 @@ constexpr int kGSWarps = 16, kEPWarps = 4;
 constexpr int kTcThreads = 32 * (kGSWarps + kEPWarps);     // 640
 constexpr int kRound = 128;                                 // points per round (MMA M)
 constexpr int kGSRegs = 80, kEPRegs = 160;                  // setmaxnreg: 512 x 80 + 128 x 160 = 640 x 96
+constexpr int kRowStride = 36;                              // floats per row of the accumulator staging tile
 
 struct TP {                                               // byte offsets in dynamic shared memory
     static constexpr int X_PT = 2 * 128;                  // X tile [128][8]: 2 chunks per 8-point group
@@ -59,15 +60,11 @@ struct TP {                                               // byte offsets in dyn
     static constexpr int VEC = W1TL + 2048;               // b1[32] b2[32] w3[32] b3 + pad            400 B
     static constexpr int DX = VEC + 400;                  // [slot 4][128][8] fp32                    16 384 B
     static constexpr int RED = DX + 16384;                // decoder-gradient block accumulator [1380] 5 520 B
-    static constexpr int BAR = RED + 5520;                // x_full[4], dx_full[4], mma_done : 9 x 8 B; tmem base 4 B
-    static constexpr int BYTES = BAR + 80;
+    static constexpr int ACC = RED + 5520;                // accumulator staging [128][kRowStride] fp32          18 432 B
+    static constexpr int BAR = ACC + 128 * kRowStride * 4; // x_full[4], dx_full[4] : 8 x 8 B
+    static constexpr int BYTES = BAR + 64;
 };
-static_assert(TP::DX % 16 == 0 && TP::BAR % 8 == 0 && TP::RED % 16 == 0, "alignment");
-
-// instruction descriptor (kind::tf32, fp32 accumulate, K-major A and B): N >> 3 at bit 17, M >> 4 at bit 24
-__host__ __device__ constexpr uint32_t tc_idesc(int n) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(kRound >> 4) << 24);
-}
+static_assert(TP::DX % 16 == 0 && TP::BAR % 8 == 0 && TP::RED % 16 == 0 && TP::ACC % 16 == 0, "alignment");
 
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
@@ -75,23 +72,50 @@ __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
     asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.shared::cta.b64 st, [%0];\n\t}" ::"r"(bar) : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
 __device__ __forceinline__ void ep_bar() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
 
-// 3xTF32 product D = A B over `ksteps` K = 8 steps (each step = 2 chunks = 256 B further in both operands); the
-// descriptors are built once and only their address field is advanced
-__device__ __forceinline__ void mma3x(uint32_t d, uint64_t ah, uint64_t al, uint64_t bh, uint64_t bl, int ksteps,
-                                      uint32_t idesc) {
-    uint32_t acc = 0u;
-#pragma unroll 1
-    for (int k = 0; k < ksteps; ++k) {
-        umma_tf32(d, al, bh, idesc, acc);
-        umma_tf32(d, ah, bl, idesc, 1u);
-        umma_tf32(d, ah, bh, idesc, 1u);
-        acc = 1u;
-        ah += 16; al += 16; bh += 16; bl += 16;            // 256 B >> 4 in the start-address field
+// 3xTF32 product D = A B of the 128-row tile over KS K = 8 steps (each step = 2 chunks = 256 B further in both
+// operands), as two m64 halves (A advanced by 8 row groups = a_half bytes); the descriptors are built once and only
+// their address field is advanced.  The MMAs are committed, not waited for.
+template <int KS, int NR>
+__device__ __forceinline__ void mma3x_issue(float (&d)[2][NR], uint64_t ah, uint64_t al, uint64_t bh, uint64_t bl,
+                                            uint32_t a_half) {
+    wgmma_fence();
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const uint64_t ho = (uint64_t)((h * a_half) >> 4);
+#pragma unroll
+        for (int k = 0; k < KS; ++k) {
+            const uint64_t ko = (uint64_t)(16 * k);      // 256 B >> 4 in the start-address field
+            if constexpr (NR == 16) {
+                wgmma_n32(d[h], al + ho + ko, bh + ko, k > 0 ? 1u : 0u);
+                wgmma_n32(d[h], ah + ho + ko, bl + ko, 1u);
+                wgmma_n32(d[h], ah + ho + ko, bh + ko, 1u);
+            } else {
+                wgmma_n8(d[h], al + ho + ko, bh + ko, k > 0 ? 1u : 0u);
+                wgmma_n8(d[h], ah + ho + ko, bl + ko, 1u);
+                wgmma_n8(d[h], ah + ho + ko, bh + ko, 1u);
+            }
+        }
+    }
+    wgmma_commit();
+}
+
+// accumulator fragments of the EP warpgroup -> staging tile [row][kRowStride] (columns 8j + 2t, +1 of rows g, g + 8 of
+// every 16-row slice); the caller synchronises the warpgroup before reading rows back
+template <int NR>
+__device__ __forceinline__ void stage_acc(float* acc, const float (&d)[2][NR], int eq, int lane) {
+    const int g = lane >> 2, t = lane & 3;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int j = 0; j < NR / 4; ++j) {
+#pragma unroll
+            for (int rr = 0; rr < 2; ++rr) {
+                const int row = 64 * h + 16 * eq + g + 8 * rr;
+                *reinterpret_cast<float2*>(acc + row * kRowStride + 8 * j + 2 * t) = make_float2(d[h][4 * j + 2 * rr], d[h][4 * j + 2 * rr + 1]);
+            }
+        }
     }
 }
 
@@ -101,10 +125,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) sdf_train_tc_kernel(const __gri
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const uint32_t sbase = (uint32_t)__cvta_generic_to_shared(sm);
     float* vec = reinterpret_cast<float*>(sm + TP::VEC);
-    const uint32_t bar_x = sbase + TP::BAR, bar_dx = sbase + TP::BAR + 32, bar_mma = sbase + TP::BAR + 64;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(sm + TP::BAR + 72);
+    const uint32_t bar_x = sbase + TP::BAR, bar_dx = sbase + TP::BAR + 32;
+    float* accs = reinterpret_cast<float*>(sm + TP::ACC);
 
-    // ---- prologue: weights in UMMA layouts (hi/lo), barriers, TMEM ------------------------------------------------------
+    // ---- prologue: weights in the K-major operand layouts (hi/lo), barriers ------------------------------------------
     for (int i = tid; i < 2048 / 4; i += kTcThreads) {             // W1^T rows 8..15 must be zero
         reinterpret_cast<uint32_t*>(sm + TP::W1TH)[i] = 0u; reinterpret_cast<uint32_t*>(sm + TP::W1TL)[i] = 0u;
     }
@@ -134,20 +158,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) sdf_train_tc_kernel(const __gri
     if (tid == 0) {
         vec[96] = P.dec.b3 ? P.dec.b3[0] : 0.f;
         for (int s = 0; s < 4; ++s) { mbar_init(bar_x + 8 * s, 8); mbar_init(bar_dx + 8 * s, 1); }
-        mbar_init(bar_mma, 1);                                   // tcgen05.commit
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == kGSWarps) {       // the first epilogue warp allocates TMEM (this CTA owns the SM: all 512 columns)
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(sbase + TP::BAR + 72) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem = *tmem_slot;
-    // TMEM columns: D1/D3 0..31 | D2 32..63 | D4 64..79 | gather-warp parking 128..383 (4 warps per lane quadrant x 2 sets x 32)
-    constexpr uint32_t cD1 = 0, cD2 = 32, cD4 = 64, cPark = 128;
 
     const int64_t tiles_total = (P.n + kRound - 1) / kRound;
     const int rounds = (int)((tiles_total > blockIdx.x) ? (tiles_total - blockIdx.x + gridDim.x - 1) / gridDim.x : 0);
@@ -160,7 +174,6 @@ __global__ void __launch_bounds__(kTcThreads, 1) sdf_train_tc_kernel(const __gri
         const int grp = warp >> 3, wg = warp & 7;
         const int g = lane >> 2, t = lane & 3, odd = t & 1, half = t >> 1;
         const int row = 16 * wg + g + 8 * odd;                                   // this lane pair's row of the tile
-        const uint32_t tpark0 = tmem + ((uint32_t)(32 * (warp & 3)) << 16) + cPark + 64u * (uint32_t)(warp >> 2);
         const bool poly = P.oct.poly_interp != 0;
         const int L = P.oct.num_levels;
         bool consecutive = true;
@@ -169,14 +182,13 @@ __global__ void __launch_bounds__(kTcThreads, 1) sdf_train_tc_kernel(const __gri
             if (i < L && P.oct.lv[i].level != P.oct.lv[0].level - i) consecutive = false;
         const int xoff = (row >> 3) * TP::X_PT + half * 128 + (row & 7) * 16;
 
-        // gather of one round: hash walk, 8-corner blend, X rows -> slot, corner rows + blend factors -> TMEM set
-        auto gather = [&](int r, int slot, uint32_t tpark) {
+        // this lane pair's point of round r and its node slot on every level (-1: miss)
+        auto locate = [&](int r, float& x, float& y, float& z, int (&slotl)[4]) {
             const int64_t myp = ((int64_t)blockIdx.x + (int64_t)r * gridDim.x) * kRound + row;
             const bool valid = myp < P.n;
-            float x = 0.f, y = 0.f, z = 0.f;
+            x = 0.f; y = 0.f; z = 0.f;
             if (valid) { x = __ldg(P.coord + 3 * myp); y = __ldg(P.coord + 3 * myp + 1); z = __ldg(P.coord + 3 * myp + 2); }
             // hash walk (model/feature_octree.py:199-218): the pair splits the LEVELS for the first probe
-            int slotl[4];
             {
                 const unsigned long long key0 = valid ? morton_of(x, y, z, P.oct.lv[0].level) : 0ull;
                 unsigned long long kq[2];
@@ -216,32 +228,32 @@ __global__ void __launch_bounds__(kTcThreads, 1) sdf_train_tc_kernel(const __gri
                     slotl[2 * j + 1] = half ? mine[j] : other;
                 }
             }
+        };
+
+        // gather of one round: hash walk, 8-corner blend, X rows -> slot
+        auto gather = [&](int r, int slot) {
+            float x, y, z;
+            int slotl[4];
+            locate(r, x, y, z, slotl);
             // 8-corner gather + blend (model/feature_octree.py:222-234): the pair splits the CORNERS by z bit
-            float pk[16], idp[16];
             float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-            for (int i = 0; i < 16; ++i) { pk[i] = 0.f; idp[i] = __int_as_float(-1); }
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
                 if (i < L && slotl[i] >= 0) {
                     const shine_level& lv = P.oct.lv[i];
                     const int4 id4 = ldg_i4(slot_ids(reinterpret_cast<const HashSlot*>(lv.hash_slots), slotl[i], half));
-                    idp[4 * i] = __int_as_float(id4.x); idp[4 * i + 1] = __int_as_float(id4.y);
-                    idp[4 * i + 2] = __int_as_float(id4.z); idp[4 * i + 3] = __int_as_float(id4.w);
                     float r0[8], r1[8], r2[8], r3[8];
                     ldg_row8(lv.features + (int64_t)id4.x * kF, r0);
                     ldg_row8(lv.features + (int64_t)id4.y * kF, r1);
                     ldg_row8(lv.features + (int64_t)id4.z * kF, r2);
                     ldg_row8(lv.features + (int64_t)id4.w * kF, r3);
                     Blend b; b.init(x, y, z, lv.level, poly);
-                    pk[3 * i] = b.tx; pk[3 * i + 1] = b.ty; pk[3 * i + 2] = b.tz;
                     const float wz = half ? b.tz : b.uz;
                     const float w0 = __fmul_rn(__fmul_rn(b.ux, b.uy), wz), w1 = __fmul_rn(__fmul_rn(b.ux, b.ty), wz);
                     const float w2 = __fmul_rn(__fmul_rn(b.tx, b.uy), wz), w3 = __fmul_rn(__fmul_rn(b.tx, b.ty), wz);
                     blend4(acc, r0, r1, r2, r3, w0, w1, w2, w3);
                 }
             }
-            tmem_st16(tpark, pk); tmem_st16(tpark + 16, idp);
             // X rows (this lane: the 4 channels of its half = one 16-byte K chunk), hi / lo
             uint32_t h4[4], l4[4];
 #pragma unroll
@@ -253,40 +265,40 @@ __global__ void __launch_bounds__(kTcThreads, 1) sdf_train_tc_kernel(const __gri
             unsigned char* xs = sm + TP::X + (2 * slot) * TP::X_BYTES;
             *reinterpret_cast<uint4*>(xs + xoff) = make_uint4(h4[0], h4[1], h4[2], h4[3]);
             *reinterpret_cast<uint4*>(xs + TP::X_BYTES + xoff) = make_uint4(l4[0], l4[1], l4[2], l4[3]);
-            tmem_wait_st();
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
             __syncwarp();
             if (lane == 0) mbar_arrive(bar_x + 8 * slot);
         };
 
         // software pipeline, depth 2 per group: the gather of local round k+1 is issued before waiting for the decoder of k
-        if (grp < rounds) gather(grp, grp, tpark0);
+        if (grp < rounds) gather(grp, grp);
         for (int r = grp, k = 0; r < rounds; r += 2, ++k) {
             const int slot = 2 * (k & 1) + grp;
-            const uint32_t tpark = tpark0 + 32u * (uint32_t)(k & 1);
-            if (r + 2 < rounds) gather(r + 2, 2 * ((k + 1) & 1) + grp, tpark0 + 32u * (uint32_t)((k + 1) & 1));
+            if (r + 2 < rounds) gather(r + 2, 2 * ((k + 1) & 1) + grp);
             // ---- dL/dfeature of round r, then scatter-add (index_put_ accumulate) ------------------------------------------
             mbar_wait(bar_dx + 8 * slot, (uint32_t)((k >> 1) & 1));
             const float4 dxv = *reinterpret_cast<const float4*>(sm + TP::DX + slot * 4096 + row * 32 + 16 * half);
             const float dx[4] = {dxv.x, dxv.y, dxv.z, dxv.w};
-            float qk[16], qid[16];
-            tmem_ld16(tpark, qk); tmem_ld16(tpark + 16, qid);
-            tmem_wait_ld();
+            float x, y, z;
+            int slotl[4];
+            locate(r, x, y, z, slotl);
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
+                int4 id4 = make_int4(-1, -1, -1, -1);
+                if (i < L && slotl[i] >= 0)
+                    id4 = ldg_i4(slot_ids(reinterpret_cast<const HashSlot*>(P.oct.lv[i].hash_slots), slotl[i], half));
+                const int qid[4] = {id4.x, id4.y, id4.z, id4.w};
                 int ids[8];
 #pragma unroll
                 for (int c = 0; c < 4; ++c) {
-                    const int mine = __float_as_int(qid[4 * i + c]);
+                    const int mine = qid[c];
                     const int other = __shfl_xor_sync(kFull, mine, 2);
                     ids[2 * c] = half ? other : mine;
                     ids[2 * c + 1] = half ? mine : other;
                 }
                 if (i < L && ids[0] >= 0) {
                     const shine_level& lv = P.oct.lv[i];
-                    Blend b;
-                    b.tx = qk[3 * i]; b.ty = qk[3 * i + 1]; b.tz = qk[3 * i + 2];
-                    b.ux = __fsub_rn(1.0f, b.tx); b.uy = __fsub_rn(1.0f, b.ty); b.uz = __fsub_rn(1.0f, b.tz);
+                    Blend b; b.init(x, y, z, lv.level, poly);
                     float* gb = grad_base(lv, (uint32_t)(blockIdx.x * kGSWarps + warp + r), kF) + 4 * half;
                     // w_c = (X * Y) * Z in the reference's association; the four X*Y products are shared by the z pair
                     const float xy[4] = {__fmul_rn(b.ux, b.uy), __fmul_rn(b.ux, b.ty), __fmul_rn(b.tx, b.uy), __fmul_rn(b.tx, b.ty)};
@@ -303,19 +315,17 @@ __global__ void __launch_bounds__(kTcThreads, 1) sdf_train_tc_kernel(const __gri
         // ============================== decoder epilogue warps (+ MMA issue by thread 0) ==============================
         asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kEPRegs));
         const int et = tid - 32 * kGSWarps;                     // row of the tile owned by this thread
-        const int eq = et >> 5;                                 // TMEM lane quadrant == warp % 4
+        const int eq = et >> 5;                                 // warp of the warpgroup: rows 16eq.. of each m64 half
         const int g = lane >> 2, t = lane & 3;
-        const uint32_t trow = tmem + ((uint32_t)(32 * eq) << 16);
-        constexpr uint32_t idN32 = tc_idesc(32), idN16 = tc_idesc(16);
+        const float* arow = accs + et * kRowStride;             // this thread's row of the staged accumulators
         // K-major descriptors (LBO = 128 between the two K chunks of a step, SBO = stride of an 8-row group)
-        const uint64_t dH1h = umma_desc(sbase + TP::H1, 128, TP::H1_PT), dH1l = umma_desc(sbase + TP::H1 + TP::H1_BYTES, 128, TP::H1_PT);
-        const uint64_t dDHh = umma_desc(sbase + TP::DH, 128, TP::DH_PT), dDHl = umma_desc(sbase + TP::DH + TP::DH_BYTES, 128, TP::DH_PT);
-        const uint64_t dW1h = umma_desc(sbase + TP::W1H, 128, 256), dW1l = umma_desc(sbase + TP::W1L, 128, 256);
-        const uint64_t dW2h = umma_desc(sbase + TP::W2H, 128, 1024), dW2l = umma_desc(sbase + TP::W2L, 128, 1024);
-        const uint64_t dW2Th = umma_desc(sbase + TP::W2TH, 128, 1024), dW2Tl = umma_desc(sbase + TP::W2TL, 128, 1024);
-        const uint64_t dW1Th = umma_desc(sbase + TP::W1TH, 128, 1024), dW1Tl = umma_desc(sbase + TP::W1TL, 128, 1024);
-        const uint64_t dX0h = umma_desc(sbase + TP::X, 128, TP::X_PT);
-        uint32_t mph = 0;                                       // parity of the next mma_done completion
+        const uint64_t dH1h = wgmma_desc(sbase + TP::H1, 128, TP::H1_PT), dH1l = wgmma_desc(sbase + TP::H1 + TP::H1_BYTES, 128, TP::H1_PT);
+        const uint64_t dDHh = wgmma_desc(sbase + TP::DH, 128, TP::DH_PT), dDHl = wgmma_desc(sbase + TP::DH + TP::DH_BYTES, 128, TP::DH_PT);
+        const uint64_t dW1h = wgmma_desc(sbase + TP::W1H, 128, 256), dW1l = wgmma_desc(sbase + TP::W1L, 128, 256);
+        const uint64_t dW2h = wgmma_desc(sbase + TP::W2H, 128, 1024), dW2l = wgmma_desc(sbase + TP::W2L, 128, 1024);
+        const uint64_t dW2Th = wgmma_desc(sbase + TP::W2TH, 128, 1024), dW2Tl = wgmma_desc(sbase + TP::W2TL, 128, 1024);
+        const uint64_t dW1Th = wgmma_desc(sbase + TP::W1TH, 128, 1024), dW1Tl = wgmma_desc(sbase + TP::W1TL, 128, 1024);
+        const uint64_t dX0h = wgmma_desc(sbase + TP::X, 128, TP::X_PT);
         float dw3acc[32];
 #pragma unroll
         for (int j = 0; j < 32; ++j) dw3acc[j] = 0.f;
@@ -348,16 +358,20 @@ __global__ void __launch_bounds__(kTcThreads, 1) sdf_train_tc_kernel(const __gri
 
             // ---- layer 1: D1 = X W1^T --------------------------------------------------------------------------------
             mbar_wait(bar_x + 8 * slot, (uint32_t)((k >> 1) & 1));
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            if (et == 0) {
-                mma3x(tmem + cD1, dXh, dXl, dW1h, dW1l, 1, idN32);
-                umma_commit(bar_mma);
-            }
-            mbar_wait(bar_mma, mph); mph ^= 1u;
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+            float d[2][16];
             float hv[32];
-            tmem_ld32(trow + cD1, hv);
-            tmem_wait_ld();
+            auto rows_of = [&]() {                              // stage d, read back this thread's row
+                stage_acc(accs, d, eq, lane);
+                ep_bar();
+#pragma unroll
+                for (int c = 0; c < 8; ++c) {
+                    const float4 v = *reinterpret_cast<const float4*>(arow + 4 * c);
+                    hv[4 * c] = v.x; hv[4 * c + 1] = v.y; hv[4 * c + 2] = v.z; hv[4 * c + 3] = v.w;
+                }
+            };
+            mma3x_issue<1>(d, dXh, dXl, dW1h, dW1l, 8 * TP::X_PT);
+            wgmma_wait_all();
+            rows_of();
             uint32_t m1 = 0;
 #pragma unroll
             for (int c = 0; c < 8; ++c) {
@@ -372,19 +386,12 @@ __global__ void __launch_bounds__(kTcThreads, 1) sdf_train_tc_kernel(const __gri
                 *reinterpret_cast<uint4*>(sm + TP::H1 + TP::H1_BYTES + hoff + 128 * c) = make_uint4(l0, l1, l2, l3);
             }
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
             ep_bar();
 
             // ---- layer 2: D2 = H1 W2^T, output layer, loss, dL/dpred ------------------------------------------------------
-            if (et == 0) {
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                mma3x(tmem + cD2, dH1h, dH1l, dW2h, dW2l, 4, idN32);
-                umma_commit(bar_mma);
-            }
-            mbar_wait(bar_mma, mph); mph ^= 1u;
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            tmem_ld32(trow + cD2, hv);
-            tmem_wait_ld();
+            mma3x_issue<4>(d, dH1h, dH1l, dW2h, dW2l, 8 * TP::H1_PT);
+            wgmma_wait_all();
+            rows_of();
             float pr = vec[96];
             uint32_t m2 = 0;
 #pragma unroll
@@ -419,19 +426,12 @@ __global__ void __launch_bounds__(kTcThreads, 1) sdf_train_tc_kernel(const __gri
                 *reinterpret_cast<uint4*>(sm + TP::DH + TP::DH_BYTES + doff + 128 * c) = make_uint4(l0, l1, l2, l3);
             }
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
             ep_bar();
 
             // ---- dgrad layer 2: D3 = dH2 W2 ------------------------------------------------------------------------------
-            if (et == 0) {
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                mma3x(tmem + cD1, dDHh, dDHl, dW2Th, dW2Tl, 4, idN32);
-                umma_commit(bar_mma);
-            }
-            mbar_wait(bar_mma, mph); mph ^= 1u;
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            tmem_ld32(trow + cD1, hv);
-            tmem_wait_ld();
+            mma3x_issue<4>(d, dDHh, dDHl, dW2Th, dW2Tl, 8 * TP::DH_PT);
+            wgmma_wait_all();
+            rows_of();
 #pragma unroll
             for (int c = 0; c < 8; ++c) {
                 uint32_t h0, h1, h2, h3, l0, l1, l2, l3;
@@ -443,17 +443,13 @@ __global__ void __launch_bounds__(kTcThreads, 1) sdf_train_tc_kernel(const __gri
                 *reinterpret_cast<uint4*>(sm + TP::DH + TP::DH_BYTES + doff + 128 * (8 + c)) = make_uint4(l0, l1, l2, l3);
             }
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
             ep_bar();
 
-            // ---- dgrad layer 1 on the tensor core: D4 = dH1 W1 ... --------------------------------------------------------------
-            if (et == 0) {
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                mma3x(tmem + cD4, dDHh + 64, dDHl + 64, dW1Th, dW1Tl, 4, idN16);      // + 8 chunks (1024 B >> 4)
-                umma_commit(bar_mma);
-            }
+            // ---- dgrad layer 1 on the tensor core: D4 = dH1 W1 (N = 8) ... ------------------------------------------------------
+            float d4[2][4];
+            mma3x_issue<4>(d4, dDHh + 64, dDHl + 64, dW1Th, dW1Tl, 8 * TP::DH_PT);      // + 8 chunks (1024 B >> 4)
             // ---- ... while the four warps contract the weight gradients of this round over its 128 points with mma.sync,
-            //      straight from the operand tiles (no tf32 MN-major layout without swizzle exists for tcgen05):
+            //      straight from the operand tiles (tf32 wgmma operands must be K-major, these are MN-major):
             //      dW2 += dH2^T H1, dW1 += dH1^T X, db2 / db1 = column sums (an all-ones B column).  Warp q: points 32q..32q+31
             if (DEC_GRAD) {
                 const uint32_t* xh = reinterpret_cast<const uint32_t*>(sm + TP::X + (2 * slot) * TP::X_BYTES);
@@ -491,11 +487,14 @@ __global__ void __launch_bounds__(kTcThreads, 1) sdf_train_tc_kernel(const __gri
                     }
                 }
             }
-            mbar_wait(bar_mma, mph); mph ^= 1u;
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+            wgmma_wait_all();
+            stage_acc(accs, d4, eq, lane);
+            ep_bar();
             float dxr[8];
-            tmem_ld8(trow + cD4, dxr);
-            tmem_wait_ld();
+            {
+                const float4 v0 = *reinterpret_cast<const float4*>(arow), v1 = *reinterpret_cast<const float4*>(arow + 4);
+                dxr[0] = v0.x; dxr[1] = v0.y; dxr[2] = v0.z; dxr[3] = v0.w; dxr[4] = v1.x; dxr[5] = v1.y; dxr[6] = v1.z; dxr[7] = v1.w;
+            }
             float* dxo = reinterpret_cast<float*>(sm + TP::DX + slot * 4096) + et * 8;
             *reinterpret_cast<float4*>(dxo) = make_float4(dxr[0], dxr[1], dxr[2], dxr[3]);
             *reinterpret_cast<float4*>(dxo + 4) = make_float4(dxr[4], dxr[5], dxr[6], dxr[7]);
@@ -503,7 +502,6 @@ __global__ void __launch_bounds__(kTcThreads, 1) sdf_train_tc_kernel(const __gri
 #pragma unroll
                 for (int q = 0; q < 8; ++q) P.debug_dx[p * 8 + q] = dxr[q];
             }
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
             ep_bar();
             if (et == 0) mbar_arrive(bar_dx + 8 * slot);
         }
@@ -563,12 +561,6 @@ __global__ void __launch_bounds__(kTcThreads, 1) sdf_train_tc_kernel(const __gri
         }
     }
 
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == kGSWarps) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem) : "memory");
-    }
 }
 
 }  // namespace

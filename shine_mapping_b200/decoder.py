@@ -4,7 +4,7 @@ Same module tree (`layers`, `lout`, `nclass_out`) and PyTorch (out,in) weight la
 `load_state_dict(torch.load(...)["geo_decoder"])` (reference shine_batch.py:46-47) and `freeze_model`
 (reference utils/tools.py:188-191) work unchanged.  The class-surface methods stay thin torch calls; the hot path
 does not come through here but through `fused.sdf_bce_step` / `fused.sdf_infer`, which hand these weights to
-the fused sm_100a kernel (`Decoder.c_descriptor`).
+the fused sm_90a kernel (`Decoder.c_descriptor`).
 """
 from __future__ import annotations
 
@@ -62,7 +62,7 @@ class Decoder(nn.Module):
     # ---- fused-kernel plumbing ---------------------------------------------------------------------------
 
     def fused_supported(self) -> bool:
-        """The sm_100a fused kernel covers the north-star lattice: F=8 -> 32 -> 32 -> 1."""
+        """The sm_90a fused kernel covers the north-star lattice: F=8 -> 32 -> 32 -> 1."""
         return (len(self.layers) == 2 and self.layers[0].in_features == 8 and self.layers[0].out_features == 32
                 and self.layers[1].in_features == 32 and self.layers[1].out_features == 32)
 
@@ -74,7 +74,7 @@ class Decoder(nn.Module):
     def c_descriptor(self, grads=None) -> _abi.ShineDecoder:
         if not self.fused_supported():
             raise _abi.ShineB200Error(
-                "fused sm_100a decoder kernel supports feature_dim=8, geo_mlp_level=2, geo_mlp_hidden_dim=32 only")
+                "fused sm_90a decoder kernel supports feature_dim=8, geo_mlp_level=2, geo_mlp_hidden_dim=32 only")
         params = self.fused_params()
         sig = (tuple(p.data_ptr() if p is not None else 0 for p in params),
                tuple(g.data_ptr() if g is not None else 0 for g in grads) if grads is not None else None)

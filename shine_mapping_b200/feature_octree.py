@@ -1,4 +1,4 @@
-"""`FeatureOctree` — drop-in for reference model/feature_octree.py:29-298 whose queries run as sm_100a kernels.
+"""`FeatureOctree` — drop-in for reference model/feature_octree.py:29-298 whose queries run as sm_90a kernels.
 
 Same constructor, attributes and methods as the reference class (SURVEY.md §8b).  What changes underneath:
 
@@ -202,7 +202,7 @@ class FeatureOctree(nn.Module):
         if self.featured_level_num < 1:
             raise ValueError('No level with grid features!')
         if self.featured_level_num > _abi.MAX_LEVELS:
-            raise ValueError(f'tree_level_feat > {_abi.MAX_LEVELS} is not supported by the sm_100a kernels')
+            raise ValueError(f'tree_level_feat > {_abi.MAX_LEVELS} is not supported by the sm_90a kernels')
         self._levels = [_LevelState(self.device) for _ in range(self.max_level + 1)]
         self._dict_cache = None
         self._desc_cache = {}

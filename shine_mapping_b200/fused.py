@@ -1,5 +1,5 @@
 """The fused hot path: reference shine_batch.py:123 (`query_feature`) + :128 (`Decoder.sdf`) + :174
-(`sdf_bce_loss`) + :209 (`backward`) as ONE sm_100a kernel launch (`shine_sdf_bce_step`).
+(`sdf_bce_loss`) + :209 (`backward`) as ONE sm_90a kernel launch (`shine_sdf_bce_step`).
 
 `sdf_bce_step(...)` returns the loss with autograd attached.  Because the loss gradient of a sample depends only
 on that sample, the kernel computes forward, loss AND the full backward (table scatter-add + decoder grads) in one
@@ -123,7 +123,7 @@ def sdf_bce_step(octree: FeatureOctree, decoder: Decoder, coord, sdf_label, sigm
     n_norm: denominator of the "mean" (defaults to len(coord); pass the GLOBAL batch when sharding points).
     morton_ordered: the batch is in Morton order (see SdfTrainer.forward_backward); a performance hint."""
     if coord.requires_grad:
-        raise NotImplementedError("gradients w.r.t. coordinates are not part of the fused sm_100a path")
+        raise NotImplementedError("gradients w.r.t. coordinates are not part of the fused sm_90a path")
     coord, sdf_label = _prep(coord, "coord"), _prep(sdf_label, "sdf_label")
     weight = _prep(weight, "weight") if weighted else None
     if weighted and weight is None:

@@ -6,7 +6,7 @@ snapshots `features_last_frame` / extends `importance_weight`; the optimiser sta
 shine_incre.py:108-109); `iters` x { get_batch -> fused fwd+loss(sum)+bwd -> + lambda_forget * d(reg)/d(features)
 -> Adam }; then `cal_feature_importance` sweeps the frame's pool and accumulates |dL/dfeature| into the importance.
 
-The BCE part is the fused sm_100a step; the regulariser (model/feature_octree.py:246-255) and the importance update touch
+The BCE part is the fused sm_90a step; the regulariser (model/feature_octree.py:246-255) and the importance update touch
 only the rows the batch touched: `shine_mark_touched` collects them (bitmap + compact list, no unique()/sort) and
 `shine_regularization_apply` / `shine_importance_accumulate` run over that list.
 """

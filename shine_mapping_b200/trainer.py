@@ -47,7 +47,7 @@ class SdfTrainer:
         self.group = process_group
         self.morton_ordered = bool(morton_ordered)   # default for every step: batches come from a Morton-sorted SamplePool
         self.tf32x1 = tf32x1
-        # decoder of the fused step on tcgen05.mma / TMEM (csrc/shine_train_tc.cu); None = the library default
+        # decoder of the fused step on wgmma, warp-specialised (csrc/shine_train_tc.cu); None = the library default
         self.tcgen05 = (os.environ.get("SHINE_TRAIN_TCGEN05", "0") == "1") if tcgen05 is None else bool(tcgen05)
         self.lr = config.lr
         self.step_count = 0

@@ -1,4 +1,4 @@
-"""Parity of the sm_100a path (through the C ABI behind the package classes) against the CPU oracle and the
+"""Parity of the sm_90a path (through the C ABI behind the package classes) against the CPU oracle and the
 reference-minted golden vectors.  Tolerances are stated in tests/parity_utils.py."""
 import ctypes as C
 
@@ -195,7 +195,7 @@ def test_infer_and_mask_match_step_pred():
 
 @pytest.mark.parametrize("levels,n_batch", [(4, 3000), (2, 100), (3, 40000), (6, 3000)])
 def test_tcgen05_infer_matches_oracle(levels, n_batch):
-    """tcgen05.mma / TMEM decoder (SHINE_FLAG_TCGEN05) vs the oracle and vs the mma.sync kernel, incl. the mask."""
+    """wgmma decoder (SHINE_FLAG_TCGEN05) vs the oracle and vs the mma.sync kernel, incl. the mask."""
     from shine_mapping_b200 import sdf_infer
     case = make_case(n_points=2500, n_batch=n_batch, feat_levels=levels, seed=90 + levels)
     cfg, octree, dec = build_cuda_models(case, DEV)
@@ -466,7 +466,7 @@ def test_abi_rejects_bad_arguments():
     assert b"invalid" in lib.shine_error_string(-1)
 
 
-# ---- the tcgen05 / TMEM training kernel (csrc/shine_train_tc.cu) ---------------------------------------------------------
+# ---- the warp-specialised wgmma training kernel (csrc/shine_train_tc.cu) ---------------------------------------------------------
 
 def _trainer_step(case, tcgen05, freeze=False):
     from shine_mapping_b200 import SdfTrainer
@@ -489,12 +489,12 @@ def _trainer_step(case, tcgen05, freeze=False):
 
 @pytest.mark.parametrize("levels,poly,weighted,reduction,n_batch", [
     (4, True, False, "mean", 3000), (2, True, False, "mean", 100), (3, False, True, "sum", 5000),
-    (4, True, True, "mean", 60000),          # > 148 tiles of 128 points: several rounds per CTA, both gather groups busy
+    (4, True, True, "mean", 60000),          # > 132 tiles of 128 points: several rounds per CTA, both gather groups busy
     (1, True, False, "mean", 0),             # 16 stragglers only: one partial tile
 ])
 def test_tcgen05_train_step_matches_oracle(levels, poly, weighted, reduction, n_batch):
-    """SHINE_FLAG_TCGEN05 on shine_sdf_bce_step: decoder forward / dgrad / wgrad as tcgen05.mma on 128-point tiles
-    (operands in shared memory, accumulators in TMEM), same tolerances as the mma.sync kernel."""
+    """SHINE_FLAG_TCGEN05 on shine_sdf_bce_step: decoder forward / dgrad as wgmma on 128-point tiles
+    (operands in shared memory), same tolerances as the mma.sync kernel."""
     from tests.parity_utils import drop_relu_kink_points
     case = make_case(n_points=2500, n_batch=n_batch, feat_levels=levels, seed=40 + levels, poly=poly, weighted=weighted,
                      reduction=reduction, n_frames=2 if n_batch > 10000 else 1)

@@ -1,51 +1,26 @@
-"""When the reference checkout is mounted (build container only), run the UNMODIFIED reference classes live (with
-oracle/kaolin_shim) on a fresh seeded case and compare with the oracle restatement.  Skipped on the GPU box, where
-/root/reference does not exist (the frozen goldens cover that)."""
+"""The oracle restatement against the UNMODIFIED reference classes on freshly seeded parity cases.  The reference's
+indices, prediction, loss and table gradients were recorded once by oracle/make_golden.py (make_live_cases, with
+oracle/kaolin_shim) into tests/golden/ref_live_cases.npz; the cases are rebuilt here from their seeds."""
 import os
-import sys
 
 import numpy as np
 import pytest
-import torch
 
 from tests.parity_utils import ROOT, make_case, run_oracle_step
 
-REF = os.environ.get("SHINE_REFERENCE", "/root/reference")
-pytestmark = pytest.mark.skipif(not os.path.isdir(REF), reason="reference checkout not mounted")
+GOLDEN = os.path.join(ROOT, "tests", "golden", "ref_live_cases.npz")
 
 
 @pytest.mark.parametrize("levels,frames,poly", [(2, 1, True), (4, 2, True), (3, 2, False)])
 def test_oracle_equals_live_reference(levels, frames, poly):
-    sys.path.insert(0, os.path.join(ROOT, "oracle", "kaolin_shim"))
-    sys.path.insert(0, REF)
-    from model.decoder import Decoder
-    from model.feature_octree import FeatureOctree
-    from utils.config import SHINEConfig
-    from utils.loss import sdf_bce_loss
+    ref = np.load(GOLDEN)
+    key = f"l{levels}_f{frames}_p{int(poly)}_"
     case = make_case(n_points=1200, n_batch=1000, feat_levels=levels, seed=77 + levels, n_frames=frames, poly=poly)
-    c = SHINEConfig(); c.device = "cpu"
-    c.tree_level_world, c.tree_level_feat, c.leaf_vox_size, c.poly_int_on = 12, levels, 0.2, poly
-    c.calculate_world_scale()
-    octree, dec = FeatureOctree(c), Decoder(c)
-    for fr in case["frames"]:
-        octree.update(torch.from_numpy(fr), False)
-    assert [tuple(p.shape) for p in octree.hier_features] == [t.shape for t in case["tables"]]
-    with torch.no_grad():
-        for p, t in zip(octree.hier_features, case["tables"]):
-            p.copy_(torch.from_numpy(t))
-    sd = dec.state_dict()
-    for k, v in case["dec"].items():
-        sd[k] = torch.from_numpy(v)
-    dec.load_state_dict(sd)
-    coord, label = torch.from_numpy(case["coord"]), torch.from_numpy(case["label"])
-    feature = octree.query_feature(coord)
-    pred = dec.sdf(feature)
-    loss = sdf_bce_loss(pred, label, case["cfg"]["sigma"], None, False, "mean")
-    loss.backward()
+    assert np.array_equal(case["coord"], ref[key + "coord"]), "the seeded case no longer matches the recorded one"
     want = run_oracle_step(case)
-    for a, b in zip(octree.hierarchical_indices, want["indices"]):
-        assert np.array_equal(a.numpy(), b)
-    assert np.abs(pred.detach().numpy() - want["pred"]).max() < 1e-6
-    assert abs(float(loss) - want["loss"]) < 1e-6
-    for p, g in zip(octree.hier_features, want["table_grads"]):
-        assert np.abs(p.grad.numpy() - g).max() <= 1e-5 * np.abs(g).max() + 1e-12
+    for i, b in enumerate(want["indices"]):
+        assert np.array_equal(ref[key + f"indices_{i}"], b)
+    assert np.abs(ref[key + "pred"] - want["pred"]).max() < 1e-6
+    assert abs(float(ref[key + "loss"]) - want["loss"]) < 1e-6
+    for i, g in enumerate(want["table_grads"]):
+        assert np.abs(ref[key + f"tgrad_{i}"] - g).max() <= 1e-5 * np.abs(g).max() + 1e-12

@@ -21,10 +21,11 @@ lib.shine_debug_set_dx(None)
 got = dbg.cpu().numpy()
 err = np.abs(got - ref).max(1) / np.abs(ref).max()
 bad = np.nonzero(err > 1e-4)[0]
+n_sm = torch.cuda.get_device_properties(0).multi_processor_count   # one CTA per SM: tile -> CTA, round
 print("dX: max rel err", err.max(), "points off:", bad.size)
 for i in bad[:40]:
     tile = i // 128; row = i % 128
-    print(f"  point {i}: tile {tile} (cta {tile % 148}, round {tile // 148}) row {row} (gs warp {row // 16}, ep warp {row // 32}) err {err[i]:.3e} got {got[i][:3]} ref {ref[i][:3]}")
+    print(f"  point {i}: tile {tile} (cta {tile % n_sm}, round {tile // n_sm}) row {row} (gs warp {row // 16}, ep warp {row // 32}) err {err[i]:.3e} got {got[i][:3]} ref {ref[i][:3]}")
 if bad.size:
     t = bad // 128
-    print("tiles affected:", np.unique(t).size, "rounds:", np.unique(t // 148, return_counts=True), "rows hist (by 16):", np.bincount((bad % 128) // 16, minlength=8))
+    print("tiles affected:", np.unique(t).size, "rounds:", np.unique(t // n_sm, return_counts=True), "rows hist (by 16):", np.bincount((bad % 128) // 16, minlength=8))

@@ -1,5 +1,6 @@
 // microbenchmark: scatter-add of 32-byte rows to random table rows: (a) 2 x red.global.add.v4.f32 per row (lane pairs),
 // (b) one cp.reduce.async.bulk (TMA) per row from shared memory.
+// build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/micro/tma_reduce tools/micro/tma_reduce.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -34,14 +35,18 @@ __global__ void k_tma(float* table, uint32_t rows, int iters) {
 int main() {
     const uint32_t rows = 86000; float* t; cudaMalloc(&t, (size_t)rows * 32); cudaMemset(t, 0, (size_t)rows * 32);
     cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1); float ms;
-    const int blocks = 148 * 4, thr = 256, iters = 256;
+    int sms = 0, khz = 0;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+    cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, 0);
+    const double hz = khz * 1e3;
+    const int blocks = sms * 4, thr = 256, iters = 256;
     for (int rep = 0; rep < 2; ++rep) {
         cudaEventRecord(e0); k_red<<<blocks, thr>>>(t, rows, iters); cudaEventRecord(e1); cudaEventSynchronize(e1); cudaEventElapsedTime(&ms, e0, e1);
         double nrows = (double)blocks * thr / 2 * iters;
-        printf("red.v4 x2 per row : %.3f ms  %.2f Grows/s  (%.2f rows/clk/SM @1.9GHz)\n", ms, nrows / ms / 1e6, nrows / (ms * 1e-3) / 148 / 1.9e9);
+        printf("red.v4 x2 per row : %.3f ms  %.2f Grows/s  (%.2f rows/clk/SM at the maximum SM clock)\n", ms, nrows / ms / 1e6, nrows / (ms * 1e-3) / sms / hz);
         cudaEventRecord(e0); k_tma<<<blocks, thr, thr * 32>>>(t, rows, iters / 2); cudaEventRecord(e1); cudaEventSynchronize(e1); cudaEventElapsedTime(&ms, e0, e1);
         nrows = (double)blocks * thr * (iters / 2);
-        printf("TMA bulk reduce   : %.3f ms  %.2f Grows/s  (%.2f rows/clk/SM)  err=%s\n", ms, nrows / ms / 1e6, nrows / (ms * 1e-3) / 148 / 1.9e9, cudaGetErrorString(cudaGetLastError()));
+        printf("TMA bulk reduce   : %.3f ms  %.2f Grows/s  (%.2f rows/clk/SM)  err=%s\n", ms, nrows / ms / 1e6, nrows / (ms * 1e-3) / sms / hz, cudaGetErrorString(cudaGetLastError()));
     }
     float h[8]; cudaMemcpy(h, t, 32, cudaMemcpyDeviceToHost); printf("row0 = %g %g ... (sanity)\n", h[0], h[7]);
     return 0;
