@@ -217,7 +217,8 @@ int shine_octree_corner_rehash(void* corner_slots, uint32_t capacity, const int6
  * Accumulates dL/d(tables) into lv[i].feature_grads and dL/d(decoder) into dec->g* (both terms).
  *   weight     [n]: sign marks surface (+) / free-space (-) samples (shine_batch.py:137); |weight| multiplies the BCE
  *              term only with SHINE_FLAG_WEIGHTED
- *   n_surface  device int32: number of samples with weight > 0 (shine_count_positive); 0 -> no eikonal contribution
+ *   n_surface  device int32: number of samples with weight > 0 (shine_count_positive) in the whole batch; when this call
+ *              sees one part of it (a rank's shard, a chunk), the count of the whole batch; 0 -> no eikonal contribution
  *   out_pred [n] / out_grad [n,3] (g) may be NULL; out_loss (+=) BCE part; out_eikonal (+=) the mean, without weight_e */
 int shine_count_positive(const float* values, int64_t n, int32_t* out_count, void* stream);
 int shine_sdf_bce_eikonal_step(const shine_octree* oct, const shine_decoder* dec, const float* coord,

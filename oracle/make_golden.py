@@ -8,6 +8,7 @@ that the oracle restatement (tests/test_oracle_golden.py) and the CUDA path (tes
 checked against the reference itself without the reference checkout.
 
     python oracle/make_golden.py            # rewrites tests/golden/*.npz
+    python oracle/make_golden.py NAME ...   # rewrites only the named ones
 """
 from __future__ import annotations
 
@@ -120,14 +121,17 @@ def make(name, feat_levels, n_frames, n_azimuth, n_batch, seed, poly=True, weigh
           f"-> {path} ({os.path.getsize(path) / 1e6:.2f} MB)")
 
 
-def make_eikonal(name, feat_levels, n_azimuth, n_batch, seed, poly=True, weight_e=0.1):
+def make_eikonal(name, feat_levels, n_azimuth, n_batch, seed, poly=True, weight_e=0.1, weighted=False, reduction="mean",
+                 table_scale=1.0):
     """Loop body with ekional_loss_on: the reference's get_gradient (utils/tools.py:175-185 — restated inline because
-    utils/tools.py imports open3d) on the reference's own FeatureOctree / Decoder, shine_batch.py:119-120,137-142,172-185."""
+    utils/tools.py imports open3d) on the reference's own FeatureOctree / Decoder, shine_batch.py:119-120,137-142,172-185.
+    table_scale multiplies the freshly initialised tables: at scale 1 |g| is ~1e-3 and the eikonal term barely moves the
+    gradients; a trained map has |g| around 1, where the sign of (|g| - 1) flips between samples."""
     SHINEConfig, FeatureOctree, Decoder, dataSampler, sdf_bce_loss = import_reference()
     sys.path.insert(0, ROOT)
     from shine_mapping_b200 import synth
     torch.manual_seed(seed)
-    cfg = reference_config(SHINEConfig, feat_levels, 0.2, poly, False, "mean")
+    cfg = reference_config(SHINEConfig, feat_levels, 0.2, poly, weighted, reduction)
     octree, decoder, sampler = FeatureOctree(cfg), Decoder(cfg), dataSampler(cfg)
     dirs, boxes = synth.lidar_directions(n_azimuth), synth.default_boxes()
     origin = torch.zeros(3)
@@ -137,6 +141,11 @@ def make_eikonal(name, feat_levels, n_azimuth, n_batch, seed, poly=True, weight_
     octree.update(surface, False)
     index = torch.randint(0, coord.shape[0], (n_batch,))
     coord, label, weight = coord[index].clone(), label[index], weight[index]
+    if weighted:
+        weight = weight * (0.5 + torch.rand(weight.shape[0]))
+    with torch.no_grad():
+        for p in octree.hier_features:
+            p.mul_(table_scale)
     sigma = cfg.logistic_gaussian_ratio * cfg.sigma_sigmoid_m * cfg.scale
     tables_before = [p.detach().numpy().copy() for p in octree.hier_features]
     coord.requires_grad_(True)                                             # shine_batch.py:119-120
@@ -145,27 +154,36 @@ def make_eikonal(name, feat_levels, n_azimuth, n_batch, seed, poly=True, weight_
     surface_mask = weight > 0
     g = torch.autograd.grad(outputs=pred, inputs=coord, grad_outputs=torch.ones_like(pred), create_graph=True,
                             retain_graph=True, only_inputs=True)[0] * sigma   # get_gradient(coord, pred) * sigma_sigmoid
-    loss = sdf_bce_loss(pred, label, sigma, torch.abs(weight), False, "mean")
+    loss = sdf_bce_loss(pred, label, sigma, torch.abs(weight), cfg.loss_weight_on, cfg.loss_reduction)   # :172-174
     eikonal = ((1.0 - g[surface_mask].norm(2, dim=-1)) ** 2).mean()          # shine_batch.py:183-185
     total = loss + weight_e * eikonal
+    # the eikonal mean's own gradients too: beside the BCE sum of a batch its share of the total is small
+    params = list(octree.hier_features) + [dict(decoder.named_parameters())[k] for k in DEC_KEYS]
+    eik_grads = torch.autograd.grad(eikonal, params, retain_graph=True, allow_unused=True)
+    eik_grads = [torch.zeros_like(p) if d is None else d for p, d in zip(params, eik_grads)]   # lout.bias: unused
     total.backward()
     out = {"cfg_json": np.array(json.dumps(dict(tree_level_world=12, tree_level_feat=feat_levels, feature_dim=cfg.feature_dim,
-                                                 poly_int_on=poly, leaf_vox_size=0.2, sigma=float(sigma), weighted=False,
-                                                 reduction="mean", decoder_frozen=False, n_frames=1, weight_e=weight_e))),
+                                                 poly_int_on=poly, leaf_vox_size=0.2, sigma=float(sigma), weighted=weighted,
+                                                 reduction=reduction, decoder_frozen=False, n_frames=1, weight_e=weight_e,
+                                                 table_scale=table_scale))),
            "frame_0": surface.numpy().copy(), "coord": coord.detach().numpy(), "label": label.numpy(), "weight": weight.numpy(),
-           "exp_g": g.detach().numpy(), "exp_eikonal": np.array(float(eikonal)), "exp_loss": np.array(float(total)),
+           "exp_g": g.detach().numpy(), "exp_eikonal": np.array(float(eikonal.detach())),
+           "exp_loss": np.array(float(total.detach())),
            "exp_pred": pred.detach().numpy()}
     for k, t in enumerate(tables_before):
         out[f"table_{k}"] = t
         out[f"exp_tgrad_{k}"] = octree.hier_features[k].grad.numpy()
+        out[f"exp_eik_tgrad_{k}"] = eik_grads[k].numpy()
     sd, params = decoder.state_dict(), dict(decoder.named_parameters())
-    for k in DEC_KEYS:
+    for j, k in enumerate(DEC_KEYS):
         out["dec_" + k] = sd[k].numpy()
         out["exp_dgrad_" + k] = params[k].grad.numpy()
+        out["exp_eik_dgrad_" + k] = eik_grads[len(tables_before) + j].numpy()
     path = os.path.join(ROOT, "tests", "golden", name + ".npz")
     np.savez_compressed(path, **out)
-    print(f"{name}: N={coord.shape[0]} eikonal={float(eikonal):.6f} loss={float(total):.6f} -> {path} "
-          f"({os.path.getsize(path) / 1e6:.2f} MB)")
+    gn = g.detach()[surface_mask].norm(dim=-1)
+    print(f"{name}: N={coord.shape[0]} eikonal={float(eikonal):.6f} loss={float(total):.6f} surface |g|: median "
+          f"{float(gn.median()):.3f}, {float((gn > 1).float().mean()):.0%} above 1 -> {path} ({os.path.getsize(path) / 1e6:.2f} MB)")
 
 
 # the make_case() cases of tests/test_reference_live.py: (levels, frames, poly)
@@ -211,13 +229,23 @@ def make_live_cases(name="ref_live_cases"):
     print(f"{name}: {len(LIVE_CASES)} cases -> {path} ({os.path.getsize(path) / 1e6:.2f} MB)")
 
 
+GOLDENS = {
+    "ref_c1_l2_mean": lambda n: make(n, feat_levels=2, n_frames=1, n_azimuth=14, n_batch=1500, seed=42),
+    "ref_c2_l4_pretrained_frozen": lambda n: make(n, feat_levels=4, n_frames=1, n_azimuth=12, n_batch=1500, seed=43,
+                                                  pretrained=True),
+    "ref_incre_l3_sum_weighted_linear": lambda n: make(n, feat_levels=3, n_frames=2, n_azimuth=10, n_batch=1200, seed=44,
+                                                       poly=False, weighted=True, reduction="sum"),
+    "ref_eikonal_l3": lambda n: make_eikonal(n, feat_levels=3, n_azimuth=10, n_batch=1000, seed=45),
+    # tables x500 (printed when minted): median surface |g| near 1, a good share of the samples on either side
+    "ref_eikonal_l3_sum_weighted": lambda n: make_eikonal(n, feat_levels=3, n_azimuth=10, n_batch=1000, seed=46,
+                                                          weighted=True, reduction="sum", table_scale=500.0),
+    "ref_live_cases": make_live_cases,
+}
+
+
 if __name__ == "__main__":
+    # python oracle/make_golden.py [NAME ...]: mint only the named goldens (default: all)
     if not os.path.isdir(REF):
         sys.exit(f"{REF} not found: goldens can only be minted where the reference is mounted")
-    make("ref_c1_l2_mean", feat_levels=2, n_frames=1, n_azimuth=14, n_batch=1500, seed=42)
-    make("ref_c2_l4_pretrained_frozen", feat_levels=4, n_frames=1, n_azimuth=12, n_batch=1500, seed=43,
-         pretrained=True)
-    make("ref_incre_l3_sum_weighted_linear", feat_levels=3, n_frames=2, n_azimuth=10, n_batch=1200, seed=44,
-         poly=False, weighted=True, reduction="sum")
-    make_eikonal("ref_eikonal_l3", feat_levels=3, n_azimuth=10, n_batch=1000, seed=45)
-    make_live_cases()
+    for golden in sys.argv[1:] or list(GOLDENS):
+        GOLDENS[golden](golden)

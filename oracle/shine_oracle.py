@@ -282,9 +282,15 @@ def cal_feature_importance(octree: OracleOctree, dec: dict, coord_pool, label_po
     return importance
 
 
-def train_step_eikonal(octree: OracleOctree, dec: dict, coord, label, weight, sigma: float, weight_e: float = 0.1):
+def train_step_eikonal(octree: OracleOctree, dec: dict, coord, label, weight, sigma: float, weight_e: float = 0.1,
+                       weighted: bool = False, reduction: str = "mean", n_surface=None):
     """Loop body with ekional_loss_on (shine_batch.py:119-120,137-142,172-185,208-209): g = d pred / d coord (create_graph)
-    * sigma_sigmoid; eikonal = mean over surface samples of (1 - |g|)^2; loss = bce(mean) + weight_e * eikonal."""
+    * sigma_sigmoid; eikonal = mean over surface samples (weight > 0) of (1 - |g|)^2; loss = bce + weight_e * eikonal.
+    BCE as shine_batch.py:172-174: |weight| applied only when `weighted`, with the given reduction.
+    n_surface: denominator of the eikonal mean (default: this batch's surface count; pass the global count when the
+    batch is one shard of a larger one).  Like the reference, a batch without a surface sample gives NaN (mean of empty).
+    Besides the total's gradients, returns those of bce alone (`bce_*_grads`) and of the eikonal mean alone (`eik_*_grads`,
+    i.e. at weight_e = 1)."""
     for f in octree.hier_features:
         f.grad = None
     for p in dec.values():
@@ -294,10 +300,22 @@ def train_step_eikonal(octree: OracleOctree, dec: dict, coord, label, weight, si
     pred = decoder_sdf(feature, dec)
     surface_mask = weight > 0
     g = torch.autograd.grad(pred, coord, torch.ones_like(pred), create_graph=True, retain_graph=True)[0] * sigma
-    bce = sdf_bce_loss(pred, label, sigma, torch.abs(weight), False, "mean")
-    eik = ((1.0 - g[surface_mask].norm(2, dim=-1)) ** 2).mean()
+    bce = sdf_bce_loss(pred, label, sigma, torch.abs(weight), weighted, reduction)
+    sq = (1.0 - g[surface_mask].norm(2, dim=-1)) ** 2
+    eik = sq.mean() if n_surface is None else sq.sum() / float(n_surface)
     loss = bce + weight_e * eik
+    params = list(octree.hier_features) + list(dec.values())
+
+    def grads(term):
+        got = torch.autograd.grad(term, params, retain_graph=True, allow_unused=True)
+        got = [torch.zeros_like(p) if d is None else d for p, d in zip(params, got)]
+        L = len(octree.hier_features)
+        return got[:L], dict(zip(dec.keys(), got[L:]))
+
+    bce_t, bce_d = grads(bce)
+    eik_t, eik_d = grads(eik) if bool(surface_mask.any()) else grads(0.0 * pred.sum())
     loss.backward()
     return {"loss": loss.detach(), "bce": bce.detach(), "eikonal": eik.detach(), "g": g.detach(), "pred": pred.detach(),
             "table_grads": [f.grad if f.grad is not None else torch.zeros_like(f) for f in octree.hier_features],
-            "dec_grads": {k: (p.grad if p.grad is not None else torch.zeros_like(p)) for k, p in dec.items()}}
+            "dec_grads": {k: (p.grad if p.grad is not None else torch.zeros_like(p)) for k, p in dec.items()},
+            "bce_table_grads": bce_t, "bce_dec_grads": bce_d, "eik_table_grads": eik_t, "eik_dec_grads": eik_d}

@@ -5,6 +5,8 @@ Per frame: the pool holds this frame's samples only, `octree.update(surface, inc
 snapshots `features_last_frame` / extends `importance_weight`; the optimiser state is rebuilt (reference
 shine_incre.py:108-109); `iters` x { get_batch -> fused fwd+loss(sum)+bwd -> + lambda_forget * d(reg)/d(features)
 -> Adam }; then `cal_feature_importance` sweeps the frame's pool and accumulates |dL/dfeature| into the importance.
+With `ekional_loss_on` (the reference's replay configs set it) the step is the fused BCE + eikonal launch instead
+(shine_incre.py:159-165: + weight_e * mean over surface samples of (1 - |g|)^2).
 
 The BCE part is the fused sm_90a step; the regulariser (model/feature_octree.py:246-255) and the importance update touch
 only the rows the batch touched: `shine_mark_touched` collects them (bitmap + compact list, no unique()/sort) and
@@ -112,7 +114,7 @@ def cal_feature_importance(trainer: SdfTrainer, octree: FeatureOctree, coord_poo
 def run_shine_mapping_incremental(config: SHINEConfig, octree: FeatureOctree, decoder: Decoder, frames, iters=None,
                                   log=None):
     """frames: iterable of (coord, sdf_label, weight) sample sets, one per scan (what `process_frame` leaves in the
-    pools).  Returns per-frame dicts with first/last loss."""
+    pools).  Returns per-frame dicts with first/last loss (and first/last eikonal mean with ekional_loss_on)."""
     if config.continual_learning_reg:
         config.loss_reduction = "sum"          # reference shine_incre.py:77-78
     iters = config.iters if iters is None else iters
@@ -133,18 +135,26 @@ def run_shine_mapping_incremental(config: SHINEConfig, octree: FeatureOctree, de
         for it in range(iters):
             index = torch.randint(0, n, (config.bs,), device=dev)
             c, l, w = coord[index], label[index], weight[index]
-            loss = trainer.forward_backward(c, l, w)
-            total = loss.clone()
+            if config.ekional_loss_on:                                              # shine_incre.py:159-165
+                loss, eik = trainer.forward_backward_eikonal(c, l, w)
+                total = loss + config.weight_e * eik
+            else:
+                loss, eik = trainer.forward_backward(c, l, w), None
+                total = loss.clone()
             if config.continual_learning_reg:
                 total = total + config.lambda_forget * add_regularization(trainer, octree, config.lambda_forget, c)
             trainer.optimizer_step(zero_grad=True)
             if it == 0:
                 first, bce_first = float(total), float(loss)
+                eik_first = float(eik) if eik is not None else None
         last, bce_last = float(total), float(loss)
+        eik_last = float(eik) if eik is not None else None
         if config.continual_learning_reg:
             cal_feature_importance(trainer, octree, coord, label, config.bs, config.cal_importance_weight_down_rate)
         history.append({"frame": fid, "loss_first": first, "loss_last": last, "bce_first": bce_first, "bce_last": bce_last,
                         "rows": [int(p.shape[0]) for p in octree.hier_features]})
+        if config.ekional_loss_on:
+            history[-1].update(eik_first=eik_first, eik_last=eik_last)
         if log:
             log(history[-1])
     return history

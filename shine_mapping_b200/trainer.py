@@ -151,11 +151,16 @@ class SdfTrainer:
             self.octree._reduce_replicas(od, coord.device)
         return self.loss
 
-    def forward_backward_eikonal(self, coord, sdf_label, weight, n_norm=None, pred_out=None, grad_out=None):
+    def forward_backward_eikonal(self, coord, sdf_label, weight, n_norm=None, pred_out=None, grad_out=None,
+                                 n_surface=None):
         """The step with `ekional_loss_on` (reference shine_batch.py:119-142,172-185,208-209) as ONE launch
         (`shine_sdf_bce_eikonal_step`): BCE + weight_e * mean over surface samples of (1 - |sigma d pred/d coord|)^2,
         gradients of both terms accumulated into the flat buffer.  -> (bce loss, eikonal mean) device scalars;
-        the loop's total loss is bce + config.weight_e * eikonal."""
+        the loop's total loss is bce + config.weight_e * eikonal.
+        n_surface: denominator of the eikonal mean, the analogue of n_norm: the number of surface samples (weight > 0) in
+        the GLOBAL batch when this call sees one part of it.  None = counted on the device from this batch and, when the
+        trainer runs on several ranks, summed over them, so that the per-rank eikonal values and gradients add up to those
+        of the global batch.  A batch without surface sample contributes 0 (not the NaN of torch's mean of nothing)."""
         self._sync()
         cfg = self.config
         n = coord.shape[0]
@@ -167,18 +172,26 @@ class SdfTrainer:
         if aux is None or aux[0].device != dev:
             aux = (torch.zeros(1, dtype=torch.int32, device=dev), torch.zeros(1, dtype=torch.float32, device=dev))
             self._eik_aux = aux
-        n_surface, eik = aux
-        n_surface.zero_(); eik.zero_()
+        count, eik = aux
+        eik.zero_()
         if not self._loss_clean:
             self.loss.zero_()
         self._loss_clean = False
         od = self.octree._descriptor(None, self.table_grads)
         dd = self.decoder.c_descriptor(self.dec_grads if self._dec_trainable else None)
         lib, st = _abi.lib(), _abi.stream_ptr(dev)
-        _abi.check(lib.shine_count_positive(_abi.ptr(weight), n, _abi.ptr(n_surface), st), "shine_count_positive")
+        if n_surface is not None:
+            count.fill_(int(n_surface))
+        else:
+            count.zero_()
+            _abi.check(lib.shine_count_positive(_abi.ptr(weight), n, _abi.ptr(count), st), "shine_count_positive")
+            if self._world() > 1:
+                total = count.float()                 # exact below 2^24 samples; the collectives here sum fp32
+                self._all_reduce(total)
+                count.copy_(total.round())
         _abi.check(lib.shine_sdf_bce_eikonal_step(
             C.byref(od), C.byref(dd), _abi.ptr(coord), _abi.ptr(sdf_label), _abi.ptr(weight), n, float(self.sigma), scale,
-            float(cfg.weight_e), _abi.ptr(n_surface), _abi.ptr(pred_out), _abi.ptr(grad_out), _abi.ptr(self.loss),
+            float(cfg.weight_e), _abi.ptr(count), _abi.ptr(pred_out), _abi.ptr(grad_out), _abi.ptr(self.loss),
             _abi.ptr(eik), flags, st), "shine_sdf_bce_eikonal_step")
         return self.loss, eik.view(())
 
@@ -188,6 +201,13 @@ class SdfTrainer:
         elif torch.distributed.is_available() and torch.distributed.is_initialized():
             torch.distributed.all_reduce(buf, group=self.group)
 
+    def _world(self) -> int:
+        if self.comm is not None:
+            return self.comm.world
+        if torch.distributed.is_available() and torch.distributed.is_initialized():
+            return torch.distributed.get_world_size(self.group)
+        return 1
+
     def all_reduce_grads(self):
         """The step's exchange, ONE sum collective (the 1/N_global is already in the per-point gradient scale):
         replicated -> the whole flat gradient; spatial -> [decoder | rows shared with other ranks]."""
@@ -195,10 +215,7 @@ class SdfTrainer:
             if self.p2p.world > 1:
                 self.p2p.exchange(self.dec_flat, self.boundary, self.table_grads)
             return
-        world = self.comm.world if self.comm is not None else (
-            torch.distributed.get_world_size(self.group)
-            if torch.distributed.is_available() and torch.distributed.is_initialized() else 1)
-        if world <= 1:
+        if self._world() <= 1:
             return
         if self.shard_mode == "replicated":
             self._all_reduce(self.flat_grad)

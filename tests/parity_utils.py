@@ -26,6 +26,11 @@ from oracle import shine_oracle as orc  # noqa: E402  (tests are allowed to impo
 DEC_KEYS = ["layers.0.weight", "layers.0.bias", "layers.1.weight", "layers.1.bias", "lout.weight", "lout.bias"]
 
 
+def dec_keys(case):
+    """The DEC_KEYS a case's decoder has (a decoder built with geo_mlp_bias_on=False has no bias entries)."""
+    return [k for k in DEC_KEYS if k in case["dec"]]
+
+
 def make_config(feat_levels=2, world_level=12, leaf_vox=0.2, device="cpu", **kw):
     from shine_mapping_b200.config import SHINEConfig
     base = dict(tree_level_world=world_level, tree_level_feat=feat_levels, leaf_vox_size=leaf_vox, device=device,
@@ -36,9 +41,10 @@ def make_config(feat_levels=2, world_level=12, leaf_vox=0.2, device="cpu", **kw)
 
 
 def make_case(n_points=3000, n_batch=2048, feat_levels=2, seed=0, n_frames=1, poly=True, weighted=False,
-              reduction="mean", world_level=12, n_azimuth=None, feature_dim=8):
+              reduction="mean", world_level=12, n_azimuth=None, feature_dim=8, bias=True):
     """Seeded synthetic case on the CPU: scans -> samples -> oracle octree -> batch (with out-of-map and
-    out-of-cube stragglers appended to exercise the miss / clamp rules)."""
+    out-of-cube stragglers appended to exercise the miss / clamp rules).  bias=False: decoder without biases
+    (geo_mlp_bias_on: False)."""
     from shine_mapping_b200 import synth
     torch.manual_seed(seed)
     cfg = make_config(feat_levels, world_level, poly_int_on=poly, loss_weight_on=weighted, loss_reduction=reduction,
@@ -68,11 +74,11 @@ def make_case(n_points=3000, n_batch=2048, feat_levels=2, seed=0, n_frames=1, po
     weight = torch.cat((weight, torch.ones(extra.shape[0]), torch.ones(10)))
     if weighted:  # make the weights non-trivial
         weight = weight * (0.5 + torch.rand(weight.shape[0], generator=gen))
-    dec = orc.make_decoder_params(cfg.feature_dim, 32, 2, True)
+    dec = orc.make_decoder_params(cfg.feature_dim, 32, 2, bias)
     return {
         "cfg": dict(tree_level_world=world_level, tree_level_feat=feat_levels, feature_dim=cfg.feature_dim,
                     poly_int_on=poly, leaf_vox_size=cfg.leaf_vox_size, sigma=float(cfg.sigma_sigmoid),
-                    weighted=weighted, reduction=reduction),
+                    weighted=weighted, reduction=reduction, bias=bias),
         "frames": frames,
         "tables": [t.detach().numpy().copy() for t in oct_o.hier_features],
         "dec": {k: v.detach().numpy().copy() for k, v in dec.items()},
@@ -98,8 +104,9 @@ def drop_relu_kink_points(case, eps=2e-6):
     o, dec = oracle_from_case(case)
     with torch.no_grad():
         f = o.query_feature(torch.from_numpy(case["coord"])).double()
-        a1 = f @ dec["layers.0.weight"].double().T + dec["layers.0.bias"].double()
-        a2 = torch.relu(a1) @ dec["layers.1.weight"].double().T + dec["layers.1.bias"].double()
+        zero = torch.zeros((), dtype=torch.float64)
+        a1 = f @ dec["layers.0.weight"].double().T + dec.get("layers.0.bias", zero).double()
+        a2 = torch.relu(a1) @ dec["layers.1.weight"].double().T + dec.get("layers.1.bias", zero).double()
         keep = ((a1.abs().min(1).values > eps) & (a2.abs().min(1).values > eps)).numpy()
     out = dict(case)
     for k in ("coord", "label", "weight"):
@@ -141,7 +148,7 @@ def build_cuda_models(case, device="cuda:0", freeze_decoder=False):
     c = case["cfg"]
     cfg = make_config(c["tree_level_feat"], c["tree_level_world"], c["leaf_vox_size"], device=device,
                       poly_int_on=c["poly_int_on"], feature_dim=c["feature_dim"], loss_weight_on=c["weighted"],
-                      loss_reduction=c["reduction"])
+                      loss_reduction=c["reduction"], geo_mlp_bias_on=c.get("bias", True))
     octree = FeatureOctree(cfg)
     for fr in case["frames"]:
         octree.update(torch.from_numpy(np.asarray(fr)).to(device))
@@ -152,7 +159,8 @@ def build_cuda_models(case, device="cuda:0", freeze_decoder=False):
             p.copy_(torch.from_numpy(np.asarray(t)))
     dec = Decoder(cfg)
     sd = dec.state_dict()
-    for k in DEC_KEYS:
+    assert all(k in case["dec"] for k in sd if k.startswith(("layers.", "lout."))), "decoder keys differ from the case's"
+    for k in dec_keys(case):
         sd[k] = torch.from_numpy(np.asarray(case["dec"][k])).to(device)
     dec.load_state_dict(sd)
     if freeze_decoder:
@@ -182,7 +190,7 @@ def run_cuda_step(case, device="cuda:0", single_pass=True, tf32x1=False, unfused
         "indices": indices, "feature": feature.detach().cpu().numpy(), "pred": pred.detach().cpu().numpy(),
         "loss": float(loss.detach()),
         "table_grads": [p.grad.cpu().numpy() for p in octree.hier_features],
-        "dec_grads": {} if freeze_decoder else {k: dict(dec.named_parameters())[k].grad.cpu().numpy() for k in DEC_KEYS},
+        "dec_grads": {} if freeze_decoder else {k: dict(dec.named_parameters())[k].grad.cpu().numpy() for k in dec_keys(case)},
     }
 
 
@@ -224,6 +232,16 @@ def compare_step(got, want, pred_atol=2e-5, pred_rtol=1e-5, grad_rel=2e-4, check
 
 GOLDEN_DIR = os.path.join(ROOT, "tests", "golden")
 GOLDEN_NAMES = ["ref_c1_l2_mean", "ref_c2_l4_pretrained_frozen", "ref_incre_l3_sum_weighted_linear"]
+
+
+def load_eikonal_golden(name):
+    """-> (case, npz) of a golden minted by oracle/make_golden.py::make_eikonal (one frame, expected outputs in the npz)."""
+    import json
+    z = np.load(os.path.join(GOLDEN_DIR, name + ".npz"))
+    cfg = json.loads(str(z["cfg_json"]))
+    case = {"cfg": cfg, "frames": [z["frame_0"]], "tables": [z[f"table_{k}"] for k in range(cfg["tree_level_feat"])],
+            "dec": {k: z["dec_" + k] for k in DEC_KEYS}, "coord": z["coord"], "label": z["label"], "weight": z["weight"]}
+    return case, z
 
 
 def load_golden(name):

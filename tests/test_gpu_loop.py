@@ -98,6 +98,67 @@ def test_two_gpu_data_parallel_matches_oracle(tmp_path, built_lib):
     assert abs(float(np.load(tmp_path / "loss.npy")) - want["loss"]) <= 2e-5 * abs(want["loss"])
 
 
+def _dp_eikonal_worker(rank, world, port, out_dir):
+    os.environ.update(RANK=str(rank), WORLD_SIZE=str(world), LOCAL_RANK=str(rank), MASTER_ADDR="127.0.0.1",
+                      MASTER_PORT=str(port))
+    from shine_mapping_b200 import SdfTrainer, dist as sdist
+    sdist.init_from_env("nccl")
+    dev = f"cuda:{rank}"
+    case = _eikonal_dp_case()
+    cfg, octree, dec = build_cuda_models(case, dev)
+    cfg.ekional_loss_on, cfg.weight_e = True, 1.0
+    n = case["coord"].shape[0]
+    b, e = sdist.shard_range(n, rank, world)
+    coord = torch.from_numpy(case["coord"][b:e]).to(dev); label = torch.from_numpy(case["label"][b:e]).to(dev)
+    weight = torch.from_numpy(case["weight"][b:e]).to(dev)
+    tr = SdfTrainer(cfg, octree, dec, shard_mode="replicated")
+    tr.zero_grad()
+    bce, eik = tr.forward_backward_eikonal(coord, label, weight, n_norm=n)    # surface count summed over the ranks
+    scalars = torch.stack([bce.clone(), eik.clone()])
+    tr.all_reduce_grads()
+    sdist.all_reduce_sum(scalars)
+    torch.cuda.synchronize()
+    if rank == 0:
+        np.save(os.path.join(out_dir, "flat.npy"), tr.flat_grad.cpu().numpy())
+        np.save(os.path.join(out_dir, "scalars.npy"), scalars.cpu().numpy())
+    torch.distributed.destroy_process_group()
+
+
+def _eikonal_dp_case():
+    case = make_case(n_points=2500, n_batch=6000, feat_levels=4, seed=52)
+    case["tables"] = [t * np.float32(300.0) for t in case["tables"]]       # surface |g| around 1
+    return case
+
+
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs")
+def test_two_gpu_data_parallel_eikonal_matches_oracle(tmp_path, built_lib):
+    """ekional_loss_on with the point batch sharded over 2 GPUs: the eikonal mean is over the surface samples of the
+    GLOBAL batch, so the summed per-rank values and the all-reduced gradients equal the oracle's for the whole batch."""
+    import torch.multiprocessing as mp
+    from oracle import shine_oracle as orc
+    from tests.parity_utils import DEC_KEYS, oracle_from_case
+    mp.spawn(_dp_eikonal_worker, args=(2, _free_port(), str(tmp_path)), nprocs=2, join=True)
+    got = np.load(tmp_path / "flat.npy")
+    bce, eik = np.load(tmp_path / "scalars.npy")
+    case = _eikonal_dp_case()
+    o, odec = oracle_from_case(case)
+    want = orc.train_step_eikonal(o, odec, torch.from_numpy(case["coord"]), torch.from_numpy(case["label"]),
+                                  torch.from_numpy(case["weight"]), case["cfg"]["sigma"], 1.0)
+    assert abs(float(eik) - float(want["eikonal"])) <= 1e-4 * float(want["eikonal"])
+    assert abs(float(bce) + float(eik) - float(want["loss"])) <= 1e-4 * float(want["loss"])
+    off = 0
+    for g in want["table_grads"]:
+        g = g.numpy()
+        seg = got[off:off + g.size].reshape(g.shape)
+        assert np.abs(seg[:-1] - g[:-1]).max() <= 1e-3 * np.abs(g).max() + 1e-10
+        off += (g.size + 3) & ~3
+    for k in DEC_KEYS:
+        g = want["dec_grads"][k].numpy()
+        seg = got[off:off + g.size].reshape(g.shape)
+        assert np.abs(seg - g).max() <= 1e-3 * np.abs(g).max() + 1e-10, k
+        off += (g.size + 3) & ~3
+
+
 @pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs")
 def test_abi_launches_on_the_device_that_owns_the_tensors(built_lib):
     """ADVICE r01: model on cuda:1 while the current device is cuda:0 — every entry point must launch on cuda:1 (device
@@ -208,6 +269,39 @@ def test_incremental_loop_runs(built_lib):
     assert hist[2]["rows"][-1] > hist[0]["rows"][-1]                       # the map grew
     assert not any(p.requires_grad for p in decoder.parameters())          # frozen after frame 2
     assert all(w.abs().sum() > 0 for w in octree.importance_weight)
+
+
+def test_incremental_loop_with_eikonal(built_lib, monkeypatch):
+    """ekional_loss_on in the incremental loop (the reference's replay configs set it; shine_incre.py:159-165): every
+    step is the fused BCE + eikonal launch, including after the decoder is frozen (the table-gradient-only kernel)."""
+    from shine_mapping_b200 import Decoder, FeatureOctree, SdfTrainer, synth
+    from shine_mapping_b200.incre_loop import run_shine_mapping_incremental
+    calls = []
+    step = SdfTrainer.forward_backward_eikonal
+
+    def counted(self, *a, **kw):
+        calls.append(self._dec_trainable)
+        return step(self, *a, **kw)
+    monkeypatch.setattr(SdfTrainer, "forward_backward_eikonal", counted)
+    cfg = make_config(3, device=DEV, bs=2048, lr=0.01, iters=40, continual_learning_reg=True, lambda_forget=1e3,
+                      freeze_after_frame=1, ekional_loss_on=True, weight_e=1.0)
+    torch.manual_seed(1)
+    octree, decoder = FeatureOctree(cfg), Decoder(cfg)
+    dirs, boxes = synth.lidar_directions(128, device=DEV), synth.default_boxes(DEV)
+    gen = torch.Generator(device=DEV).manual_seed(3)
+    frames = []
+    for f in range(2):
+        origin = torch.tensor([2.0 * f, 0.0, 0.0], device=DEV)
+        hits = synth.raycast_scene(origin, dirs, boxes, cfg.min_range, cfg.pc_radius)
+        frames.append(synth.sample_rays(hits * cfg.scale, origin * cfg.scale, cfg, gen))
+    hist = run_shine_mapping_incremental(cfg, octree, decoder, frames)
+    assert len(hist) == 2, hist
+    for h in hist:
+        assert all(np.isfinite(h[k]) for k in ("loss_first", "loss_last", "eik_first", "eik_last")), h
+        # first step of a frame: the regulariser is 0 (features == last frame's), total = bce + weight_e * eikonal
+        assert abs(h["loss_first"] - (h["bce_first"] + h["eik_first"])) <= 1e-5 * abs(h["loss_first"]), h
+    assert calls == [True] * 40 + [False] * 40                        # frame 1: frozen decoder
+    assert not any(p.requires_grad for p in decoder.parameters())
 
 
 def test_capture_step_replays_the_eager_step():

@@ -6,8 +6,8 @@ import numpy as np
 import pytest
 import torch
 
-from tests.parity_utils import (DEC_KEYS, GOLDEN_NAMES, build_cuda_models, compare_step, load_golden, make_case,
-                                run_cuda_step, run_oracle_step, sort_case_morton)
+from tests.parity_utils import (DEC_KEYS, GOLDEN_NAMES, build_cuda_models, compare_step, load_eikonal_golden, load_golden,
+                                make_case, run_cuda_step, run_oracle_step, sort_case_morton)
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -209,35 +209,156 @@ def test_tcgen05_infer_matches_oracle(levels, n_batch):
     assert (pred - ref).abs().max() < 1e-5
 
 
-@pytest.mark.parametrize("levels,poly", [(2, True), (4, True), (3, False), (6, True)])
-def test_eikonal_through_class_surface_matches_oracle(levels, poly):
-    """ekional_loss_on (reference shine_batch.py:141-142,183-185): d pred / d coord with create_graph=True through
-    query_feature's coordinate-gradient kernels, and the second backward through the tangent kernels."""
+# ---- ekional_loss_on: the fused double-backward kernel (csrc/shine_eikonal.cu) and the class surface ------------------
+# Both are checked at the reference's weight_e = 0.1 (totals, the tolerances of the BCE tests) and, because the step is
+# linear in weight_e, the eikonal term on its own: (gradients at weight_e = W - gradients at weight_e = 0) / W against the
+# oracle's gradients of the eikonal mean alone, graded against that term's own maximum.  W (_eik_weight) is large enough
+# that the fp32 reordering of the BCE part, which does not cancel in the difference, stays far below that bar even where
+# the BCE part is a sum over the batch.  On freshly initialised tables
+# |g| ~ 1e-3 and the eikonal term is ~1e-3 of the total, so the totals alone could not see it; scaling the tables
+# (x300: median surface |g| ~0.6, a fifth of the samples above 1) puts |g| where a trained map has it.
+
+def _eikonal_case(levels, poly, seed, weighted=False, reduction="mean", scale=1.0, n=None, ordered=False, bias=True,
+                  n_batch=1500, feature_dim=8):
+    """n: keep the last n points of the batch (the 10 surface points and 6 stragglers make_case appends come last)."""
+    case = make_case(n_points=2000, n_batch=n_batch, feat_levels=levels, seed=seed, poly=poly, weighted=weighted,
+                     reduction=reduction, bias=bias, feature_dim=feature_dim)
+    if scale != 1.0:
+        case["tables"] = [(t * np.float32(scale)).astype(np.float32) for t in case["tables"]]
+    if n is not None:
+        for k in ("coord", "label", "weight"):
+            case[k] = np.ascontiguousarray(case[k][-n:])
+    return sort_case_morton(case) if ordered else case
+
+
+def _eik_weight(case):
+    return 100.0 * (case["coord"].shape[0] if case["cfg"]["reduction"] == "sum" else 1)
+
+
+def _oracle_eikonal(case, weight_e=0.1, n_surface=None):
     from oracle import shine_oracle as orc
+    from tests.parity_utils import oracle_from_case
+    o, odec = oracle_from_case(case)
+    c = case["cfg"]
+    r = orc.train_step_eikonal(o, odec, torch.from_numpy(case["coord"]), torch.from_numpy(case["label"]),
+                               torch.from_numpy(case["weight"]), c["sigma"], weight_e, c["weighted"], c["reduction"], n_surface)
+    out = {k: float(r[k]) for k in ("loss", "bce", "eikonal")}
+    out.update(g=r["g"].numpy(), pred=r["pred"].numpy(), table_grads=[t.numpy() for t in r["table_grads"]],
+               eik_table_grads=[t.numpy() for t in r["eik_table_grads"]],
+               dec_grads={k: v.numpy() for k, v in r["dec_grads"].items()},
+               eik_dec_grads={k: v.numpy() for k, v in r["eik_dec_grads"].items()})
+    return out
+
+
+def _grads(tr, frozen):
+    return ([t.cpu().numpy().copy() for t in tr.table_grads],
+            {} if frozen else {k: g.cpu().numpy().copy() for k, g in zip(DEC_KEYS, tr.dec_grads) if g is not None})
+
+
+def _fused_eikonal_runs(case, weights=None, frozen=False, outs=True):
+    """The fused step (SdfTrainer.forward_backward_eikonal, one launch) at each weight_e, on one trainer."""
+    from shine_mapping_b200 import SdfTrainer
+    cfg, octree, dec = build_cuda_models(case, DEV, freeze_decoder=frozen)
+    coord = torch.from_numpy(case["coord"]).to(DEV); label = torch.from_numpy(case["label"]).to(DEV)
+    weight = torch.from_numpy(case["weight"]).to(DEV)
+    n = coord.shape[0]
+    tr = SdfTrainer(cfg, octree, dec)
+    runs = {}
+    for w in weights or (0.1, 0.0, _eik_weight(case)):
+        cfg.weight_e = w
+        tr.zero_grad()
+        g = torch.full((n, 3), float("nan"), device=DEV) if outs else None
+        pred = torch.full((n,), float("nan"), device=DEV) if outs else None
+        bce, eik = tr.forward_backward_eikonal(coord, label, weight, pred_out=pred, grad_out=g)
+        torch.cuda.synchronize()
+        tg, dg = _grads(tr, frozen)
+        runs[w] = {"bce": float(bce), "eikonal": float(eik), "table_grads": tg, "dec_grads": dg,
+                   "g": g.cpu().numpy() if outs else None, "pred": pred.cpu().numpy() if outs else None}
+    if frozen:     # DEC_GRAD = false: the decoder segment of the flat buffer stays as zero_grad() left it
+        assert all(float(g.abs().max()) == 0.0 for g in tr.dec_grads if g is not None)
+        assert all(p.grad is None for p in dec.parameters())
+    return runs
+
+
+def _class_surface_eikonal_runs(case):
+    """The reference's autograd recipe on the class surface (coordinate-gradient and tangent kernels + torch MLP)."""
     from shine_mapping_b200 import SdfTrainer
     from shine_mapping_b200.batch_loop import eikonal_iteration
-    from tests.parity_utils import oracle_from_case
-    case = make_case(n_points=2000, n_batch=1500, feat_levels=levels, seed=100 + levels, poly=poly)
     cfg, octree, dec = build_cuda_models(case, DEV)
-    cfg.ekional_loss_on, cfg.weight_e = True, 0.1
+    cfg.ekional_loss_on = True
     coord = torch.from_numpy(case["coord"]).to(DEV); label = torch.from_numpy(case["label"]).to(DEV)
     weight = torch.from_numpy(case["weight"]).to(DEV)
     tr = SdfTrainer(cfg, octree, dec)
-    tr.zero_grad()
-    total, eik, g = eikonal_iteration(cfg, octree, dec, tr, coord, label, weight)
-    o, odec = oracle_from_case(case)
-    want = orc.train_step_eikonal(o, odec, torch.from_numpy(case["coord"]), torch.from_numpy(case["label"]),
-                                  torch.from_numpy(case["weight"]), case["cfg"]["sigma"], 0.1)
-    gw = want["g"].numpy()
-    assert np.abs(g.cpu().numpy() - gw).max() <= 1e-4 * np.abs(gw).max() + 1e-7
-    assert abs(float(eik) - float(want["eikonal"])) <= 1e-4 * abs(float(want["eikonal"])) + 1e-7
-    assert abs(float(total) - float(want["loss"])) <= 1e-4 * abs(float(want["loss"]))
+    runs = {}
+    for w in (0.1, 0.0, _eik_weight(case)):
+        cfg.weight_e = w
+        tr.zero_grad()
+        total, eik, g = eikonal_iteration(cfg, octree, dec, tr, coord, label, weight)
+        torch.cuda.synchronize()
+        tg, dg = _grads(tr, False)
+        runs[w] = {"bce": float(total) - w * float(eik), "eikonal": float(eik), "table_grads": tg, "dec_grads": dg,
+                   "g": g.cpu().numpy(), "pred": None}
+    return runs
+
+
+def _check_eikonal(runs, want, weight_e=0.1):
+    """runs: {weight_e: outputs} at weight_e, 0 and W.  want: the oracle's (or a golden's) outputs at weight_e with the
+    eikonal mean's own gradients.  Asserts parity; returns a line with the worst deviations, each relative to the
+    maximum it is graded against (bars: 1e-4 for g / eikonal / loss, 1e-3 for the gradients)."""
+    big = max(runs)
+    tot, r0, r1 = runs[weight_e], runs[0.0], runs[big]
+    worst = {}
+
+    def rel(name, got, exp, bound, floor=0.0):
+        got, exp = np.asarray(got, dtype=np.float64), np.asarray(exp, dtype=np.float64)
+        scale = float(np.abs(exp).max()) if exp.size else 0.0
+        d = float(np.abs(got - exp).max()) if exp.size else 0.0
+        assert d <= bound * scale + floor, f"{name}: max|d| {d:.3e} > {bound:g} x {scale:.3e} + {floor:.1e}"
+        if scale > 0:        # lout.bias has no eikonal part: graded by the floor alone
+            worst[name.split(" ")[0]] = max(worst.get(name.split(" ")[0], 0.0), d / scale)
+
+    if tot["g"] is not None:
+        rel("g", tot["g"], want["g"], 1e-4, 1e-7)
+    if tot["pred"] is not None:
+        assert np.all(np.abs(tot["pred"] - want["pred"]) <= 2e-5 + 1e-5 * np.abs(want["pred"]))
+    for r in (tot, r0, r1):
+        rel("eikonal", r["eikonal"], want["eikonal"], 1e-4, 1e-7)
+    rel("loss", tot["bce"] + weight_e * tot["eikonal"], want["loss"], 1e-4)
     for k, gt in enumerate(want["table_grads"]):
-        got = tr.table_grads[k].cpu().numpy()
-        assert np.abs(got - gt.numpy())[:-1].max() <= 1e-3 * np.abs(gt.numpy()).max() + 1e-9, k
-    for name, p in zip(DEC_KEYS, dec.fused_params()):
-        gt = want["dec_grads"][name].numpy()
-        assert np.abs(p.grad.cpu().numpy() - gt).max() <= 1e-3 * np.abs(gt).max() + 1e-9, name
+        rel(f"total_table level {k}", tot["table_grads"][k][:-1], gt[:-1], 1e-3, 1e-9)
+    for name, gt in want["dec_grads"].items():
+        if name in tot["dec_grads"]:
+            rel(f"total_dec {name}", tot["dec_grads"][name], gt, 1e-3, 1e-9)
+    # the eikonal term alone; what does not cancel between the two runs is fp32 reordering of the BCE part
+    for k, gt in enumerate(want["eik_table_grads"]):
+        base = r0["table_grads"][k][:-1]
+        rel(f"eik_table level {k}", (r1["table_grads"][k][:-1] - base) / big, gt[:-1], 1e-3,
+            1e-5 * float(np.abs(base).max()) / big + 1e-12)
+    for name, gt in want["eik_dec_grads"].items():
+        if name in r1["dec_grads"]:
+            base = r0["dec_grads"][name]
+            rel(f"eik_dec {name}", (r1["dec_grads"][name] - base) / big, gt, 1e-3,
+                1e-5 * float(np.abs(base).max()) / big + 1e-12)
+    return " ".join(f"{k}={v:.1e}" for k, v in worst.items())
+
+
+@pytest.mark.parametrize("levels,poly,feature_dim,scale,bias,weighted,reduction", [
+    pytest.param(2, True, 8, 1.0, True, False, "mean", id="2-True"),
+    pytest.param(4, True, 8, 1.0, True, False, "mean", id="4-True"),
+    pytest.param(3, False, 8, 1.0, True, False, "mean", id="3-False"),
+    pytest.param(6, True, 8, 1.0, True, False, "mean", id="6-True"),
+    pytest.param(3, True, 8, 300.0, True, True, "sum", id="3-True-weighted-sum-x300"),
+    pytest.param(2, False, 8, 300.0, False, True, "mean", id="2-False-nobias-weighted-mean-x300"),
+    # the coordinate-gradient and tangent kernels are generic in F
+    pytest.param(3, True, 4, 300.0, True, False, "mean", id="3-True-F4-x300"),
+    pytest.param(3, False, 16, 300.0, True, True, "sum", id="3-False-F16-weighted-sum-x300"),
+])
+def test_eikonal_through_class_surface_matches_oracle(levels, poly, feature_dim, scale, bias, weighted, reduction):
+    """ekional_loss_on (reference shine_batch.py:141-142,183-185): d pred / d coord with create_graph=True through
+    query_feature's coordinate-gradient kernels, and the second backward through the tangent kernels."""
+    case = _eikonal_case(levels, poly, 100 + levels + (0 if scale == 1.0 else 20 + feature_dim), weighted, reduction, scale,
+                         bias=bias, feature_dim=feature_dim)
+    print(_check_eikonal(_class_surface_eikonal_runs(case), _oracle_eikonal(case)))
 
 
 def test_eikonal_matches_reference_golden():
@@ -269,39 +390,128 @@ def test_eikonal_matches_reference_golden():
 
 
 def _fused_eikonal(case, weight_e):
+    runs = _fused_eikonal_runs(case, (weight_e,))[weight_e]
+    return runs, runs["bce"] + weight_e * runs["eikonal"], runs["eikonal"], runs["g"]
+
+
+@pytest.mark.parametrize("levels,poly,weighted,reduction,scale,n,ordered,frozen,bias,outs,seed", [
+    pytest.param(2, True, False, "mean", 1.0, None, False, False, True, True, 102, id="2-True"),
+    pytest.param(3, False, False, "mean", 1.0, None, False, False, True, True, 103, id="3-False"),
+    pytest.param(4, True, False, "mean", 1.0, None, False, False, True, True, 104, id="4-True"),
+    pytest.param(1, True, False, "mean", 300.0, None, False, False, True, True, 111, id="L1-x300"),
+    pytest.param(3, False, False, "mean", 300.0, None, False, False, True, True, 103, id="L3-linear-x300"),
+    pytest.param(4, True, True, "mean", 300.0, None, False, False, True, False, 114, id="L4-weighted-mean-x300"),
+    pytest.param(6, False, True, "sum", 300.0, None, False, False, True, True, 116, id="L6-linear-weighted-sum-x300"),
+    pytest.param(8, True, True, "mean", 300.0, None, False, False, True, True, 118, id="L8-weighted-mean-x300"),
+    pytest.param(2, True, True, "sum", 1.0, None, False, False, True, True, 112, id="L2-weighted-sum"),
+    pytest.param(4, True, False, "mean", 300.0, None, False, True, True, True, 124, id="L4-frozen-x300"),
+    pytest.param(2, False, False, "mean", 1.0, None, False, True, True, False, 122, id="L2-linear-frozen"),
+    pytest.param(3, True, False, "mean", 300.0, None, False, False, False, True, 133, id="L3-nobias-x300"),
+    pytest.param(2, False, True, "sum", 300.0, None, False, True, False, True, 132, id="L2-linear-nobias-frozen-x300"),
+    pytest.param(4, True, False, "mean", 300.0, None, True, False, True, True, 144, id="L4-morton-x300"),
+    pytest.param(3, False, True, "sum", 1.0, None, True, False, True, False, 143, id="L3-linear-morton-weighted-sum"),
+    pytest.param(2, True, False, "mean", 300.0, 1, False, False, True, True, 152, id="n1"),
+    pytest.param(3, False, False, "mean", 300.0, 31, False, False, True, True, 153, id="n31"),
+    pytest.param(2, True, True, "sum", 300.0, 33, False, False, True, False, 152, id="n33"),
+    pytest.param(4, True, False, "mean", 300.0, 129, False, False, True, True, 154, id="n129"),
+    # > 2 blocks/SM x 4 warps x 32 points: warps loop over several tiles of the grid-stride loop
+    pytest.param(4, True, True, "mean", 300.0, 60016, False, False, True, True, 164, id="n60016-x300"),
+])
+def test_fused_eikonal_step_matches_oracle(levels, poly, weighted, reduction, scale, n, ordered, frozen, bias, outs, seed):
+    """ONE launch (shine_sdf_bce_eikonal_step) against the oracle's autograd double backward, for every configuration
+    the kernel takes: 1..8 levels, poly / linear interpolation, weighted BCE with mean / sum, the frozen-decoder
+    instantiation (table gradients only), a decoder without biases, table scale 1 and x300, tile tails, the grid-stride
+    loop, a Morton-ordered batch (lanes of a warp hit the same rows), pred_out / grad_out passed or not."""
+    case = _eikonal_case(levels, poly, seed, weighted, reduction, scale, n=n, ordered=ordered, bias=bias,
+                         n_batch=60000 if (n or 0) > 10000 else 1500)
+    want = _oracle_eikonal(case)
+    if frozen:
+        want["dec_grads"], want["eik_dec_grads"] = {}, {}
+    surf = case["weight"] > 0
+    print(f"N={case['coord'].shape[0]} surface={int(surf.sum())} median|g|={np.median(np.linalg.norm(want['g'][surf], axis=1)):.3f}",
+          _check_eikonal(_fused_eikonal_runs(case, frozen=frozen, outs=outs), want))
+
+
+def test_fused_eikonal_step_without_surface_sample():
+    """No sample with weight > 0: the eikonal value is exactly 0 (as include/shine_b200.h documents; the reference's
+    torch mean over an empty selection would be NaN) and the gradients are those of the BCE-only step."""
+    case = _eikonal_case(3, True, 171, True, "mean", 300.0)
+    case["weight"] = -np.abs(case["weight"])
+    runs = _fused_eikonal_runs(case)
+    want = run_oracle_step(case)
+    for w, r in runs.items():
+        assert r["eikonal"] == 0.0, w
+        assert abs(r["bce"] - want["loss"]) <= 1e-4 * abs(want["loss"]), w
+        assert np.all(np.abs(r["pred"] - want["pred"]) <= 2e-5 + 1e-5 * np.abs(want["pred"])), w
+        for k, gt in enumerate(want["table_grads"]):
+            assert np.abs(r["table_grads"][k] - gt)[:-1].max() <= 2e-4 * np.abs(gt).max() + 1e-10, (w, k)
+        for k, gt in want["dec_grads"].items():
+            assert np.abs(r["dec_grads"][k] - gt).max() <= 2e-4 * np.abs(gt).max() + 1e-10, (w, k)
+        for k in range(len(want["table_grads"])):       # weight_e does not enter: the same kernel arithmetic every time
+            assert np.abs(r["table_grads"][k] - runs[0.0]["table_grads"][k]).max() <= 1e-6 * np.abs(want["table_grads"][k]).max()
+
+
+def test_fused_eikonal_step_surface_samples_that_miss_every_level():
+    """Surface samples outside the map: g = 0, so each adds (1 - 0)^2 = 1 to the mean and nothing to the gradients
+    (torch's d|g|/dg is 0 at g = 0)."""
+    case = _eikonal_case(3, False, 172, scale=300.0)
+    rng = np.random.default_rng(11)
+    far = rng.uniform(0.6, 0.9, size=(77, 3)).astype(np.float32)
+    case["coord"] = np.concatenate([case["coord"], far])
+    case["label"] = np.concatenate([case["label"], np.zeros(77, np.float32)])
+    case["weight"] = np.concatenate([case["weight"], np.ones(77, np.float32)])
+    want = _oracle_eikonal(case)
+    runs = _fused_eikonal_runs(case)
+    assert np.all(want["g"][-77:] == 0.0) and np.all(runs[0.1]["g"][-77:] == 0.0)
+    n_surf = int((case["weight"] > 0).sum())
+    assert want["eikonal"] >= 77.0 / n_surf
+    print(_check_eikonal(runs, want))
+
+
+def test_fused_eikonal_shards_add_up_to_the_global_batch():
+    """A batch in two uneven parts accumulated into one trainer, with n_norm and n_surface of the whole batch, gives the
+    full batch's gradients, and the two eikonal values add up to its mean: what a rank of a data-parallel run computes."""
     from shine_mapping_b200 import SdfTrainer
+    case = _eikonal_case(3, True, 181, scale=300.0, n_batch=3000)
+    want = _oracle_eikonal(case, weight_e=1.0)
     cfg, octree, dec = build_cuda_models(case, DEV)
-    cfg.ekional_loss_on, cfg.weight_e = True, weight_e
+    cfg.weight_e = 1.0
     coord = torch.from_numpy(case["coord"]).to(DEV); label = torch.from_numpy(case["label"]).to(DEV)
     weight = torch.from_numpy(case["weight"]).to(DEV)
+    n, n_surf = coord.shape[0], int((case["weight"] > 0).sum())
     tr = SdfTrainer(cfg, octree, dec)
     tr.zero_grad()
-    g = torch.empty(coord.shape[0], 3, device=DEV)
-    bce, eik = tr.forward_backward_eikonal(coord, label, weight, grad_out=g)
+    bce = eik = 0.0
+    for sl in (slice(0, 2 * n // 5), slice(2 * n // 5, n)):
+        b, e = tr.forward_backward_eikonal(coord[sl], label[sl], weight[sl], n_norm=n, n_surface=n_surf)
+        bce, eik = bce + float(b), eik + float(e)
     torch.cuda.synchronize()
-    return tr, dec, float(bce) + weight_e * float(eik), float(eik), g.cpu().numpy()
+    parts = _grads(tr, False)
+    tr.zero_grad()
+    b, e = tr.forward_backward_eikonal(coord, label, weight)
+    torch.cuda.synchronize()
+    full = _grads(tr, False)
+    assert abs(eik - float(e)) <= 1e-5 * abs(float(e)) and abs(bce - float(b)) <= 1e-5 * abs(float(b))
+    assert abs(eik - want["eikonal"]) <= 1e-4 * want["eikonal"]
+    assert abs(bce + eik - want["loss"]) <= 1e-4 * want["loss"]
+    for got, ful, gt in zip(parts[0], full[0], want["table_grads"]):
+        assert np.abs(got - ful)[:-1].max() <= 1e-5 * np.abs(ful).max()
+        assert np.abs(got - gt)[:-1].max() <= 1e-3 * np.abs(gt).max()
+    for k, gt in want["dec_grads"].items():
+        assert np.abs(parts[1][k] - full[1][k]).max() <= 1e-5 * np.abs(full[1][k]).max(), k
+        assert np.abs(parts[1][k] - gt).max() <= 1e-3 * np.abs(gt).max(), k
 
 
-@pytest.mark.parametrize("levels,poly", [(2, True), (3, False), (4, True)])
-def test_fused_eikonal_step_matches_oracle(levels, poly):
-    """ONE launch (shine_sdf_bce_eikonal_step) against the oracle's autograd double backward."""
-    from oracle import shine_oracle as orc
-    from tests.parity_utils import oracle_from_case
-    case = make_case(n_points=2000, n_batch=1500, feat_levels=levels, seed=100 + levels, poly=poly)
-    tr, dec, total, eik, g = _fused_eikonal(case, 0.1)
-    o, odec = oracle_from_case(case)
-    want = orc.train_step_eikonal(o, odec, torch.from_numpy(case["coord"]), torch.from_numpy(case["label"]),
-                                  torch.from_numpy(case["weight"]), case["cfg"]["sigma"], 0.1)
-    gw = want["g"].numpy()
-    assert np.abs(g - gw).max() <= 1e-4 * np.abs(gw).max() + 1e-7
-    assert abs(eik - float(want["eikonal"])) <= 1e-4 * abs(float(want["eikonal"])) + 1e-7
-    assert abs(total - float(want["loss"])) <= 1e-4 * abs(float(want["loss"]))
-    for k, gt in enumerate(want["table_grads"]):
-        got = tr.table_grads[k].cpu().numpy()
-        assert np.abs(got - gt.numpy())[:-1].max() <= 1e-3 * np.abs(gt.numpy()).max() + 1e-9, k
-    for name, gd in zip(DEC_KEYS, tr.dec_grads):
-        gt = want["dec_grads"][name].numpy()
-        assert np.abs(gd.cpu().numpy() - gt).max() <= 1e-3 * np.abs(gt).max() + 1e-9, name
+def test_fused_eikonal_step_matches_scaled_reference_golden():
+    """The fused entry against the reference's own classes on tables scaled x500 (median surface |g| ~1), weighted BCE
+    with sum reduction (tests/golden/ref_eikonal_l3_sum_weighted.npz, which also holds the eikonal mean's own gradients)."""
+    case, z = load_eikonal_golden("ref_eikonal_l3_sum_weighted")
+    w = case["cfg"]["weight_e"]
+    L = case["cfg"]["tree_level_feat"]
+    want = {"g": z["exp_g"], "pred": z["exp_pred"], "eikonal": float(z["exp_eikonal"]), "loss": float(z["exp_loss"]),
+            "table_grads": [z[f"exp_tgrad_{k}"] for k in range(L)], "eik_table_grads": [z[f"exp_eik_tgrad_{k}"] for k in range(L)],
+            "dec_grads": {k: z["exp_dgrad_" + k] for k in DEC_KEYS}, "eik_dec_grads": {k: z["exp_eik_dgrad_" + k] for k in DEC_KEYS}}
+    print(_check_eikonal(_fused_eikonal_runs(case, (w, 0.0, _eik_weight(case))), want, w))
 
 
 def test_fused_eikonal_step_matches_reference_golden_and_beats_class_surface():
@@ -316,16 +526,16 @@ def test_fused_eikonal_step_matches_reference_golden_and_beats_class_surface():
     cfg_j = json.loads(str(z["cfg_json"]))
     case = {"cfg": cfg_j, "frames": [z["frame_0"]], "tables": [z[f"table_{k}"] for k in range(cfg_j["tree_level_feat"])],
             "dec": {k: z["dec_" + k] for k in DEC_KEYS}, "coord": z["coord"], "label": z["label"], "weight": z["weight"]}
-    tr, dec, total, eik, g = _fused_eikonal(case, cfg_j["weight_e"])
+    run, total, eik, g = _fused_eikonal(case, cfg_j["weight_e"])
     assert np.abs(g - z["exp_g"]).max() <= 1e-4 * np.abs(z["exp_g"]).max() + 1e-7
     assert abs(eik - float(z["exp_eikonal"])) <= 1e-4 * abs(float(z["exp_eikonal"]))
     assert abs(total - float(z["exp_loss"])) <= 1e-4 * abs(float(z["exp_loss"]))
     for k in range(cfg_j["tree_level_feat"]):
         want = z[f"exp_tgrad_{k}"]
-        assert np.abs(tr.table_grads[k].cpu().numpy() - want)[:-1].max() <= 1e-3 * np.abs(want).max() + 1e-9
-    for name, gd in zip(DEC_KEYS, tr.dec_grads):
+        assert np.abs(run["table_grads"][k] - want)[:-1].max() <= 1e-3 * np.abs(want).max() + 1e-9
+    for name, gd in run["dec_grads"].items():
         want = z["exp_dgrad_" + name]
-        assert np.abs(gd.cpu().numpy() - want).max() <= 1e-3 * np.abs(want).max() + 1e-9
+        assert np.abs(gd - want).max() <= 1e-3 * np.abs(want).max() + 1e-9
     # timing at the KITTI batch size (config/kitti/kitti_batch.yaml: batch_size 16384)
     big = make_case(n_points=3000, n_batch=16384, feat_levels=4, seed=7)
     cfg, octree, dec2 = build_cuda_models(big, DEV)
@@ -483,7 +693,8 @@ def _trainer_step(case, tcgen05, freeze=False):
         "feature": octree.query_feature(coord).detach().cpu().numpy(),
         "pred": pred.cpu().numpy(), "loss": float(loss),
         "table_grads": [g.detach().cpu().numpy().copy() for g in tr.table_grads],
-        "dec_grads": {} if freeze else {k: g.detach().cpu().numpy().copy() for k, g in zip(DEC_KEYS, tr.dec_grads)},
+        "dec_grads": {} if freeze else {k: g.detach().cpu().numpy().copy() for k, g in zip(DEC_KEYS, tr.dec_grads)
+                                        if g is not None},
     }
 
 
@@ -508,6 +719,32 @@ def test_tcgen05_train_step_frozen_decoder():
     want = run_oracle_step(case)
     want["dec_grads"] = {}
     print(compare_step(got, want))
+
+
+def test_biasless_decoder_matches_oracle():
+    """geo_mlp_bias_on: False — every fused kernel reads the biases through null-pointer branches: the general and the
+    grouped (Morton-ordered) kernels of sdf_bce_step, its two-pass mode, the wgmma training kernel, and both inference
+    kernels."""
+    from shine_mapping_b200 import sdf_infer
+    from tests.parity_utils import drop_relu_kink_points
+    case = make_case(n_points=2500, n_batch=3000, feat_levels=3, seed=57, weighted=True, reduction="sum", bias=False)
+    case, dropped = drop_relu_kink_points(case)
+    want = run_oracle_step(case)
+    assert sorted(want["dec_grads"]) == ["layers.0.weight", "layers.1.weight", "lout.weight"]
+    print("general", compare_step(run_cuda_step(case, DEV), want))
+    print("two-pass", compare_step(run_cuda_step(case, DEV, single_pass=False), want))
+    want_f = dict(want); want_f["dec_grads"] = {}
+    print("frozen", compare_step(run_cuda_step(case, DEV, freeze_decoder=True), want_f))
+    ordered = sort_case_morton(case)
+    print("grouped", compare_step(run_cuda_step(ordered, DEV, morton_ordered=True), run_oracle_step(ordered)))
+    print("wgmma train", compare_step(_trainer_step(case, True), want))
+    cfg, octree, dec = build_cuda_models(case, DEV)
+    assert all(p is None for p in dec.fused_params()[1::2])
+    coord = torch.from_numpy(case["coord"]).to(DEV)
+    for tc in (False, True):
+        pred = sdf_infer(octree, dec, coord, tcgen05=tc)
+        torch.cuda.synchronize()
+        assert np.abs(pred.cpu().numpy() - want["pred"]).max() < 2e-5, tc
 
 
 def test_two_queries_before_one_backward():

@@ -4,7 +4,8 @@ import numpy as np
 import pytest
 import torch
 
-from tests.parity_utils import GOLDEN_NAMES, compare_step, load_golden, oracle_from_case, run_oracle_step, orc
+from tests.parity_utils import (DEC_KEYS, GOLDEN_NAMES, compare_step, load_eikonal_golden, load_golden, oracle_from_case,
+                                orc, run_oracle_step)
 
 
 @pytest.mark.parametrize("name", GOLDEN_NAMES)
@@ -86,16 +87,22 @@ def test_raises_without_featured_level():
 def test_oracle_eikonal_matches_reference_golden():
     """ekional_loss_on: d pred / d coord with create_graph=True on the reference's own classes (golden minted by
     oracle/make_golden.py::make_eikonal) vs the oracle's train_step_eikonal."""
-    import json
-    import os
-    from tests.parity_utils import DEC_KEYS, GOLDEN_DIR
-    z = np.load(os.path.join(GOLDEN_DIR, "ref_eikonal_l3.npz"))
-    cfg = json.loads(str(z["cfg_json"]))
-    case = {"cfg": cfg, "frames": [z["frame_0"]], "tables": [z[f"table_{k}"] for k in range(cfg["tree_level_feat"])],
-            "dec": {k: z["dec_" + k] for k in DEC_KEYS}, "coord": z["coord"], "label": z["label"], "weight": z["weight"]}
+    _check_oracle_against_eikonal_golden("ref_eikonal_l3")
+
+
+def test_oracle_eikonal_matches_scaled_reference_golden():
+    """The same on ref_eikonal_l3_sum_weighted: tables scaled x500 (median surface |g| ~1), weighted BCE with sum
+    reduction, and the eikonal mean's own gradients (beside a summed BCE its share of the total is small)."""
+    _check_oracle_against_eikonal_golden("ref_eikonal_l3_sum_weighted")
+
+
+def _check_oracle_against_eikonal_golden(name):
+    case, z = load_eikonal_golden(name)
+    cfg = case["cfg"]
     o, dec = oracle_from_case(case)
     got = orc.train_step_eikonal(o, dec, torch.from_numpy(z["coord"]), torch.from_numpy(z["label"]),
-                                 torch.from_numpy(z["weight"]), cfg["sigma"], cfg["weight_e"])
+                                 torch.from_numpy(z["weight"]), cfg["sigma"], cfg["weight_e"], cfg["weighted"],
+                                 cfg["reduction"])
     assert np.abs(got["g"].numpy() - z["exp_g"]).max() <= 1e-5 * np.abs(z["exp_g"]).max()
     assert abs(float(got["eikonal"]) - float(z["exp_eikonal"])) <= 1e-5 * abs(float(z["exp_eikonal"]))
     assert abs(float(got["loss"]) - float(z["exp_loss"])) <= 1e-6 * abs(float(z["exp_loss"]))
@@ -105,3 +112,11 @@ def test_oracle_eikonal_matches_reference_golden():
     for k in DEC_KEYS:
         want = z["exp_dgrad_" + k]
         assert np.abs(got["dec_grads"][k].numpy() - want).max() <= 1e-4 * np.abs(want).max() + 1e-12
+    if "exp_eik_tgrad_0" not in z.files:
+        return
+    for k, g in enumerate(got["eik_table_grads"]):
+        want = z[f"exp_eik_tgrad_{k}"]
+        assert np.abs(g.numpy() - want).max() <= 1e-4 * np.abs(want).max() + 1e-12, k
+    for k in DEC_KEYS:
+        want = z["exp_eik_dgrad_" + k]
+        assert np.abs(got["eik_dec_grads"][k].numpy() - want).max() <= 1e-4 * np.abs(want).max() + 1e-12, k
