@@ -319,3 +319,46 @@ def train_step_eikonal(octree: OracleOctree, dec: dict, coord, label, weight, si
             "table_grads": [f.grad if f.grad is not None else torch.zeros_like(f) for f in octree.hier_features],
             "dec_grads": {k: (p.grad if p.grad is not None else torch.zeros_like(p)) for k, p in dec.items()},
             "bce_table_grads": bce_t, "bce_dec_grads": bce_d, "eik_table_grads": eik_t, "eik_dec_grads": eik_d}
+
+
+# --------------------------------------------------------------------------------------------------
+# the optimizer: utils/tools.py:57-83 (setup_optimizer) and torch.optim.Adam (shine_batch.py:210 `opt.step()`)
+# --------------------------------------------------------------------------------------------------
+
+
+def reference_param_groups(L: int, lr: float, weight_decay: float, lr_level_reduce_ratio: float):
+    """setup_optimizer (utils/tools.py:57-83) without the semantic / ray-loss groups: the geometry decoder at `lr`
+    with weight decay, then one group per table level, leaf first (hier_features[L - 1]), the lr multiplied by
+    lr_level_reduce_ratio per level towards the coarse end, no decay.
+    -> [{"params": "decoder" | table index into hier_features, "lr", "weight_decay"}, ...]"""
+    groups = [{"params": "decoder", "lr": lr, "weight_decay": weight_decay}]
+    lr_cur = lr
+    for i in range(L):
+        groups.append({"params": L - i - 1, "lr": lr_cur, "weight_decay": 0.0})
+        lr_cur *= lr_level_reduce_ratio
+    return groups
+
+
+def adam_reference(params, grads, exp_avg, exp_avg_sq, step: int, lr: float, weight_decay: float,
+                   betas=(0.9, 0.99), eps: float = 1e-15):
+    """One step of torch.optim.Adam (amsgrad off, L2 weight decay added to the gradient) for the tensors of one
+    parameter group, in float64.  `step` is the step number after this update (1 for the first).  Inputs are not
+    modified.  -> (params, exp_avg, exp_avg_sq) after the step, float64 tensors (lists when lists were given)."""
+    single = torch.is_tensor(params)
+    if single:
+        params, grads, exp_avg, exp_avg_sq = [params], [grads], [exp_avg], [exp_avg_sq]
+    b1, b2 = float(betas[0]), float(betas[1])
+    bc1 = 1.0 - b1 ** step
+    bc2_sqrt = (1.0 - b2 ** step) ** 0.5
+    out_p, out_m, out_v = [], [], []
+    for p, g, m, v in zip(params, grads, exp_avg, exp_avg_sq):
+        p, g, m, v = (t.detach().to(torch.float64) for t in (p, g, m, v))
+        if weight_decay != 0.0:
+            g = g + weight_decay * p
+        m = b1 * m + (1.0 - b1) * g
+        v = b2 * v + (1.0 - b2) * g * g
+        p = p - (lr / bc1) * m / (v.sqrt() / bc2_sqrt + eps)
+        out_p.append(p); out_m.append(m); out_v.append(v)
+    if single:
+        return out_p[0], out_m[0], out_v[0]
+    return out_p, out_m, out_v

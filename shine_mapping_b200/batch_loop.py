@@ -107,7 +107,6 @@ class _GraphedIteration:
         tr = self.trainer
         if self.graph is None or self.lr != tr.lr:
             dev = tr.flat_grad.device
-            tr._sync_adam_state()             # other paths (train_step, eikonal loop) count on the host only
             side = torch.cuda.Stream(device=dev)
             side.wait_stream(torch.cuda.current_stream(dev))
             with torch.cuda.stream(side):     # warm-up outside capture (lazy inits, allocator)
@@ -119,8 +118,7 @@ class _GraphedIteration:
                 self._body()
             self.lr = tr.lr
             return        # the warm-up call above did this iteration's work; capturing does not execute anything
-        self.graph.replay()
-        tr.step_count += 1    # keep the host-side count in step with the device counter the replayed Adam uses
+        tr._replay_with_adam(self.graph)
 
 
 def run_shine_mapping_batch(config: SHINEConfig, octree: FeatureOctree, decoder: Decoder, pool, iters=None,

@@ -1876,6 +1876,18 @@ int shine_reduce_grad_replicas(const shine_octree* oct, void* stream) {
     return (int)cudaGetLastError();
 }
 
+// every argument is checked before anything is launched: a rejected shine_adam_step_dev leaves its step counter alone
+static int adam_check(const shine_adam_tensor* tensors, int32_t count) {
+    if (!tensors || count < 1 || count > SHINE_ADAM_MAX_TENSORS) return SHINE_ERR_INVALID_ARG;
+    for (int i = 0; i < count; ++i) {
+        const shine_adam_tensor& t = tensors[i];
+        if (!t.param || !t.grad || !t.exp_avg || !t.exp_avg_sq || t.numel < 0) return SHINE_ERR_INVALID_ARG;
+        if ((((uintptr_t)t.param | (uintptr_t)t.grad | (uintptr_t)t.exp_avg | (uintptr_t)t.exp_avg_sq) & 15) != 0)
+            return SHINE_ERR_INVALID_ARG;
+    }
+    return SHINE_OK;
+}
+
 static int adam_launch(const shine_adam_tensor* tensors, int32_t count, float beta1, float beta2, float eps, int32_t step,
                        const float* bc_dev, int32_t zero_grad, cudaStream_t st) {
     AdamParams A;
@@ -1883,9 +1895,6 @@ static int adam_launch(const shine_adam_tensor* tensors, int32_t count, float be
     int64_t max_n = 0;
     for (int i = 0; i < count; ++i) {
         const shine_adam_tensor& t = tensors[i];
-        if (!t.param || !t.grad || !t.exp_avg || !t.exp_avg_sq || t.numel < 0) return SHINE_ERR_INVALID_ARG;
-        if ((((uintptr_t)t.param | (uintptr_t)t.grad | (uintptr_t)t.exp_avg | (uintptr_t)t.exp_avg_sq) & 15) != 0)
-            return SHINE_ERR_INVALID_ARG;
         A.t[i] = t;
         if (t.numel > max_n) max_n = t.numel;
     }
@@ -1904,13 +1913,15 @@ static int adam_launch(const shine_adam_tensor* tensors, int32_t count, float be
 
 int shine_adam_step(const shine_adam_tensor* tensors, int32_t count, float beta1, float beta2, float eps, int32_t step,
                     int32_t zero_grad, void* stream) {
-    if (!tensors || count < 1 || count > SHINE_ADAM_MAX_TENSORS || step < 1) return SHINE_ERR_INVALID_ARG;
+    if (step < 1) return SHINE_ERR_INVALID_ARG;
+    if (int rc = adam_check(tensors, count)) return rc;
     return adam_launch(tensors, count, beta1, beta2, eps, step, nullptr, zero_grad, (cudaStream_t)stream);
 }
 
 int shine_adam_step_dev(const shine_adam_tensor* tensors, int32_t count, float beta1, float beta2, float eps,
                         void* state, int32_t zero_grad, void* stream) {
-    if (!tensors || count < 1 || count > SHINE_ADAM_MAX_TENSORS || !state) return SHINE_ERR_INVALID_ARG;
+    if (!state) return SHINE_ERR_INVALID_ARG;
+    if (int rc = adam_check(tensors, count)) return rc;
     AdamDevState* st = reinterpret_cast<AdamDevState*>(state);
     DeviceGuard guard(state);
     adam_bump_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(st, beta1, beta2);

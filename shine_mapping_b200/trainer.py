@@ -92,6 +92,7 @@ class SdfTrainer:
         self.exp_avg_sq = torch.zeros(total, dtype=torch.float32, device=dev)
         self.step_count = 0   # fresh Adam state, like a rebuilt torch optimizer
         self.adam_state = torch.zeros(3, dtype=torch.int32, device=dev)   # {step, bc1, bc2_sqrt} for graph replay
+        self._device_steps = 0   # what adam_state[0] holds (host-step Adam advances step_count alone)
         views = []
         for p, o, s in zip(tables + dec, offs, sizes):
             views.append(self.flat_grad[o:o + s].view(p.shape) if p is not None else None)
@@ -233,7 +234,10 @@ class SdfTrainer:
         cfg = self.config
         tables, dec = self._params()
         capturing = torch.cuda.is_current_stream_capturing()
-        if not capturing:             # a captured call executes nothing: whoever replays the graph bumps the count
+        if not capturing:             # a captured call executes nothing: whoever replays the graph counts its step
+            if device_step:
+                self._align_device_step()
+                self._device_steps += 1
             self.step_count += 1
         entries = []
         L = len(tables)
@@ -265,10 +269,21 @@ class SdfTrainer:
                                               1 if zero_grad else 0, _abi.stream_ptr(tables[0].device)),
                    "shine_adam_step")
 
-    def _sync_adam_state(self):
-        """The host step_count is the single source of truth: write it to the device-side Adam state (the bump kernel
-        recomputes the bias corrections from the step number on every call)."""
-        self.adam_state[0] = max(int(self.step_count), 0)
+    def _align_device_step(self):
+        """The host step_count is the single source of truth.  Host-step Adam advances it alone, so before a device-step
+        Adam runs (eagerly or in a replayed graph) the device counter is set to it (the bump kernel recomputes the bias
+        corrections from the step number on every call).  While only device-step Adam runs, as in the graphed loop,
+        the two agree and this launches nothing."""
+        if self._device_steps != self.step_count:
+            self.adam_state[0] = self.step_count
+            self._device_steps = self.step_count
+
+    def _replay_with_adam(self, graph):
+        """Replay a CUDA graph that holds one device-step Adam, counted like an eager call."""
+        self._align_device_step()
+        graph.replay()
+        self._device_steps += 1
+        self.step_count += 1
 
     def train_step(self, coord, sdf_label, weight=None, n_norm=None):
         """shine_batch.py:123-210: fwd + loss + bwd (+ all-reduce when data parallel) + Adam."""
@@ -310,11 +325,14 @@ class SdfTrainer:
     class StepGraph:
         """One whole step on device tensors as a CUDA graph (see `capture_step`)."""
 
-        def __init__(self, trainer, graph, launches):
-            self.trainer, self.graph, self.launches = trainer, graph, launches
+        def __init__(self, trainer, graph, launches, optimizer):
+            self.trainer, self.graph, self.launches, self.optimizer = trainer, graph, launches, optimizer
 
         def replay(self):
-            self.graph.replay()
+            if self.optimizer:
+                self.trainer._replay_with_adam(self.graph)
+            else:
+                self.graph.replay()
             self.trainer._loss_clean = False
             _abi.LAUNCHES["count"] += self.launches       # the replayed kernels are this library's launches too
             return self.trainer.loss
@@ -335,8 +353,6 @@ class SdfTrainer:
             if optimizer:
                 self.optimizer_step(zero_grad=False, device_step=True)
 
-        if optimizer:
-            self._sync_adam_state()
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(side):
@@ -349,7 +365,7 @@ class SdfTrainer:
             body()
         launches = _abi.LAUNCHES["count"] - before
         _abi.LAUNCHES["count"] = before                  # capturing launched nothing
-        return SdfTrainer.StepGraph(self, graph, launches)
+        return SdfTrainer.StepGraph(self, graph, launches, optimizer)
 
     class HostStepHandle:
         """Result of `submit_host_step`: `.result()` blocks until that step's loss is on the host."""
@@ -450,9 +466,8 @@ class SdfTrainer:
             with torch.cuda.graph(graph):
                 self._host_step_body(coord_h, label_h, weight_h, n, chunks, weighted, optimizer)
             self._host_graphs[key] = graph
-            if optimizer:             # bring the device counter back in line with the host one after the warm-up
-                self._sync_adam_state()
-        graph.replay()
         if optimizer:
-            self.step_count += 1      # the replayed Adam advanced the device-side step counter
+            self._replay_with_adam(graph)
+        else:
+            graph.replay()
         return float(self.loss.item())
