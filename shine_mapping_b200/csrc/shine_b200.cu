@@ -57,7 +57,7 @@
 // The per-point training kernels with decoder gradients keep 56 accumulators per lane live through the whole tile: at 2
 // blocks/SM (128 registers) they spill ~0.5 KB per thread, at 1 block/SM (255) they do not, and on H100 the spill-free
 // build is faster (C2 batch in the order drawn, kernel: 0.460 vs 0.564 ms).  The grouped kernel timed on Morton-ordered batches
-// spills ~0.3 KB at 2 blocks/SM and is still faster there than at 1 (0.228 vs 0.252 ms): it keeps SHINE_TRAIN_MINB.
+// splits the weight-gradient contraction across the block (block-wide rounds) and fits SHINE_TRAIN_MINB without spilling.
 #ifndef SHINE_TRAIN_DECGRAD_MINB
 #define SHINE_TRAIN_DECGRAD_MINB 1
 #endif
@@ -323,9 +323,24 @@ __device__ __forceinline__ void from_cfrag(const float (&c)[4], int odd, float (
     else      { v[0] = r0;   v[1] = r1;   v[2] = c[2]; v[3] = c[3]; }
 }
 
-// decoder-gradient accumulators of a lane (mma.sync C fragments): dW2[2][4][4], dW1[2][4], and the per-column partial
-// sums of db2, db1, dw3 ([4][2]: columns 8j + 2t + q)
+// Sums 24 per-lane values over the 8 lanes of equal t (lane bits 2-4) and leaves lane (g, t) the sums of slots 3g .. 3g+2:
+// a butterfly that halves the values it keeps at each step (21 shuffles instead of 72 for a full all-reduce).
+__device__ __forceinline__ void reduce_scatter_g(const float (&v)[24], float (&out)[3], int lane) {
+    float a[12], b[6];
+    const bool b4 = (lane & 16) != 0, b3 = (lane & 8) != 0, b2 = (lane & 4) != 0;
+#pragma unroll
+    for (int i = 0; i < 12; ++i) a[i] = (b4 ? v[12 + i] : v[i]) + __shfl_xor_sync(kFull, b4 ? v[i] : v[12 + i], 16);
+#pragma unroll
+    for (int i = 0; i < 6; ++i) b[i] = (b3 ? a[6 + i] : a[i]) + __shfl_xor_sync(kFull, b3 ? a[i] : a[6 + i], 8);
+#pragma unroll
+    for (int i = 0; i < 3; ++i) out[i] = (b2 ? b[3 + i] : b[i]) + __shfl_xor_sync(kFull, b2 ? b[i] : b[3 + i], 4);
+}
+
+// decoder-gradient accumulators of a lane in the per-point kernels (mma.sync C fragments): dW2[2][4][4], dW1[2][4], and the
+// per-column partial sums of db2, db1, dw3 ([4][2]: columns 8j + 2t + q)
 #define SHINE_ACC_DECL float dW2[2][4][4], dW1[2][4], db2p[4][2], db1p[4][2], dw3p[4][2]
+
+__device__ __forceinline__ void round_bar(int id) { asm volatile("bar.sync %0, 256;" ::"r"(id) : "memory"); }
 
 // ------------------------------------------------------------------------------------------------------
 // the fused kernel: hash walk + gather + blend + MLP (+ BCE loss) (+ full backward with scatter-add)
@@ -346,7 +361,8 @@ struct SmemPlan {
     static constexpr int W3 = B2 + kH;
     static constexpr int B3 = W3 + kH;                 // [1] (+3 pad)
     static constexpr int kDecGradFloats = kH * kF + kH + kH * kH + kH + kH + 1;   // 1377 (a warp's partial goes to its staging area)
-    static constexpr int PRE = B3 + 4;                 // per-warp input prefetch: [16][3] coord | [16] label | [16] weight
+    static constexpr int RND = B3 + 4;                 // [8] per warp: 1 if its tile of the current round is staged
+    static constexpr int PRE = RND + 8;                // per-warp input prefetch: [16][3] coord | [16] label | [16] weight
     static constexpr int kPrePerWarp = 5 * kTile;
     static constexpr int STAGE = PRE + 8 * kPrePerWarp;   // per-warp staging: 3 x [16][kWS] + [16][8]
     static constexpr int kStagePerWarp = 3 * kTile * kWS + kTile * kF;   // dh2 | h1 | dh1 | feat tiles
@@ -480,6 +496,7 @@ template <int NTF, bool TRAIN, bool DEC_GRAD, int LMAX, bool GROUPED = false>
 __global__ void __launch_bounds__(256, !TRAIN ? SHINE_INFER_MINB : (DEC_GRAD && !GROUPED) ? SHINE_TRAIN_DECGRAD_MINB : SHINE_TRAIN_MINB)
 sdf_fused_kernel(const __grid_constant__ StepParams P) {
     static_assert(!GROUPED || TRAIN, "the grouped scatter belongs to the training kernels");
+    static_assert(!DEC_GRAD || TRAIN, "decoder gradients belong to the training kernels");
     static_assert(SmemPlan::kStagePerWarp >= SmemPlan::kDecGradFloats, "a warp's staging area holds its partial decoder gradient");
     extern __shared__ __align__(16) float smem[];
     uint32_t* smu = reinterpret_cast<uint32_t*>(smem);
@@ -509,6 +526,7 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
     constexpr int kPark = LMAX <= 4 ? 16 : 32;                           // blend factors of every level, per lane
     constexpr int kIdPark = 4 * LMAX;                                    // this lane's 4 corner rows of every level
     __syncthreads();
+    // Decoder gradients, per-point kernels: every warp accumulates the whole gradient over its own tiles (SHINE_ACC_DECL).
     SHINE_ACC_DECL;
 #pragma unroll
     for (int a = 0; a < 2; ++a) {
@@ -518,6 +536,16 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
     }
 #pragma unroll
     for (int j = 0; j < 4; ++j) { db2p[j][0] = db2p[j][1] = db1p[j][0] = db1p[j][1] = dw3p[j][0] = dw3p[j][1] = 0.f; }
+    // Grouped kernel (kRounds): the block's warps advance in rounds of one tile each; a round's staged operands are
+    // contracted by the whole block, each warp owning a slice of the outputs (K = the up to 128 points of the round), so that
+    // the kernel fits 2 blocks/SM without spilling.  (At 1 block/SM, the per-point kernels lose more to the round
+    // barriers than they gain: C2 batch in the order drawn, kernel 0.56 vs 0.46 ms on H100.)
+    //   dW2 [32 x 32]: m16n8 fragment (warp >> 2, warp & 3), over every staged tile;
+    //   dW1 [32 x 8]:  m16n8 fragment warp & 1, over the tiles 2 (warp >> 1) and 2 (warp >> 1) + 1 (4 partial sums each);
+    //   db1, db2, dw3: this warp's own tiles, reduced per tile to 3 columns per lane (reduce_scatter_g); db3: lane sums.
+    float dW2acc[4] = {0.f, 0.f, 0.f, 0.f}, dW1acc[4] = {0.f, 0.f, 0.f, 0.f};
+    float vecacc[3] = {0.f, 0.f, 0.f};
+    constexpr bool kRounds = DEC_GRAD && GROUPED;
 
     constexpr bool kSectorProbe = TRAIN ? (SHINE_SECTOR_PROBE_TRAIN != 0) : (SHINE_SECTOR_PROBE_INFER != 0);
     constexpr bool kSlotPrefetch = TRAIN && !kSectorProbe && (SHINE_SLOT_PREFETCH != 0) && (SHINE_CPASYNC_PREFETCH == 0);
@@ -539,6 +567,53 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
     float* gpt = smem + SmemPlan::STAGE + (DEC_GRAD ? 8 * SmemPlan::kStagePerWarp : 0) +
                  warp * (LMAX * SmemPlan::kGroupPerLevel + (DEC_GRAD ? 0 : kTile * kF));
     float* gdx = DEC_GRAD ? stX : gpt + LMAX * SmemPlan::kGroupPerLevel;
+
+    // End of a round (kRounds): every warp of the block arrives here once per round, `staged` telling whether its staging
+    // area holds a tile (zero tiles, tiles past the end and the idle warps of the virtual backward round do not).  The
+    // second barrier releases the staging areas (the grouped scatter reuses stX right after).
+    auto wgrad_round = [&](bool staged) {
+        if (lane == 0) smu[SmemPlan::RND + warp] = staged ? 1u : 0u;
+        round_bar(1);
+        uint32_t present = 0;
+#pragma unroll
+        for (int v = 0; v < kWarps; ++v) present |= (smu[SmemPlan::RND + v] != 0u ? 1u : 0u) << v;
+        const int mt = warp >> 2, nt = warp & 3;
+#pragma unroll
+        for (int v = 0; v < kWarps; ++v) {
+            if (!((present >> v) & 1u)) continue;
+            const float* sA = smem + SmemPlan::STAGE + v * SmemPlan::kStagePerWarp;   // dh2
+            const float* sB = sA + kTile * kWS;                                       // h1
+            // dW2[n2][k1] += sum_rows dh2[row][n2] * h1[row][k1]
+#pragma unroll
+            for (int ks = 0; ks < 2; ++ks) {
+                uint2 bh, bl;
+                split_fast2(sB[(8 * ks + t) * kWS + 8 * nt + g], sB[(8 * ks + t + 4) * kWS + 8 * nt + g], bh.x, bh.y, bl.x, bl.y);
+                AFrag<NTF> a;
+                a.set_packed(sA[(8 * ks + t) * kWS + 16 * mt + g], sA[(8 * ks + t) * kWS + 16 * mt + g + 8],
+                             sA[(8 * ks + t + 4) * kWS + 16 * mt + g], sA[(8 * ks + t + 4) * kWS + 16 * mt + g + 8]);
+                mma3<NTF>(dW2acc, a, bh, bl);
+            }
+        }
+        const int m1 = warp & 1;
+#pragma unroll
+        for (int vv = 0; vv < 2; ++vv) {
+            const int v = 2 * (warp >> 1) + vv;
+            if (!((present >> v) & 1u)) continue;
+            const float* sC = smem + SmemPlan::STAGE + v * SmemPlan::kStagePerWarp + 2 * kTile * kWS;   // dh1
+            const float* sX = sC + kTile * kWS;                                                       // feat
+            // dW1[n1][ch] += sum_rows dh1[row][n1] * feat[row][ch]
+#pragma unroll
+            for (int ks = 0; ks < 2; ++ks) {
+                uint2 bh, bl;
+                split_fast2(sX[(8 * ks + t) * kF + g], sX[(8 * ks + t + 4) * kF + g], bh.x, bh.y, bl.x, bl.y);
+                AFrag<NTF> a;
+                a.set_packed(sC[(8 * ks + t) * kWS + 16 * m1 + g], sC[(8 * ks + t) * kWS + 16 * m1 + g + 8],
+                             sC[(8 * ks + t + 4) * kWS + 16 * m1 + g], sC[(8 * ks + t + 4) * kWS + 16 * m1 + g + 8]);
+                mma3<NTF>(dW1acc, a, bh, bl);
+            }
+        }
+        round_bar(2);
+    };
 
     const int warp_global = blockIdx.x * kWarps + warp;
     const int warp_stride = gridDim.x * kWarps;
@@ -612,7 +687,8 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
     };
     prefetch_inputs(warp_global);
 
-    for (int tile = warp_global; tile < P.num_tiles; tile += warp_stride) {
+    // kRounds: the block's warps run the same rounds; a tile past the end has no valid point and contributes zeros
+    for (int tile = warp_global; tile - (kRounds ? warp : 0) < P.num_tiles; tile += warp_stride) {
         const int64_t base = (int64_t)tile * kTile;
         const int64_t myp = base + g + 8 * odd;
         asm volatile("cp.async.wait_group 0;" ::: "memory");
@@ -649,7 +725,8 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
     // linear in dL/dpred.  In a Morton-ordered batch free-space samples fill whole tiles (35 % of the C2 tiles): such a tile
     // only walks the hash, evaluates its loss terms against pred0 and adds its dL/dpred to a sum.  Pass 0 of the loop below
     // is one virtual tile (no points: features 0) run through the forward to get pred0; after the block's real tiles, warp 0
-    // runs one more virtual tile whose first point carries the block's dL/dpred sum through the ordinary backward.
+    // runs one more virtual tile whose first point carries the block's dL/dpred sum through the ordinary backward (with
+    // DEC_GRAD: one more round, in which the other warps stage nothing).
     int phase = kZeroSkip ? 0 : 1;          // 0: virtual forward, 1: this warp's tiles, 2: virtual backward (warp 0)
     bool advance = false, last_pass = false;
     float pred0 = 0.f, zsum = 0.f;
@@ -667,20 +744,22 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
     };
     // tile schedule: the first tile of a warp is its global index; every further one is drawn from P.tile_counter (counter
     // value k <-> tile warp_stride + k), requested a whole tile ahead so that the atomic's latency is never waited for
-    const bool dynamic = (SHINE_DYNAMIC_TILES != 0) && P.tile_counter != nullptr;
+    // (kRounds keeps the static schedule: its warps run in block-wide rounds)
+    const bool dynamic = (SHINE_DYNAMIC_TILES != 0) && !kRounds && P.tile_counter != nullptr;
     int next_tile = 0, pending = 0;
     if (dynamic && lane == 0) pending = atomicAdd(P.tile_counter, 1);
     for (int seq = warp_global;; seq = !advance ? seq : (dynamic ? next_tile : seq + warp_stride)) {
         if (last_pass) break;
         const int tile = tile_of(seq);
-        if (phase == 1 && seq >= P.num_tiles) {
+        // kRounds: the rounds go on while warp 0 of the block has a tile; a later warp's tile past the end is a zero tile
+        if (phase == 1 && seq - (kRounds ? warp : 0) >= P.num_tiles) {
             if constexpr (kZeroSkip && DEC_GRAD) {
                 // hand the all-miss dL/dpred sums of the block's warps to warp 0 (every warp passes here exactly once)
 #pragma unroll
                 for (int o = 16; o > 0; o >>= 1) zsum += __shfl_xor_sync(kFull, zsum, o);
                 if (lane == 0) smem[SmemPlan::PRE + warp] = zsum;
                 __syncthreads();
-                if (warp != 0) break;
+                if (!kRounds && warp != 0) break;
                 float tot = 0.f;
 #pragma unroll
                 for (int w = 0; w < kWarps; ++w) tot += smem[SmemPlan::PRE + w];
@@ -694,6 +773,7 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
         const bool virt = phase != 1;
         last_pass = phase == 2;
         advance = !virt;
+        if (kRounds && phase == 2 && warp != 0) { wgrad_round(false); continue; }
         const int64_t base = (int64_t)tile * kTile;
         const int64_t myp = base + g + 8 * odd;
         const bool valid = virt ? false : nvalid;
@@ -879,6 +959,7 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
                 bce_point(pred0, lab, wgt, li, dpz);
                 if (half == 0) { loss_acc += wgt * li; zsum += dpz; }
             }
+            if (kRounds) wgrad_round(false);
             continue;
         }
 #endif
@@ -969,7 +1050,10 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
 #endif
         if (P.pred && half == 0 && valid) P.pred[myp] = pown;
 
-        if (P.label == nullptr) continue;   // pure inference
+        if (P.label == nullptr) {   // pure inference
+            if (kRounds) wgrad_round(false);
+            continue;
+        }
 
         // ---- sdf_bce_loss (utils/loss.py:17-24) + dL/dpred ---------------------------------------------
         float dpo = 0.f;
@@ -999,7 +1083,7 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
         const float dpx = __shfl_xor_sync(kFull, dpo, 1);
         const float dp0 = odd ? dpx : dpo, dp8 = odd ? dpo : dpx;
         float dh2[4][4];
-        float db2t[4][2], db1t[4][2], dw3t[4][2];   // this tile's partials, folded into the accumulators in the wgrad section
+        float db2t[4][2], db1t[4][2], dw3t[4][2];   // this tile's partials (rows g, g+8), folded into vecacc before the round
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             dh2[j][0] = h2[j][0] > 0.f ? dp0 * w3a[j] : 0.f; dh2[j][1] = h2[j][1] > 0.f ? dp0 * w3b[j] : 0.f;
@@ -1059,8 +1143,8 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
             for (int r = 0; r < 4; ++r) dxc[r] += dxo[r];
         }
 
-        // ---- backward: decoder weight grads (contraction over the tile's 16 points) -------------------
-        if (DEC_GRAD) {
+        // ---- backward: decoder weight grads ------------------------------------------------------------------------
+        if (DEC_GRAD && !kRounds) {       // contraction over the tile's 16 points
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
                 db2p[j][0] += db2t[j][0]; db2p[j][1] += db2t[j][1];
@@ -1098,6 +1182,19 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
                 mma3x2<NTF>(dW1[0], dW1[1], a0, a1, bh, bl, bh, bl);
             }
             __syncwarp();
+                }
+        if (kRounds) {                    // bias / output-layer columns here, the weight matrices by the round
+            float cols[24];   // slot 8k + 2j + q: column 8j + 2t + q of db1 (k = 0), db2 (k = 1), dw3 (k = 2)
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+#pragma unroll
+                for (int q = 0; q < 2; ++q) { cols[2 * j + q] = db1t[j][q]; cols[8 + 2 * j + q] = db2t[j][q]; cols[16 + 2 * j + q] = dw3t[j][q]; }
+            }
+            float sums[3];
+            reduce_scatter_g(cols, sums, lane);
+#pragma unroll
+            for (int i = 0; i < 3; ++i) vecacc[i] += sums[i];
+            wgrad_round(true);
         }
 
         // ---- backward: scatter-add into the corner-feature tables (index_put_ accumulate) -------------
@@ -1158,7 +1255,50 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
         for (int o = 16; o > 0; o >>= 1) loss_acc += __shfl_xor_sync(kFull, loss_acc, o);
         if (lane == 0 && loss_acc != 0.f) atomicAdd(P.loss, loss_acc * P.loss_scale);
     }
-    if (DEC_GRAD) {
+    if (kRounds) {
+        // dW2: this warp is the only owner of its fragment, one global atomic per non-zero element
+        {
+            const int mt = warp >> 2, nt = warp & 3;
+#pragma unroll
+            for (int r = 0; r < 4; ++r)
+                if (dW2acc[r] != 0.f) atomicAdd(P.dec.gw2 + (16 * mt + g + 8 * (r >> 1)) * kH + 8 * nt + 2 * t + (r & 1), dW2acc[r]);
+        }
+        // the rest: per-warp partials [dW1 fragment warp & 1: 128 | gb1 32 | gb2 32 | gw3 32 | gb3 1] in the staging area
+        // (free after the last round), summed by the block, one global atomic per non-zero element
+        float* part = stage;
+        constexpr int oB1 = 128, oB3 = 224, kParts = 225;
+        *reinterpret_cast<float2*>(part + g * kF + 2 * t) = make_float2(dW1acc[0], dW1acc[1]);
+        *reinterpret_cast<float2*>(part + (g + 8) * kF + 2 * t) = make_float2(dW1acc[2], dW1acc[3]);
+#pragma unroll
+        for (int i = 0; i < 3; ++i) {
+            const int s = 3 * g + i, k = s >> 3, j = (s & 7) >> 1, q = s & 1;
+            part[oB1 + 32 * k + 8 * j + 2 * t + q] = vecacc[i];
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) db3p += __shfl_xor_sync(kFull, db3p, o);
+        if (lane == 0) part[oB3] = db3p;
+        __syncthreads();
+        for (int i = tid; i < 2 * oB1 + (kParts - oB1); i += blockDim.x) {
+            float v = 0.f;
+            float* dst;
+            if (i < 2 * oB1) {      // dW1 row 16 m + r: the partials of warps m, m + 2, m + 4, m + 6
+                const int m = i / oB1, e = i % oB1;
+#pragma unroll
+                for (int c = 0; c < kWarps / 2; ++c) v += smem[SmemPlan::STAGE + (2 * c + m) * SmemPlan::kStagePerWarp + e];
+                dst = P.dec.gw1 + 16 * m * kF + e;
+            } else {
+                const int e = i - oB1;
+#pragma unroll
+                for (int w = 0; w < kWarps; ++w) v += smem[SmemPlan::STAGE + w * SmemPlan::kStagePerWarp + e];
+                if (e < oB1 + kH) dst = P.dec.gb1 ? P.dec.gb1 + (e - oB1) : nullptr;
+                else if (e < oB1 + 2 * kH) dst = P.dec.gb2 ? P.dec.gb2 + (e - oB1 - kH) : nullptr;
+                else if (e < oB3) dst = P.dec.gw3 + (e - oB1 - 2 * kH);
+                else dst = P.dec.gb3;
+            }
+            if (v != 0.f && dst) atomicAdd(dst, v);
+        }
+    }
+    if (DEC_GRAD && !kRounds) {
         // every warp writes its complete partial gradient vector [gw1 256 | gb1 32 | gw2 1024 | gb2 32 | gw3 32 | gb3 1]
         // into its own staging area (each element has exactly one owner lane: plain stores, no shared-memory atomics),
         // then the block sums the eight vectors and issues one global atomic per non-zero element
