@@ -30,7 +30,7 @@
 extern "C" {
 #endif
 
-#define SHINE_ABI_VERSION 2
+#define SHINE_ABI_VERSION 3
 #define SHINE_MAX_LEVELS 8
 #define SHINE_HASH_SLOT_BYTES 64
 
@@ -172,18 +172,21 @@ int shine_adam_step_dev(const shine_adam_tensor* tensors, int32_t count, float b
                         void* state, int32_t zero_grad, void* stream);
 
 /* ---- FeatureOctree.update on the GPU (model/feature_octree.py:114-166) ---------------------------------------------
- * All featured levels of one scan at once; lv[] here is coarse -> fine.  Scratch (frame-local key sets, lists) is
- * caller-owned; sets are arrays of u64 filled with 0xFF, capacity a power of two >= 2x the insertions.
- * Sequence: frame_nodes -> (host reads new_node_count, sizes tables) -> frame_corners -> (host reads new_corner_count)
- * -> sort_corners -> assign_rows -> fill_nodes.  Row numbering is the reference's: unseen corners of the new nodes,
- * unique, in lexicographic (x, y, z) order, appended after the existing rows (:131-151). */
+ * All featured levels of one scan at once; lv[] here is coarse -> fine; world levels 1 .. 15 (kaolin's int16 points).
+ * Scratch (frame-local key sets, lists) is caller-owned; sets are arrays of u64 filled with 0xFF, capacity a power of
+ * two >= 2x the insertions.
+ * Sequence: frame_nodes -> (host reads new_node_count, sizes tables, copies the N node entries to the front of the sort
+ * input and points new_corner_keys right behind them) -> frame_corners -> (host reads new_corner_count) ->
+ * sort_new_keys over the N + C entries -> assign_rows (the first C sorted entries) -> fill_nodes (the last N).
+ * Row numbering is the reference's: unseen corners of the new nodes, unique, in lexicographic (x, y, z) order of
+ * kaolin's int16 points, appended after the existing rows (:131-151).  Node numbering too: new nodes in ascending
+ * Morton order, appended (:164-166). */
 typedef struct shine_build_level {
     void* node_slots;               /* the level's node table (64-byte slots), NULL while the level is empty          */
     void* corner_slots;             /* the level's corner table: 16-byte slots {u64 lexicographic key, i32 row, pad} */
     void* frame_node_set;           /* scratch u64 set                                                                */
     void* frame_corner_set;         /* scratch u64 set (frame_corners onwards)                                        */
-    int64_t* new_node_keys;         /* out [<= n points] Morton keys of this scan's unseen nodes (unordered)         */
-    int32_t* node_ids_out;          /* out [new nodes, 8] corner rows of those nodes (fill_nodes)                     */
+    int32_t* node_ids_out;          /* out [new nodes, 8] corner rows of those nodes, Morton order (fill_nodes)       */
     int64_t* corner_morton_out;     /* out [new corners] Morton code of each new row, in row order (assign_rows)      */
     uint32_t node_capacity, corner_capacity, frame_node_set_capacity, frame_corner_set_capacity;
     int32_t level;                  /* world level                                                                    */
@@ -195,17 +198,21 @@ typedef struct shine_build {
     int32_t* new_node_count;        /* device [L], zero on entry                                                      */
     int32_t* new_corner_count;      /* device [L], zero on entry                                                      */
     int32_t* new_corner_total;      /* device [1], zero on entry                                                      */
-    uint64_t* new_corner_keys;      /* scratch [8 * sum new nodes]: (level index << 51) | lexicographic key           */
+    int32_t* new_node_total;        /* device [1], zero on entry                                                      */
+    uint64_t* new_node_keys;        /* out [<= L * n points] (1 << 51) | (level index << 45) | Morton key, unordered  */
+    uint64_t* new_corner_keys;      /* scratch [8 * sum new nodes]: (level index << 48) | lexicographic key           */
     shine_build_level lv[SHINE_MAX_LEVELS];
 } shine_build;
 
 int shine_octree_frame_nodes(const shine_build* plan, const float* points, int64_t n, void* stream);
-int shine_octree_frame_corners(const shine_build* plan, int32_t max_new_nodes, void* stream);
+int shine_octree_frame_corners(const shine_build* plan, int32_t new_nodes, void* stream);
 int64_t shine_octree_sort_scratch_bytes(int32_t n);
-int shine_octree_sort_corners(const void* keys_in, void* keys_out, int32_t n, void* scratch, int64_t scratch_bytes,
-                              void* stream);
+int shine_octree_sort_new_keys(const void* keys_in, void* keys_out, int32_t n, void* scratch, int64_t scratch_bytes,
+                               void* stream);
 int shine_octree_assign_rows(const shine_build* plan, const void* sorted_keys, int32_t total, void* stream);
-int shine_octree_fill_nodes(const shine_build* plan, int32_t max_new_nodes, int32_t* overflow_count, void* stream);
+/* sorted_nodes: the last new_nodes entries of the sort output; their tags are cleared in place (plain Morton keys) */
+int shine_octree_fill_nodes(const shine_build* plan, void* sorted_nodes, int32_t new_nodes, int32_t* overflow_count,
+                            void* stream);
 /* rebuild a corner table from the per-row Morton codes (after growing it, moving devices or unpickling) */
 int shine_octree_corner_rehash(void* corner_slots, uint32_t capacity, const int64_t* corner_morton_by_row, int64_t rows,
                                void* stream);

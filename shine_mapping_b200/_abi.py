@@ -13,7 +13,7 @@ import torch
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("SHINE_B200_LIB") or os.path.join(_HERE, "csrc", "libshine_b200.so")
 
-ABI_VERSION = 2
+ABI_VERSION = 3
 MAX_LEVELS = 8
 HASH_SLOT_BYTES = 64
 ADAM_MAX_TENSORS = 16
@@ -73,7 +73,7 @@ class ShineBoundary(C.Structure):
 
 class ShineBuildLevel(C.Structure):
     _fields_ = [("node_slots", C.c_void_p), ("corner_slots", C.c_void_p), ("frame_node_set", C.c_void_p),
-                ("frame_corner_set", C.c_void_p), ("new_node_keys", C.c_void_p), ("node_ids_out", C.c_void_p),
+                ("frame_corner_set", C.c_void_p), ("node_ids_out", C.c_void_p),
                 ("corner_morton_out", C.c_void_p),
                 ("node_capacity", C.c_uint32), ("corner_capacity", C.c_uint32), ("frame_node_set_capacity", C.c_uint32),
                 ("frame_corner_set_capacity", C.c_uint32),
@@ -82,7 +82,8 @@ class ShineBuildLevel(C.Structure):
 
 class ShineBuild(C.Structure):
     _fields_ = [("num_levels", C.c_int32), ("max_level", C.c_int32), ("new_node_count", C.c_void_p),
-                ("new_corner_count", C.c_void_p), ("new_corner_total", C.c_void_p), ("new_corner_keys", C.c_void_p),
+                ("new_corner_count", C.c_void_p), ("new_corner_total", C.c_void_p), ("new_node_total", C.c_void_p),
+                ("new_node_keys", C.c_void_p), ("new_corner_keys", C.c_void_p),
                 ("lv", ShineBuildLevel * MAX_LEVELS)]
 
 
@@ -112,9 +113,9 @@ SYMBOLS = {
     "shine_octree_frame_nodes": (C.c_int, [C.POINTER(ShineBuild), _vp, _i64, _vp]),
     "shine_octree_frame_corners": (C.c_int, [C.POINTER(ShineBuild), _i32, _vp]),
     "shine_octree_sort_scratch_bytes": (C.c_int64, [_i32]),
-    "shine_octree_sort_corners": (C.c_int, [_vp, _vp, _i32, _vp, _i64, _vp]),
+    "shine_octree_sort_new_keys": (C.c_int, [_vp, _vp, _i32, _vp, _i64, _vp]),
     "shine_octree_assign_rows": (C.c_int, [C.POINTER(ShineBuild), _vp, _i32, _vp]),
-    "shine_octree_fill_nodes": (C.c_int, [C.POINTER(ShineBuild), _i32, _vp, _vp]),
+    "shine_octree_fill_nodes": (C.c_int, [C.POINTER(ShineBuild), _vp, _i32, _vp, _vp]),
     "shine_octree_corner_rehash": (C.c_int, [_vp, _u32, _vp, _i64, _vp]),
     "shine_count_positive": (C.c_int, [_vp, _i64, _vp, _vp]),
     "shine_sdf_bce_eikonal_step": (C.c_int, [_OCT, _DEC, _vp, _vp, _vp, _i64, _f32, _f32, _f32, _vp, _vp, _vp, _vp, _vp, _u32, _vp]),

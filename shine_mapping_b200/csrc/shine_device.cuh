@@ -58,7 +58,7 @@ constexpr unsigned kFull = 0xFFFFFFFFu;
 // once: a first-probe hit costs a single memory round trip before the feature rows can be requested.
 struct __align__(64) HashSlot {
     unsigned long long key;   // Morton code of the voxel, kEmptyKey when free
-    int32_t node;             // insertion ordinal (diagnostics)
+    int32_t node;             // insertion ordinal = index in node_keys, the reference's order (Morton order within a frame)
     int32_t maxdisp;          // as HOME slot: largest probe index of any key whose probe sequence starts here (<= 0: none
                               // was displaced) — a lookup that does not find its key in its home slot stops right there
                               // unless this says that some key of this home lives further along

@@ -72,9 +72,19 @@ def points_to_corners(p: torch.Tensor) -> torch.Tensor:
 
 
 def _lex_key(c: torch.Tensor) -> torch.Tensor:
-    """Order-preserving key of lexicographic (x, y, z) — the order of torch.unique(dim=0) (reference :132)."""
-    c = c.long()
-    return (c[..., 0] << 34) | (c[..., 1] << 17) | c[..., 2]
+    """Order-preserving key of lexicographic (x, y, z) — the order of torch.unique(dim=0) (reference :132) on kaolin's
+    int16 corner points, where the coordinate 2^15 of the + face at world level 15 wraps to -2^15 and comes first:
+    c ^ 0x8000 maps that order onto unsigned 16-bit order (csrc/shine_octree_build.cu keys its corners the same way)."""
+    c = c.long() ^ 0x8000
+    return (c[..., 0] << 32) | (c[..., 1] << 16) | c[..., 2]
+
+
+def _lex_to_points(k: torch.Tensor) -> torch.Tensor:
+    return torch.stack((k >> 32, (k >> 16) & 0xFFFF, k & 0xFFFF), -1) ^ 0x8000
+
+
+# kaolin's octree points are int16: level 15 is the deepest whose corner coordinates (0 .. 2^15) fit 16 bits
+MAX_WORLD_LEVEL = 15
 
 
 def _next_pow2(n: int) -> int:
@@ -85,7 +95,7 @@ class _LevelState:
     """Authoritative per-level arrays (world level numbering)."""
 
     def __init__(self, device):
-        self.node_keys = torch.empty(0, dtype=torch.int64, device=device)        # insertion order
+        self.node_keys = torch.empty(0, dtype=torch.int64, device=device)        # insertion order (Morton per frame)
         self.node_ids = torch.empty(0, 8, dtype=torch.int32, device=device)      # rows of the 8 corners
         self.node_keys_sorted = torch.empty(0, dtype=torch.int64, device=device)
         self.corner_lex_sorted = torch.empty(0, dtype=torch.int64, device=device)
@@ -203,6 +213,10 @@ class FeatureOctree(nn.Module):
             raise ValueError('No level with grid features!')
         if self.featured_level_num > _abi.MAX_LEVELS:
             raise ValueError(f'tree_level_feat > {_abi.MAX_LEVELS} is not supported by the sm_90a kernels')
+        if self.max_level > MAX_WORLD_LEVEL:
+            raise ValueError(f'tree_level_world > {MAX_WORLD_LEVEL} is not supported: kaolin keeps octree points as int16, '
+                             f'so the corners of level {MAX_WORLD_LEVEL + 1} (coordinates up to 2^{MAX_WORLD_LEVEL + 1}) '
+                             'cannot be represented')
         self._levels = [_LevelState(self.device) for _ in range(self.max_level + 1)]
         self._dict_cache = None
         self._desc_cache = {}
@@ -391,8 +405,7 @@ class FeatureOctree(nn.Module):
                 all_rows = torch.cat((st.corner_rows_sorted, fresh_rows))
                 order = torch.argsort(all_lex)
                 st.corner_lex_sorted, st.corner_rows_sorted = all_lex[order], all_rows[order]
-                fresh_xyz = torch.stack((fresh >> 34, (fresh >> 17) & 0x1FFFF, fresh & 0x1FFFF), -1)
-                st.corner_morton_by_row = torch.cat((st.corner_morton_by_row, points_to_morton(fresh_xyz)))
+                st.corner_morton_by_row = torch.cat((st.corner_morton_by_row, points_to_morton(_lex_to_points(fresh))))
             ids = st.corner_rows_sorted[torch.searchsorted(st.corner_lex_sorted, lex)].reshape(-1, 8).to(torch.int32)
             st.node_keys = torch.cat((st.node_keys, new_m))
             st.node_ids = torch.cat((st.node_ids, ids))
@@ -432,7 +445,8 @@ class FeatureOctree(nn.Module):
 
     def _update_cuda(self, pts, incremental_on):
         """update() as kernels over the scan (csrc/shine_octree_build.cu): no unique/sort/searchsorted over the scan, one
-        radix sort over the NEW corners only; two small count read-backs size the tables and the new feature rows."""
+        radix sort over the NEW nodes and corners only; two small count read-backs size the tables and the new feature
+        rows."""
         lib = _abi.lib()
         dev = pts.device
         st_ptr = _abi.stream_ptr(dev)
@@ -441,15 +455,17 @@ class FeatureOctree(nn.Module):
             return
         L = self.featured_level_num
         levels = list(range(self.free_level_num, self.max_level + 1))         # coarse -> fine, like hier_features
-        counts = torch.zeros(2 * L + 1, dtype=torch.int32, device=dev)
+        counts = torch.zeros(2 * L + 2, dtype=torch.int32, device=dev)
         plan = _abi.ShineBuild()
         plan.num_levels, plan.max_level = L, self.max_level
         plan.new_node_count = counts.data_ptr()
         plan.new_corner_count = counts.data_ptr() + 4 * L
         plan.new_corner_total = counts.data_ptr() + 8 * L
+        plan.new_node_total = counts.data_ptr() + 8 * L + 4
         set_cap = _next_pow2(2 * n)
         node_sets = torch.full((L, set_cap), -1, dtype=torch.int64, device=dev)
-        new_keys = torch.empty(L, n, dtype=torch.int64, device=dev)
+        node_list = torch.empty(L * n, dtype=torch.int64, device=dev)
+        plan.new_node_keys = node_list.data_ptr()
         for l, lvl in enumerate(levels):
             st = self._levels[lvl]
             self._ensure_level_tables(st, lvl)
@@ -458,10 +474,10 @@ class FeatureOctree(nn.Module):
             b.node_slots = st.hash.data_ptr() if st.hash is not None else None
             b.node_capacity = st.hash_capacity
             b.frame_node_set, b.frame_node_set_capacity = node_sets[l].data_ptr(), set_cap
-            b.new_node_keys = new_keys[l].data_ptr()
         _abi.check(lib.shine_octree_frame_nodes(C.byref(plan), _abi.ptr(pts), n, st_ptr), "shine_octree_frame_nodes")
         c_nodes = counts[:L].tolist()                                          # read-back 1
-        if sum(c_nodes) == 0:
+        n_new = sum(c_nodes)
+        if n_new == 0:
             return
         keep = []       # scratch referenced by the plan must outlive the launches
         for l, lvl in enumerate(levels):
@@ -477,17 +493,18 @@ class FeatureOctree(nn.Module):
             b.frame_corner_set, b.frame_corner_set_capacity = cs.data_ptr(), cap
             b.node_ids_out = ids.data_ptr()
             keep.append((cs, ids))
-        corner_keys = torch.empty(8 * sum(c_nodes), dtype=torch.int64, device=dev)
-        plan.new_corner_keys = corner_keys.data_ptr()
-        _abi.check(lib.shine_octree_frame_corners(C.byref(plan), max(c_nodes), st_ptr), "shine_octree_frame_corners")
-        c_corners = counts[L:].tolist()                                        # read-back 2
+        # sort input: the node entries, then room for the corner entries frame_corners appends
+        keys = torch.empty(9 * n_new, dtype=torch.int64, device=dev)
+        keys[:n_new].copy_(node_list[:n_new])
+        plan.new_corner_keys = keys.data_ptr() + 8 * n_new
+        _abi.check(lib.shine_octree_frame_corners(C.byref(plan), n_new, st_ptr), "shine_octree_frame_corners")
+        c_corners = counts[L:2 * L + 1].tolist()                               # read-back 2
         total = c_corners[-1]
-        sorted_keys = torch.empty(max(total, 1), dtype=torch.int64, device=dev)
-        if total:
-            nbytes = int(lib.shine_octree_sort_scratch_bytes(total))
-            scratch = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=dev)
-            _abi.check(lib.shine_octree_sort_corners(_abi.ptr(corner_keys), _abi.ptr(sorted_keys), total, _abi.ptr(scratch),
-                                                     nbytes, st_ptr), "shine_octree_sort_corners")
+        sorted_keys = torch.empty(total + n_new, dtype=torch.int64, device=dev)  # [corners | nodes]
+        nbytes = int(lib.shine_octree_sort_scratch_bytes(total + n_new))
+        scratch = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=dev)
+        _abi.check(lib.shine_octree_sort_new_keys(_abi.ptr(keys), _abi.ptr(sorted_keys), total + n_new, _abi.ptr(scratch),
+                                                  nbytes, st_ptr), "shine_octree_sort_new_keys")
         mortons = []
         for l in range(L):
             m = torch.empty(max(c_corners[l], 1), dtype=torch.int64, device=dev)
@@ -496,9 +513,11 @@ class FeatureOctree(nn.Module):
         if total:
             _abi.check(lib.shine_octree_assign_rows(C.byref(plan), _abi.ptr(sorted_keys), total, st_ptr),
                        "shine_octree_assign_rows")
+        new_keys = sorted_keys[total:]                                         # Morton order per level, after fill_nodes
         overflow = torch.zeros(1, dtype=torch.int32, device=dev)
-        _abi.check(lib.shine_octree_fill_nodes(C.byref(plan), max(c_nodes), _abi.ptr(overflow), st_ptr),
+        _abi.check(lib.shine_octree_fill_nodes(C.byref(plan), _abi.ptr(new_keys), n_new, _abi.ptr(overflow), st_ptr),
                    "shine_octree_fill_nodes")
+        start = 0
         for l, lvl in enumerate(levels):          # ascending levels: the reference's randn call order (:139,153)
             if c_nodes[l] == 0:
                 continue
@@ -506,10 +525,11 @@ class FeatureOctree(nn.Module):
             first = st.corner_morton_by_row.numel() == 0 and len(self.hier_features) <= l
             self._grow_features(l, c_corners[l], first, incremental_on, dev)
             st.corner_morton_by_row = torch.cat((st.corner_morton_by_row, mortons[l][:c_corners[l]]))
-            st.node_keys = torch.cat((st.node_keys, new_keys[l, :c_nodes[l]]))
+            st.node_keys = torch.cat((st.node_keys, new_keys[start:start + c_nodes[l]]))
             st.node_ids = torch.cat((st.node_ids, keep[l][1][:c_nodes[l]]))
             st.hash_count = int(st.node_keys.numel())
             st.corner_hash_count = int(st.corner_morton_by_row.numel())
+            start += c_nodes[l]
         if int(overflow.item()):
             raise _abi.ShineB200Error("node table overflow while growing the octree")
         self._dict_cache = None

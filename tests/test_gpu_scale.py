@@ -157,8 +157,8 @@ def test_hash_insert_reports_overflow():
 
 def test_cuda_update_matches_oracle_tables_frame_by_frame():
     """FeatureOctree.update on the GPU (build kernels, csrc/shine_octree_build.cu): after every frame of an incremental
-    run the node / corner tables equal the oracle's dicts (append-only lexicographic row numbering), no ATen sort /
-    unique over the scan is launched, and the per-frame launch count stays small."""
+    run the node / corner tables equal the oracle's dicts, in the same order (nodes appended in Morton order, rows in
+    lexicographic order), no ATen sort / unique over the scan is launched, and the per-frame launch count stays small."""
     from torch.profiler import ProfilerActivity, profile
     from shine_mapping_b200 import FeatureOctree, synth
     from tests.parity_utils import make_config
@@ -184,6 +184,9 @@ def test_cuda_update_matches_oracle_tables_frame_by_frame():
         for lvl in range(octree.free_level_num, octree.max_level + 1):
             assert octree.nodes_lookup_tables[lvl] == o.nodes_lookup_tables[lvl], f"nodes differ at level {lvl}"
             assert octree.corners_lookup_tables[lvl] == o.corners_lookup_tables[lvl], f"corners differ at level {lvl}"
+            # insertion order too: new nodes in Morton order, new corner rows in lexicographic order
+            assert list(octree.nodes_lookup_tables[lvl]) == list(o.nodes_lookup_tables[lvl]), f"node order at level {lvl}"
+            assert list(octree.corners_lookup_tables[lvl]) == list(o.corners_lookup_tables[lvl]), f"row order at {lvl}"
         assert [tuple(p.shape) for p in octree.hier_features] == [tuple(t.shape) for t in o.hier_features]
         assert [tuple(w.shape) for w in octree.importance_weight] == [tuple(p.shape) for p in octree.hier_features]
     print("update() device launches per frame (kernels + memsets + copies):", launches,

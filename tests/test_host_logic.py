@@ -18,7 +18,8 @@ def test_library_exports_every_declared_symbol(built_lib):
     assert declared == set(_abi.SYMBOLS), declared ^ set(_abi.SYMBOLS)
     for name in declared:
         assert getattr(built_lib, name) is not None
-    assert built_lib.shine_abi_version() == 2
+    # 3: shine_build carries one tagged new-node list (node numbering in the reference's Morton order)
+    assert built_lib.shine_abi_version() == _abi.ABI_VERSION == 3
     assert built_lib.shine_error_string(-2).decode().startswith("shine_b200: unsupported")
 
 
@@ -30,6 +31,8 @@ def test_struct_layouts_match_header():
     assert C.sizeof(_abi.ShineDecoder) == 12 * 8 + 16
     assert C.sizeof(_abi.ShineAdamTensor) == 48
     assert C.sizeof(_abi.ShineBoundaryInverse) == 8 * 8 + 8 * 4 + 8 * 8      # row_of_slot | slots | holders (SHINE_MAX_LEVELS = 8)
+    assert C.sizeof(_abi.ShineBuildLevel) == 6 * 8 + 4 * 4 + 4 * 4
+    assert C.sizeof(_abi.ShineBuild) == 8 + 6 * 8 + 8 * C.sizeof(_abi.ShineBuildLevel)
 
 
 def test_abi_argument_checks_need_no_gpu(built_lib):
@@ -41,6 +44,24 @@ def test_abi_argument_checks_need_no_gpu(built_lib):
     assert built_lib.shine_query_fwd(C.byref(d), None, 4, None, None) == -2          # F not a multiple of 4
     assert built_lib.shine_hash_insert(None, 16, None, None, 0, 0, None, None) == -1
     assert built_lib.shine_points_to_morton(None, 0, 12, None, None) == 0            # empty is fine
+    # the octree build accepts world levels up to 15 (kaolin's int16 points); the checks run before any launch, so an
+    # empty scan with placeholder pointers returns OK
+    scratch = (C.c_int64 * 64)()
+    plan = _abi.ShineBuild()
+    plan.num_levels, plan.max_level = 1, 15
+    plan.new_node_count = plan.new_corner_count = plan.new_corner_total = plan.new_node_total = C.addressof(scratch)
+    plan.new_node_keys = plan.new_corner_keys = C.addressof(scratch)
+    plan.lv[0].level, plan.lv[0].frame_node_set, plan.lv[0].frame_node_set_capacity = 15, C.addressof(scratch), 16
+    assert built_lib.shine_octree_frame_nodes(C.byref(plan), None, 0, None) == 0
+    assert built_lib.shine_octree_frame_corners(C.byref(plan), 0, None) == 0
+    plan.max_level = plan.lv[0].level = 16
+    assert built_lib.shine_octree_frame_nodes(C.byref(plan), None, 0, None) == -1
+    assert built_lib.shine_octree_frame_corners(C.byref(plan), 0, None) == -1
+    assert built_lib.shine_octree_assign_rows(C.byref(plan), None, 0, None) == -1
+    assert built_lib.shine_octree_fill_nodes(C.byref(plan), None, 0, None, None) == -1
+    plan.max_level = plan.lv[0].level = 15
+    plan.new_node_total = None
+    assert built_lib.shine_octree_frame_nodes(C.byref(plan), None, 0, None) == -1
 
 
 @pytest.mark.parametrize("name", GOLDEN_NAMES)
@@ -99,6 +120,14 @@ def test_constructor_contract_and_attributes():
     cfg.tree_level_feat = 0
     with pytest.raises(ValueError, match="No level with grid features"):
         FeatureOctree(cfg)
+    cfg.tree_level_feat = 4
+    for world in (15, 16):
+        cfg.tree_level_world = world
+        if world == 15:
+            assert FeatureOctree(cfg).max_level == 15
+        else:
+            with pytest.raises(ValueError, match="int16"):
+                FeatureOctree(cfg)
 
 
 def test_octree_pickles_like_the_reference_checkpoint():

@@ -10,7 +10,7 @@ from tests.parity_utils import make_config, orc
 
 @settings(max_examples=25, deadline=None)
 @given(seed=st.integers(0, 2 ** 31 - 1), n=st.integers(1, 400), frames=st.integers(1, 3),
-       levels=st.integers(1, 4), world=st.sampled_from([6, 9, 12]), spread=st.sampled_from([0.003, 0.05, 1.2]))
+       levels=st.integers(1, 4), world=st.sampled_from([6, 9, 12, 15]), spread=st.sampled_from([0.003, 0.05, 1.2]))
 def test_update_matches_oracle_on_random_clouds(seed, n, frames, levels, world, spread):
     from shine_mapping_b200 import FeatureOctree
     levels = min(levels, world)
