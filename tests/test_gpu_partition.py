@@ -45,7 +45,9 @@ def _check_decoder_and_loss(trainer, loss, res_glob):
     assert abs(loss - float(res_glob["loss"])) <= 2e-5 * abs(float(res_glob["loss"]))
 
 
-def test_three_ranges_on_one_gpu_equal_the_single_step(built_lib):
+def _three_ranges_on_one_gpu(replicas_per_rank=None):
+    """replicas_per_rank: a list that receives, per rank, the R per level of the step's replica fold (which runs inside
+    forward_backward, before the boundary pack)."""
     from shine_mapping_b200 import SdfTrainer
     from shine_mapping_b200.partition import BoundaryPlan, coarse_keys, owner_of, partition_pool
     world = 3
@@ -60,6 +62,13 @@ def test_three_ranges_on_one_gpu_equal_the_single_step(built_lib):
     trainers = []
     for r, (cfg, octree, decoder, keys) in enumerate(built):
         tr = SdfTrainer(cfg, octree, decoder, shard_mode="spatial", boundary=plans[r])
+        if replicas_per_rank is not None:
+            fold = octree._reduce_replicas
+
+            def spy(desc, device, fold=fold):
+                replicas_per_rank.append([max(1, desc.lv[i].num_replicas) for i in range(desc.num_levels)])
+                fold(desc, device)
+            octree._reduce_replicas = spy
         tr.zero_grad()
         m = owner == r
         tr.forward_backward(batch[0][m].to(DEV), batch[1][m].to(DEV), None, n_norm=n_global)
@@ -75,6 +84,23 @@ def test_three_ranges_on_one_gpu_equal_the_single_step(built_lib):
                                           res_glob)
         _check_decoder_and_loss(tr, loss, res_glob)
     print("3 ranges on one GPU == single step; boundary rows per level:", plans[0].counts, "worst rel", worst)
+    for tr in trainers:
+        assert all(int(torch.count_nonzero(b)) == 0 for b in tr.octree._grad_scratch.values())
+
+
+def test_three_ranges_on_one_gpu_equal_the_single_step(built_lib):
+    _three_ranges_on_one_gpu()
+
+
+def test_three_ranges_on_one_gpu_with_forced_replicas(built_lib, monkeypatch):
+    """The same partition with gradient replicas on every rank's coarse levels."""
+    from shine_mapping_b200 import FeatureOctree
+    monkeypatch.setattr(FeatureOctree, "_REPLICA_TARGET", 1)
+    monkeypatch.setattr(FeatureOctree, "_REPLICA_MAX", 64)
+    seen = []
+    _three_ranges_on_one_gpu(seen)
+    assert len(seen) == 3 and all(max(r) > 1 for r in seen), f"R per level and rank: {seen}"
+    print("R per level (leaf first) and rank:", seen)
 
 
 def _free_port():

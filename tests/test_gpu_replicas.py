@@ -1,0 +1,706 @@
+"""Gradient replicas against an fp64 oracle, element by element, at the replica counts that switch them on.
+
+An unordered training batch spreads its table-gradient atomics over R replicas of every small, hot level
+(`FeatureOctree._replicas_for`: R = pow2 <= min(8 n / (rows * _REPLICA_TARGET), _REPLICA_MAX)).  Warp w adds into replica
+w & (R - 1) (the voxel-grouped kernel picks it by tile); replica 0 is the gradient table itself, replicas 1..R-1 live in the octree's scratch, and
+`shine_reduce_grad_replicas` adds them back in the order 1..R-1 and re-zeroes them.  At the sizes of the parity cases R is 1
+on every level, so the cases here lower `_REPLICA_TARGET` and raise `_REPLICA_MAX` (class attributes read at call time) on a
+fresh octree, and every case asserts the R per level that its step's descriptor carried (a spy on `_reduce_replicas`): a
+case that silently runs at R = 1 fails.  One case runs at a natural size without a patch.
+
+Reference.  The oracle step (`oracle.shine_oracle.train_step`) runs in float64: tables, decoder and labels in float64, the
+coordinates kept fp32, so the blend weights are the reference's fp32 values (the kernels compute the same expression in
+the same fp32 operations) and everything after them is fp64.
+
+Per-element bound, u = 2^-24.  Row u, channel f of a level's gradient is the sum over the k_u (point, corner) terms that land
+on that row of w_{j,c} dfeat_{j,f}.  Every path forms a term as one fp32 product and adds terms with fp32 adds (atomics into
+one of R partial sums, then the fold); an add into an exact zero is exact, so a term passes at most k_u - 1 roundings after
+its product, whatever the order or the replica: the summation is off by at most k_u u S_{u,f}, S = sum_j w_{j,c} |dfeat_{j,f}|
+(in fp64 from the oracle's indices and weights).  The slack C = 4 covers second-order terms.  The voxel-grouped kernel forms
+the per-node sums of up to 16 points as a 3xTF32 contraction, so it adds EPS_MM(16) to C.
+    |got - want64| <= (k_u + C) u S_{u,f} + T_{u,f}
+For `query_bwd` dfeat is the input and T = 0.  The fused kernels compute dfeat themselves; T = sum_j w_{j,c} E_{j,f} carries
+its error E_j:
+  * decoder contractions are 3xTF32: x = hi + lo with hi cut to tf32 and lo = x - hi, x y ~ hi hi' + hi lo' + lo hi' with lo
+    cut to tf32 too.  The dropped lo lo' and both cuts of lo stay below 2^-20 |x y| each (truncation, the worst case), so a
+    K-term contraction is off by at most EPS_MM(K) = (64 + 8K) u of sum |x||y| (48 u for the products, up to 2 u per fp32 add in
+    each of the three passes, rounded up).  Plain TF32 (tf32x1) cuts both operands once: 2^-9 + 8K u;
+  * forward, on absolute values with the fp64 pass's ReLU masks (A0 = sum w |row|, A1 = |W1| A0 + |b1|, A2 = |W2| A1 + |b2|,
+    Ap = |w3| A2 + |b3|): the blend is off by (8L + 2) u A0, layer k adds EPS_MM(K) and the bias add u, so
+    |pred - pred64| <= P = EPS_FWD Ap (checked against the kernel's own pred);
+  * dL/dpred = s (sigmoid(pred) - sigmoid(label / sigma)), s = loss scale x |weight|: off by s (P / 4 + 16 u) + 4 u |g|;
+  * dfeat = W1^T (m1 . W2^T (m2 . w3 g)), two 32-term contractions: E = D ((2 EPS_MM(32) + 2 u) |g| + dg), D = |W1|^T (m1 .
+    |W2|^T (m2 . |w3|)).
+Points within twice the forward error of a ReLU kink are dropped from the fused cases: there a correct fp32 kernel may take
+the other branch.  `compare_step` (2e-4 of the level maximum) runs as a second check, and each case prints its worst
+error / bound.
+"""
+import ctypes as C
+
+import numpy as np
+import pytest
+import torch
+
+from oracle import shine_oracle as orc
+from tests.parity_utils import build_cuda_models, compare_step, make_case, oracle_from_case, sort_case_morton
+
+DEV = "cuda:0"
+U = 2.0 ** -24
+C_SLACK = 4
+H = 32
+INVALID = -1                            # SHINE_ERR_INVALID_ARG
+gpu = pytest.mark.gpu
+
+
+def eps_mm(k, tf32x1=False):
+    return (2.0 ** -9 if tf32x1 else 64 * U) + 8 * k * U
+
+
+# ---- forcing replicas and proving they were on ----------------------------------------------------------------------------
+
+def expected_replicas(tables, n):
+    """R per level, coarse -> fine, from the rule of the module docstring and the CURRENT class attributes."""
+    from shine_mapping_b200 import FeatureOctree
+    out = []
+    for t in tables:
+        want = (8 * n) // max(1, t.shape[0] * FeatureOctree._REPLICA_TARGET)
+        r = 1
+        while r * 2 <= min(want, FeatureOctree._REPLICA_MAX):
+            r *= 2
+        out.append(r)
+    return out
+
+
+@pytest.fixture
+def force(monkeypatch):
+    """force(target, rmax): switch replicas on at small batches for octrees that build their descriptors afterwards."""
+    from shine_mapping_b200 import FeatureOctree
+
+    def set_(target, rmax=64):
+        monkeypatch.setattr(FeatureOctree, "_REPLICA_TARGET", target)
+        monkeypatch.setattr(FeatureOctree, "_REPLICA_MAX", rmax)
+    return set_
+
+
+class FoldSpy:
+    """Records the R per level (coarse -> fine) of every descriptor handed to the octree's fold."""
+
+    def __init__(self, octree):
+        self.calls = []
+        fold = octree._reduce_replicas
+        L = octree.featured_level_num
+
+        def spy(desc, device):
+            self.calls.append([max(1, desc.lv[L - 1 - k].num_replicas) for k in range(L)])   # 0 and 1: no replicas
+            fold(desc, device)
+        octree._reduce_replicas = spy
+
+    def expect(self, want, what=""):
+        assert self.calls, f"{what}: the step never called the replica fold"
+        assert self.calls[-1] == want, f"{what}: the step ran with R = {self.calls[-1]} per level, expected {want}"
+        assert max(want) > 1, f"{what}: the case does not switch replicas on"
+        self.calls.clear()
+
+
+def assert_scratch_zero(octree, what=""):
+    torch.cuda.synchronize()
+    assert octree._grad_scratch, f"{what}: no replica scratch was allocated"
+    for k, buf in octree._grad_scratch.items():
+        nz = int(torch.count_nonzero(buf))
+        assert nz == 0, f"{what}: replica scratch of level {k} holds {nz} non-zero values after the step"
+
+
+# ---- fp64 reference and the per-element bound -----------------------------------------------------------------------------
+
+def subset(case, keep):
+    out = dict(case)
+    for k in ("coord", "label", "weight"):
+        out[k] = np.ascontiguousarray(case[k][keep])
+    return out
+
+
+def _oracle64(case):
+    o, dec = oracle_from_case(case)
+    o.hier_features = [t.detach().double().requires_grad_(True) for t in o.hier_features]
+    return o, {k: v.detach().double().requires_grad_(True) for k, v in dec.items()}
+
+
+def _blend(o, coord):
+    """Per level (bottom-up): the oracle's corner rows [N*8] and fp32 blend weights [N*8] as fp64."""
+    idx = o.get_indices(coord)
+    out = []
+    for i in range(o.featured_level_num):
+        w = o.interpolat(coord, o.max_level - i, o.polynomial_interpolation).reshape(-1).double()
+        out.append((idx[i].reshape(-1), w))
+    return out
+
+
+def _decoder_passes(feat, absfeat, dec, tf32x1, n_levels):
+    """fp64 forward with the absolute-value passes of the module docstring -> dict of per-point quantities."""
+    z = torch.zeros((), dtype=torch.float64)
+    W1, W2, w3 = (dec[k].detach() for k in ("layers.0.weight", "layers.1.weight", "lout.weight"))
+    b1, b2, b3 = (dec.get(k, z).detach() for k in ("layers.0.bias", "layers.1.bias", "lout.bias"))
+    F = W1.shape[1]
+    a1 = feat @ W1.T + b1
+    m1 = (a1 > 0).double()
+    a2 = (a1 * m1) @ W2.T + b2
+    m2 = (a2 > 0).double()
+    A1 = absfeat @ W1.abs().T + b1.abs()
+    A2 = (A1 * m1) @ W2.abs().T + b2.abs()
+    Ap = ((A2 * m2) @ w3.abs().T + b3.abs()).squeeze(1)
+    e1 = (8 * n_levels + 2) * U + eps_mm(F, tf32x1) + U
+    e2 = e1 + eps_mm(H, tf32x1) + U
+    efwd = e2 + eps_mm(H, tf32x1) + U
+    D = ((m2 * w3.abs()) @ W2.abs() * m1) @ W1.abs()
+    kink = ((a1.abs() <= 2 * e1 * A1).any(1) | (a2.abs() <= 2 * e2 * A2).any(1))
+    return {"A0": absfeat, "P": efwd * Ap, "D": D, "kink": kink, "ebwd": 2 * eps_mm(H, tf32x1) + 2 * U}
+
+
+def drop_kinks(case, tf32x1=False):
+    """The case without the points whose pre-activations lie within twice the forward error of a ReLU kink."""
+    o, dec = _oracle64(case)
+    coord = torch.from_numpy(case["coord"])
+    with torch.no_grad():
+        feat = o.query_feature(coord)
+        absfeat = _abs_feature(o, coord)
+        kink = _decoder_passes(feat, absfeat, dec, tf32x1, o.featured_level_num)["kink"].numpy()
+    return subset(case, ~kink), int(kink.sum())
+
+
+def _abs_feature(o, coord):
+    total = torch.zeros(coord.shape[0], o.feature_dim, dtype=torch.float64)
+    for i, (ix, w) in enumerate(_blend(o, coord)):
+        t = o.hier_features[o.featured_level_num - 1 - i].detach().abs()
+        total += (t[ix] * w[:, None]).reshape(coord.shape[0], 8, -1).sum(1)
+    return total
+
+
+class Ref:
+    """fp64 oracle step of a case (or the fp64 query backward of a given dfeat), with S, k and T per row."""
+
+    def __init__(self, case, dfeat=None, tf32x1=False, grouped=False):
+        c = case["cfg"]
+        o, dec = _oracle64(case)
+        coord = torch.from_numpy(case["coord"])
+        n, L, F = coord.shape[0], c["tree_level_feat"], c["feature_dim"]
+        self.n, self.tables, self.slack = n, case["tables"], C_SLACK + (eps_mm(16) / U if grouped else 0)
+        if dfeat is None:
+            label = torch.from_numpy(case["label"]).double()
+            weight = torch.from_numpy(case["weight"]).double()
+            res = orc.train_step(o, dec, coord, label, weight, c["sigma"], c["weighted"], c["reduction"])
+            self.want = [g.detach().numpy() for g in res["table_grads"]]
+            self.pred = res["pred"].numpy()
+            self.step = {"loss": float(res["loss"]), "dec_grads": {k: g.numpy() for k, g in res["dec_grads"].items()}}
+            feat = res["feature"].clone().requires_grad_(True)
+            dd = {k: v.detach() for k, v in dec.items()}
+            pred = orc.decoder_sdf(feat, dd)
+            loss = orc.sdf_bce_loss(pred, label, c["sigma"], weight.abs(), c["weighted"], c["reduction"])
+            dfeat64, g = torch.autograd.grad(loss, [feat, pred])
+            with torch.no_grad():
+                dp = _decoder_passes(feat.detach(), _abs_feature(o, coord), dd, tf32x1, L)
+                s = (weight.abs() if c["weighted"] else torch.ones(n, dtype=torch.float64))
+                s = s / n if c["reduction"] == "mean" else s
+                dg = s * (dp["P"] / 4 + 16 * U) + 4 * U * g.abs()
+                E = dp["D"] * (dp["ebwd"] * g.abs() + dg)[:, None]
+            self.P = dp["P"].numpy()
+            self.kinks = int(dp["kink"].sum())
+        else:
+            dfeat64 = torch.from_numpy(dfeat).double()
+            feat = o.query_feature(coord)
+            feat.backward(dfeat64)
+            self.want = [t.grad.numpy() for t in o.hier_features]
+            E = torch.zeros(n, F, dtype=torch.float64)
+            self.P, self.kinks = None, 0
+        pts = torch.arange(n).repeat_interleave(8)
+        self.S, self.k, self.T = [None] * L, [None] * L, [None] * L
+        for i, (ix, w) in enumerate(_blend(o, coord)):
+            kk = L - 1 - i
+            rows = self.want[kk].shape[0]
+            hit = ix >= 0
+            r, wj, pj = ix[hit], w[hit][:, None], pts[hit]
+            self.S[kk] = torch.zeros(rows, F, dtype=torch.float64).index_add_(0, r, wj * dfeat64.abs()[pj]).numpy()
+            self.T[kk] = torch.zeros(rows, F, dtype=torch.float64).index_add_(0, r, wj * E[pj]).numpy()
+            self.k[kk] = torch.bincount(r, minlength=rows).numpy()
+
+    def grade(self, got_tables, what, pred=None):
+        """Every element of every level (trash row excluded) against its bound -> worst error / bound."""
+        worst = 0.0
+        for kk, got in enumerate(got_tables):
+            got = np.asarray(got, dtype=np.float64)[:-1]
+            want, S, k, T = self.want[kk][:-1], self.S[kk][:-1], self.k[kk][:-1], self.T[kk][:-1]
+            bound = (k[:, None] + self.slack) * U * S + T
+            err = np.abs(got - want)
+            bad = np.argwhere(err > bound)
+            if bad.size:
+                r, f = bad[0]
+                raise AssertionError(
+                    f"{what}: level {kk} has {len(bad)} elements outside the bound; first: row {r} channel {f} got "
+                    f"{got[r, f]:.9g} want {want[r, f]:.9g} bound {bound[r, f]:.3g} (k_u = {k[r]}, S = {S[r, f]:.3g})")
+            if err.size:
+                worst = max(worst, float((err / np.where(bound > 0, bound, 1.0)).max()))
+        if pred is not None:
+            e = np.abs(np.asarray(pred, dtype=np.float64) - self.pred)
+            assert (e <= self.P).all(), f"{what}: pred outside its bound at {int((e > self.P).sum())} points"
+            print(f"[replica bounds] {what}: pred worst {float((e / self.P).max()):.3f} of the bound")
+        print(f"[replica bounds] {what}: table grads worst {worst:.3f} of the bound")
+        return worst
+
+    def compare(self, got_tables, pred, loss, dec_grads, tf32x1=False):
+        """compare_step on the same step (fp32-graded quantities: loss, pred, decoder gradients)."""
+        got = {"indices": [], "feature": np.zeros(0), "pred": pred, "loss": loss, "table_grads": got_tables,
+               "dec_grads": dec_grads}
+        want = {"indices": [], "feature": np.zeros(0), "pred": self.pred, "loss": self.step["loss"],
+                "table_grads": self.want, "dec_grads": {k: self.step["dec_grads"][k] for k in dec_grads}}
+        kw = dict(pred_atol=5e-3, pred_rtol=5e-3, grad_rel=3e-2) if tf32x1 else {}
+        return compare_step(got, want, **kw)
+
+
+# ---- running the kernels -------------------------------------------------------------------------------------------------
+
+def _dev(case):
+    return tuple(torch.from_numpy(case[k]).to(DEV) for k in ("coord", "label", "weight"))
+
+
+def trainer(case, freeze=False, **kw):
+    from shine_mapping_b200 import SdfTrainer
+    cfg, octree, dec = build_cuda_models(case, DEV, freeze_decoder=freeze)
+    tr = SdfTrainer(cfg, octree, dec, **kw)
+    tr.use_replicas = True
+    return tr, FoldSpy(octree)
+
+
+def train_step(tr, case, morton_ordered=None):
+    coord, label, weight = _dev(case)
+    tr.zero_grad()
+    pred = torch.empty(coord.shape[0], device=DEV)
+    loss = float(tr.forward_backward(coord, label, weight, pred_out=pred, morton_ordered=morton_ordered))
+    torch.cuda.synchronize()
+    tables = [g.detach().cpu().numpy().copy() for g in tr.table_grads]
+    dec = {k: g.detach().cpu().numpy().copy() for k, g in zip(("layers.0.weight", "layers.0.bias", "layers.1.weight",
+                                                                "layers.1.bias", "lout.weight", "lout.bias"), tr.dec_grads)
+           if g is not None and tr._dec_trainable}
+    return tables, pred.cpu().numpy(), loss, dec
+
+
+def check_step(tr, spy, case, ref, what, tf32x1=False, morton_ordered=None):
+    """One trainer step: R per level as expected, every element within its bound, compare_step, scratch all zero."""
+    tables, pred, loss, dec = train_step(tr, case, morton_ordered)
+    spy.expect(expected_replicas(case["tables"], ref.n), what)
+    worst = ref.grade(tables, what, pred)
+    print(what, ref.compare(tables, pred, loss, dec, tf32x1))
+    assert_scratch_zero(tr.octree, what)
+    return worst
+
+
+def query_bwd(octree, case, dfeat):
+    coord = torch.from_numpy(case["coord"]).to(DEV)
+    feature = octree.query_feature(coord)
+    grads = torch.autograd.grad(feature, list(octree.hier_features), torch.from_numpy(dfeat).to(DEV))
+    torch.cuda.synchronize()
+    return [g.cpu().numpy() for g in grads]
+
+
+def random_dfeat(n, F, seed):
+    g = np.random.default_rng(seed)
+    return (g.standard_normal((n, F)) * 10.0 ** g.uniform(-2, 2, (n, F))).astype(np.float32)
+
+
+def check_query_bwd(octree, spy, case, ref, dfeat, what):
+    got = query_bwd(octree, case, dfeat)
+    spy.expect(expected_replicas(case["tables"], ref.n), what)
+    ref.grade(got, what)
+    scale = [max(float(np.abs(w[:-1]).max()), 1e-30) for w in ref.want]
+    for kk, (a, b) in enumerate(zip(got, ref.want)):
+        assert float(np.abs(a[:-1] - b[:-1]).max()) <= 2e-4 * scale[kk], f"{what}: level {kk} beyond 2e-4 of its maximum"
+    assert_scratch_zero(octree, what)
+
+
+# ---- fused kernels at forced R ------------------------------------------------------------------------------------------
+
+@gpu
+@pytest.mark.parametrize("rmax", [2, 4, 8, 16, 32, 64])
+def test_general_kernel_at_every_replica_count(rmax, force):
+    """The LMAX = 8 general kernel (6 levels) with the coarsest level at R = rmax and the finer ones at smaller R: every tail
+    split of the fold's 8-wide loop (nrep = 1, 3, 7, 15, 31, 63)."""
+    force(1, rmax)
+    case, dropped = drop_kinks(make_case(n_points=2500, n_batch=3000, feat_levels=6, seed=60 + rmax))
+    assert expected_replicas(case["tables"], case["coord"].shape[0])[0] == rmax
+    tr, spy = trainer(case)
+    check_step(tr, spy, case, Ref(case), f"general L=6 R<={rmax} (kinks dropped: {dropped})")
+
+
+@gpu
+@pytest.mark.parametrize("levels", [3, 8])
+@pytest.mark.parametrize("variant,weighted,reduction", [("tf32x1", False, "mean"), ("frozen", True, "sum"),
+                                                        ("biasless", True, "mean"), ("plain", False, "sum")])
+def test_general_kernel_variants(levels, variant, weighted, reduction, force):
+    """L <= 4 and L > 4 instantiations with plain TF32, a frozen decoder (no decoder gradients) and a bias-less decoder.
+    Plain TF32 puts many points within its forward error of a ReLU kink, hence the larger batch."""
+    force(1, 64)
+    tf32x1 = variant == "tf32x1"
+    case = make_case(n_points=2500, n_batch=12000 if tf32x1 else 3000, feat_levels=levels, seed=70 + levels,
+                     weighted=weighted, reduction=reduction, bias=variant != "biasless", n_frames=2 if levels == 8 else 1)
+    case, dropped = drop_kinks(case, tf32x1)
+    tr, spy = trainer(case, freeze=variant == "frozen", tf32x1=tf32x1)
+    check_step(tr, spy, case, Ref(case, tf32x1=tf32x1), f"general L={levels} {variant} (kinks dropped: {dropped})", tf32x1)
+
+
+@gpu
+@pytest.mark.parametrize("ordered", [True, False])
+def test_grouped_kernel_with_replicas(ordered, force):
+    """The voxel-grouped kernel with `grouped_replicas`: replica by tile, per-node 3xTF32 sums (Morton-ordered batch) and
+    its per-point fall-back (batch in the order drawn)."""
+    force(1, 64)
+    case = make_case(n_points=2500, n_batch=6000, feat_levels=4, seed=81)
+    if ordered:
+        case = sort_case_morton(case)
+    case, dropped = drop_kinks(case)
+    tr, spy = trainer(case, morton_ordered=True)
+    tr.grouped_replicas = True
+    check_step(tr, spy, case, Ref(case, grouped=True), f"grouped ordered={ordered} (kinks dropped: {dropped})",
+               morton_ordered=True)
+
+
+@gpu
+@pytest.mark.parametrize("levels,n_batch,frozen", [(2, 3000, False), (4, 5000, False), (4, 4000, True)])
+def test_wgmma_kernel_with_replicas(levels, n_batch, frozen, force):
+    force(1, 64)
+    case, dropped = drop_kinks(make_case(n_points=2500, n_batch=n_batch, feat_levels=levels, seed=90 + levels))
+    tr, spy = trainer(case, freeze=frozen, tcgen05=True)
+    check_step(tr, spy, case, Ref(case), f"wgmma L={levels} frozen={frozen} (kinks dropped: {dropped})")
+
+
+@gpu
+@pytest.mark.parametrize("feature_dim", [4, 8, 16])
+def test_query_bwd_with_replicas(feature_dim, force):
+    """The class-surface backward (`shine_query_bwd`, LP = F / 4 lanes per point) with replicas."""
+    force(1, 64)
+    case = make_case(n_points=2000, n_batch=3000, feat_levels=4, seed=100 + feature_dim, feature_dim=feature_dim)
+    cfg, octree, dec = build_cuda_models(case, DEV)
+    spy = FoldSpy(octree)
+    dfeat = random_dfeat(case["coord"].shape[0], feature_dim, feature_dim)
+    check_query_bwd(octree, spy, case, Ref(case, dfeat=dfeat), dfeat, f"query_bwd F={feature_dim}")
+
+
+# ---- natural size: no patch -----------------------------------------------------------------------------------------------
+
+@pytest.fixture(scope="module")
+def natural_case():
+    return make_case(n_points=2500, n_batch=50000, feat_levels=8, seed=58, n_frames=2)
+
+
+@gpu
+def test_natural_size_general_kernel(natural_case):
+    """50 000 points at L = 8 switch replicas on by themselves: R = 16 / 8 / 4 / 2 on the four coarsest levels."""
+    case, dropped = drop_kinks(natural_case)
+    assert expected_replicas(case["tables"], case["coord"].shape[0])[:4] == [16, 8, 4, 2]
+    tr, spy = trainer(case)
+    check_step(tr, spy, case, Ref(case), f"natural L=8 general (kinks dropped: {dropped})")
+
+
+@gpu
+def test_natural_size_query_bwd(natural_case):
+    case = natural_case
+    assert expected_replicas(case["tables"], case["coord"].shape[0])[:4] == [16, 8, 4, 2]
+    cfg, octree, dec = build_cuda_models(case, DEV)
+    spy = FoldSpy(octree)
+    dfeat = random_dfeat(case["coord"].shape[0], 8, 5)
+    check_query_bwd(octree, spy, case, Ref(case, dfeat=dfeat), dfeat, "natural L=8 query_bwd")
+
+
+# ---- scratch lifecycle ---------------------------------------------------------------------------------------------------
+
+@gpu
+def test_consecutive_steps(force):
+    """Three steps in a row on the same trainer, the batch permuted in between (other warps, other replicas); a fold that
+    leaves a replica dirty doubles that replica's share in the next step."""
+    force(1, 64)
+    case, _ = drop_kinks(make_case(n_points=2500, n_batch=3000, feat_levels=6, seed=111))
+    tr, spy = trainer(case)
+    rng = np.random.default_rng(0)
+    for s in range(3):
+        batch = case if s == 0 else subset(case, rng.permutation(case["coord"].shape[0]))
+        check_step(tr, spy, batch, Ref(batch), f"consecutive step {s}")
+
+
+@gpu
+def test_batch_size_changes_replica_count(force):
+    force(4, 64)
+    case, _ = drop_kinks(make_case(n_points=2500, n_batch=6000, feat_levels=6, seed=112))
+    small = subset(case, np.arange(0, case["coord"].shape[0], 5))
+    assert expected_replicas(case["tables"], case["coord"].shape[0]) != expected_replicas(small["tables"],
+                                                                                          small["coord"].shape[0])
+    refs = {"full": Ref(case), "fifth": Ref(small)}
+    tr, spy = trainer(case)
+    for name in ("full", "fifth", "full", "fifth"):
+        check_step(tr, spy, case if name == "full" else small, refs[name], f"batch {name}")
+
+
+def _first_frame_case(case):
+    """The case after its first frame only: the oracle's tables are append-only, so its rows are a prefix of the final ones."""
+    c0 = dict(case)
+    c0["frames"] = case["frames"][:1]
+    o = orc.OracleOctree(case["cfg"]["tree_level_world"], case["cfg"]["tree_level_feat"], case["cfg"]["feature_dim"])
+    o.update(torch.from_numpy(np.asarray(c0["frames"][0])))
+    c0["tables"] = [np.concatenate((t[:f.shape[0] - 1], np.zeros_like(t[-1:]))) for t, f in zip(case["tables"], o.hier_features)]
+    return c0
+
+
+@gpu
+def test_step_after_update_grows_the_tables(force):
+    """update() grows every level: the replica stride (rows x F) changes, the scratch is either reused at the new stride
+    (R lowered) or reallocated (R raised)."""
+    force(1, 64)
+    case, _ = drop_kinks(make_case(n_points=2500, n_batch=4000, feat_levels=4, seed=113, n_frames=2))
+    c0 = _first_frame_case(case)
+    assert all(a.shape[0] < b.shape[0] for a, b in zip(c0["tables"], case["tables"]))
+    tr, spy = trainer(c0)
+    octree = tr.octree
+    check_step(tr, spy, c0, Ref(c0), "before update")
+    before = {k: (b.data_ptr(), b.numel()) for k, b in octree._grad_scratch.items()}
+    octree.update(torch.from_numpy(np.asarray(case["frames"][1])).to(DEV))
+    with torch.no_grad():
+        for p, t in zip(octree.hier_features, case["tables"]):
+            p.copy_(torch.from_numpy(t))
+    ref = Ref(case)
+    force(1, 16)
+    check_step(tr, spy, case, ref, "after update, R <= 16")
+    reused = sum(before[k] == (b.data_ptr(), b.numel()) for k, b in octree._grad_scratch.items())
+    force(1, 64)
+    octree._desc_cache = {}
+    check_step(tr, spy, case, ref, "after update, R <= 64")
+    print("scratch buffers reused at the new stride:", reused, "of", len(before))
+
+
+@gpu
+def test_two_trainers_alternate_on_one_octree(force):
+    """The general and the wgmma trainer on one octree share its replica scratch."""
+    from shine_mapping_b200 import SdfTrainer
+    force(1, 64)
+    case, _ = drop_kinks(make_case(n_points=2500, n_batch=4000, feat_levels=4, seed=114))
+    ref = Ref(case)
+    tr1, spy = trainer(case)
+    tr2 = SdfTrainer(tr1.config, tr1.octree, tr1.decoder, tcgen05=True)
+    tr2.use_replicas = True
+    for s, tr in enumerate((tr1, tr2, tr1, tr2)):
+        check_step(tr, spy, case, ref, f"alternating step {s} ({'wgmma' if tr.tcgen05 else 'general'})")
+
+
+@gpu
+def test_class_surface_backward_between_trainer_steps(force):
+    force(1, 64)
+    case, _ = drop_kinks(make_case(n_points=2500, n_batch=4000, feat_levels=5, seed=115))
+    ref = Ref(case)
+    dfeat = random_dfeat(case["coord"].shape[0], 8, 1)
+    qref = Ref(case, dfeat=dfeat)
+    tr, spy = trainer(case)
+    check_step(tr, spy, case, ref, "trainer step before the class surface")
+    check_query_bwd(tr.octree, spy, case, qref, dfeat, "class-surface backward")
+    check_step(tr, spy, case, ref, "trainer step after the class surface")
+
+
+@gpu
+def test_step_from_host_chunks_with_different_replica_counts(force):
+    """step_from_host(chunks=3) with n = 3m + 2: chunks of m, m + 1 and m + 1 points, and a target chosen so that the
+    coarsest level flips from R = 32 to R = 64 between m and m + 1."""
+    case, _ = drop_kinks(make_case(n_points=2500, n_batch=70000, feat_levels=4, seed=116, n_frames=2))
+    rows0 = case["tables"][0].shape[0]
+    target = max(1, round(8 * 22000 / (64 * rows0)))
+    m = -(-64 * rows0 * target // 8) - 1                    # 8 m < 64 rows0 target <= 8 (m + 1)
+    n = 3 * m + 2
+    assert 65536 < n <= case["coord"].shape[0]
+    case = subset(case, np.arange(n))
+    force(target, 64)
+    chunks = [(n * k // 3, n * (k + 1) // 3) for k in range(3)]
+    want = [expected_replicas(case["tables"], e - b) for b, e in chunks]
+    assert [r[0] for r in want] == [32, 64, 64], want
+    tr, spy = trainer(case)
+    coord_h = torch.from_numpy(case["coord"]).pin_memory(); label_h = torch.from_numpy(case["label"]).pin_memory()
+    tr.step_from_host(coord_h, label_h, chunks=3)
+    torch.cuda.synchronize()
+    assert spy.calls[:3] == want, f"chunks ran with R = {spy.calls[:3]}, expected {want}"
+    ref = Ref(case)
+    ref.grade([g.detach().cpu().numpy() for g in tr.table_grads], "step_from_host chunks=3")
+    assert_scratch_zero(tr.octree, "step_from_host")
+
+
+@gpu
+def test_capture_step_replays_on_changed_data(force):
+    force(1, 64)
+    case, _ = drop_kinks(make_case(n_points=2500, n_batch=6000, feat_levels=6, seed=117))
+    n = case["coord"].shape[0] // 2
+    a, b = subset(case, np.arange(n)), subset(case, np.arange(n, 2 * n))
+    refs = {"A": Ref(a), "B": Ref(b)}
+    tr, spy = trainer(a)
+    coord, label, weight = _dev(a)
+    graph = tr.capture_step(coord, label, weight, exchange=False)
+    spy.expect(expected_replicas(a["tables"], n), "capture")
+    refs["A"].grade([g.detach().cpu().numpy() for g in tr.table_grads], "capture warm-up on A")
+    for name in ("B", "A", "B"):
+        src = _dev(b if name == "B" else a)
+        for dst, s in zip((coord, label, weight), src):
+            dst.copy_(s)
+        graph.replay()
+        torch.cuda.synchronize()
+        refs[name].grade([g.detach().cpu().numpy() for g in tr.table_grads], f"replay on {name}")
+        assert_scratch_zero(tr.octree, f"replay on {name}")
+
+
+# ---- the fold kernel on its own, bit-exact ---------------------------------------------------------------------------------
+
+F_FOLD = 8
+BIG_ROWS = 150_000              # rows * F / 4 = 300 000 float4 > 132 SMs * 8 blocks * 256 threads: the grid-stride loop wraps
+
+
+def fold_levels(rmax):
+    """(rows, R, has_grads) of the hand-built descriptor: R = rmax, a second R, R = 1 (skipped), a level without
+    gradients (skipped, its replicas untouched) and the big level."""
+    return [(37, rmax, True), (1000, 1, True), (513, max(2, rmax // 4), True), (2000, rmax, False),
+            (BIG_ROWS, rmax, True)]
+
+
+def fold_data(rows, r, seed):
+    """main [rows, F] and replicas [r - 1, rows, F], fp32 over twelve decades with both signs: sums depend on their order."""
+    g = np.random.default_rng(seed)
+    shape = (r, rows, F_FOLD)
+    x = g.standard_normal(shape, dtype=np.float32)
+    x *= np.power(np.float32(10), g.random(shape, dtype=np.float32) * np.float32(12) - np.float32(6))
+    return x[0], x[1:]
+
+
+def fold_model(main, reps):
+    """The fold's fixed order in fp32: main, then replicas 0 .. nrep - 1."""
+    acc = main.copy()
+    for rep in reps:
+        acc = acc + rep
+    return acc
+
+
+@pytest.mark.parametrize("r", [2, 4, 8, 16, 32, 64])
+def test_fold_model_is_order_sensitive(r):
+    """The numpy model of the fold, on the data the GPU test uses: within the fp64 bound of its nrep adds, and different
+    (bit for bit) from a fold that skips a replica, adds them in another order, or sums the replicas before the main table,
+    so that the bit-exact GPU comparison would see each of those."""
+    main, reps = fold_data(513, r, r)
+    got = fold_model(main, reps)
+    exact = main.astype(np.float64) + reps.astype(np.float64).sum(0)
+    mag = np.abs(main).astype(np.float64) + np.abs(reps).astype(np.float64).sum(0)
+    assert (np.abs(got - exact) <= (r - 1) * U * mag * 1.0001).all()
+    alternatives = {"skip last": fold_model(main, reps[:-1]), "reversed": fold_model(main, reps[::-1]),
+                    "replicas first": fold_model(np.zeros_like(main), np.concatenate((reps, main[None]))),
+                    "skip first": fold_model(main, reps[1:])}
+    for name, alt in alternatives.items():
+        if name in ("reversed", "replicas first") and r == 2:
+            continue            # one replica: the order of two fp32 terms does not change their sum
+        assert not np.array_equal(alt, got), f"R={r}: the data cannot tell the fold from '{name}'"
+
+
+@gpu
+@pytest.mark.parametrize("r", [2, 4, 8, 16, 32, 64])
+def test_fold_kernel_is_bit_exact(r, built_lib):
+    from shine_mapping_b200 import _abi
+    levels = fold_levels(r)
+    d = _abi.ShineOctree()
+    d.num_levels, d.feature_dim = len(levels), F_FOLD
+    keep, host = [], []
+    hash_slots = torch.zeros(16 * _abi.HASH_SLOT_BYTES, dtype=torch.uint8, device=DEV)
+    for i, (rows, rr, has_grads) in enumerate(levels):
+        main, reps = fold_data(rows, rr, 1000 * r + i)
+        feats = torch.zeros(rows, F_FOLD, device=DEV)
+        g = torch.from_numpy(main).to(DEV) if has_grads else None
+        rep = torch.from_numpy(np.ascontiguousarray(reps)).to(DEV) if rr > 1 else None
+        lv = d.lv[i]
+        lv.hash_slots, lv.features, lv.hash_capacity, lv.rows, lv.level = hash_slots.data_ptr(), feats.data_ptr(), 16, rows, 12 - i
+        lv.feature_grads = g.data_ptr() if g is not None else None
+        lv.num_replicas = rr
+        lv.grad_replicas = rep.data_ptr() if rep is not None else None
+        keep.append((feats, g, rep))
+        host.append((main, reps))
+    assert built_lib.shine_reduce_grad_replicas(C.byref(d), _abi.stream_ptr(DEV)) == 0
+    torch.cuda.synchronize()
+    for i, ((rows, rr, has_grads), (feats, g, rep), (main, reps)) in enumerate(zip(levels, keep, host)):
+        if has_grads:
+            want = fold_model(main, reps) if rr > 1 else main
+            got = g.cpu().numpy()
+            bad = np.argwhere(got.view(np.uint32) != want.view(np.uint32))
+            assert bad.size == 0, f"level {i} (rows {rows}, R {rr}): {len(bad)} elements differ from the model, first {bad[0]}"
+            if rep is not None:
+                assert int(torch.count_nonzero(rep)) == 0, f"level {i}: replicas not re-zeroed"
+        else:   # no gradient table: the level is skipped and its replicas stay as they were
+            assert np.array_equal(rep.cpu().numpy(), reps), f"level {i} without gradients was touched"
+
+
+# ---- ABI rejections (no GPU: the descriptor checks run before any device call) -------------------------------------------------
+
+def _abi_call(lib, name, desc):
+    from shine_mapping_b200 import _abi
+    dec = _abi.ShineDecoder()
+    dec.w1 = dec.w2 = dec.w3 = 0x1000
+    dec.in_dim, dec.hidden, dec.mlp_level = 8, 32, 2
+    o = C.byref(desc)
+    if name == "shine_sdf_bce_step":
+        return lib.shine_sdf_bce_step(o, C.byref(dec), None, None, None, 0, 1.0, 1.0, None, None, None, 0, None)
+    if name == "shine_sdf_bce_eikonal_step":
+        return lib.shine_sdf_bce_eikonal_step(o, C.byref(dec), None, None, None, 0, 1.0, 1.0, 0.1, None, None, None, None,
+                                              None, 0, None)
+    if name == "shine_query_bwd":
+        return lib.shine_query_bwd(o, None, 0, None, None)
+    return lib.shine_reduce_grad_replicas(o, None)
+
+
+@pytest.mark.parametrize("name", ["shine_sdf_bce_step", "shine_query_bwd", "shine_reduce_grad_replicas",
+                                  "shine_sdf_bce_eikonal_step"])
+def test_abi_replica_checks(name, built_lib):
+    """R must be a power of two up to 64 with a scratch pointer; R = 0 and 1 need no scratch.  Placeholder pointers and an
+    empty batch: an accepted descriptor returns OK without touching the device."""
+    from shine_mapping_b200 import _abi
+    d = _abi.ShineOctree()
+    d.num_levels, d.feature_dim = 2, 8
+    for lv in d.lv[:2]:
+        lv.hash_slots = lv.features = lv.feature_grads = 0x1000
+        lv.hash_capacity, lv.rows, lv.level = 16, 10, 12
+    for r in (0, 1):
+        d.lv[1].num_replicas, d.lv[1].grad_replicas = r, None
+        assert _abi_call(built_lib, name, d) == 0, f"R = {r} without scratch was refused"
+    for r in (3, 65, 128):
+        d.lv[1].num_replicas, d.lv[1].grad_replicas = r, 0x2000
+        assert _abi_call(built_lib, name, d) == INVALID, f"R = {r} was accepted"
+    d.lv[1].num_replicas, d.lv[1].grad_replicas = 2, None
+    assert _abi_call(built_lib, name, d) == INVALID, "R = 2 without scratch was accepted"
+    d.lv[1].grad_replicas = 0x2000
+    d.lv[0].num_replicas, d.lv[0].grad_replicas = 64, None
+    assert _abi_call(built_lib, name, d) == INVALID, "a bad first level was accepted"
+
+
+# ---- the bound itself -------------------------------------------------------------------------------------------------------
+
+def test_bound_passes_the_fp32_oracle_and_sees_one_lost_term():
+    """The fp32 oracle (a correct fp32 implementation in another summation order) is inside the bound; the same gradients
+    with one (point, corner) term taken out of a row that several points touch, or added twice, are not."""
+    from tests.parity_utils import run_oracle_step
+    case, _ = drop_kinks(make_case(n_points=1500, n_batch=1500, feat_levels=3, seed=5))
+    ref = Ref(case)
+    got = run_oracle_step(case)["table_grads"]
+    ref.grade(got, "fp32 oracle")
+    o, dec = _oracle64(case)
+    coord = torch.from_numpy(case["coord"])
+    ix, w = _blend(o, coord)[0]                    # leaf level = table L - 1
+    kk = len(got) - 1
+    feat = o.query_feature(coord).detach().requires_grad_(True)
+    c = case["cfg"]
+    pred = orc.decoder_sdf(feat, {k: v.detach() for k, v in dec.items()})
+    loss = orc.sdf_bce_loss(pred, torch.from_numpy(case["label"]).double(), c["sigma"],
+                            torch.from_numpy(case["weight"]).double().abs(), c["weighted"], c["reduction"])
+    dfeat = torch.autograd.grad(loss, feat)[0]
+    terms = (w[:, None] * dfeat.repeat_interleave(8, 0)).numpy()          # w_{j,c} dfeat_j of every (point, corner)
+    rows = ix.numpy()
+    # a median-sized term in a row that three or more terms touch
+    cand = [j for j in range(len(rows)) if rows[j] >= 0 and ref.k[kk][rows[j]] >= 3 and np.abs(terms[j]).max() > 0]
+    cand.sort(key=lambda j: np.abs(terms[j]).max())
+    j = cand[len(cand) // 2]
+    term = terms[j]
+    for sign, name in ((-1.0, "lost"), (1.0, "duplicated")):
+        bad = [t.copy() for t in got]
+        bad[kk][rows[j]] += sign * term.astype(np.float32)
+        with pytest.raises(AssertionError, match="outside the bound"):
+            ref.grade(bad, f"one {name} term")
