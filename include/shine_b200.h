@@ -271,6 +271,30 @@ int shine_regularization_apply(const shine_octree* oct, const shine_touched* tou
 int shine_importance_accumulate(const shine_octree* oct, const shine_touched* touched, const shine_row_tables* aux,
                                 int32_t zero_grads, int32_t clear_marks, void* stream);
 
+/* ---- the sample pool of incremental mapping with replay (continual.window_replay_on) -------------------------------
+ * Structure of arrays, fp32, device memory of one GPU; samples [0, size) are the pool, [size, capacity) free room. */
+typedef struct shine_sample_pool {
+    float* coord; float* label; float* weight;   /* [capacity,3], [capacity], [capacity] fp32, device                  */
+    int64_t size, capacity;
+} shine_sample_pool;
+
+/* Bytes of caller scratch that shine_pool_window_append needs for size + n_new samples (tile counter and one status word
+ * per 2048-sample tile); SHINE_ERR_INVALID_ARG for a negative count. */
+int64_t shine_pool_scratch_bytes(int64_t n_total);
+
+/* Replaces dataset/lidar_dataset.py:237-251 (drop the pool samples at `window_radius * scale` or more from the new frame's
+ * origin: `(coord_pool - origin).norm(2, dim=-1) < r` and the masked gathers of coord, weight and sdf_label) followed by
+ * :263-270 (`torch.cat` of the frame's samples), as ONE launch, in place, in the reference's order:
+ *   pool = [old samples with sqrt((dx*dx + dy*dy) + dz*dz) < radius, fp32 without contraction | the n_new frame samples]
+ * radius is the fp32 value the reference compares with (float32(window_radius * scale), the product taken in double);
+ * the comparison is strict and a NaN coordinate is dropped.  The new size goes to the device int64 *size_out.
+ * pool->size + n_new must not exceed pool->capacity.  The frame buffers (coord [n_new,3], label, weight) must not overlap
+ * the pool; they are device memory of the pool's GPU or pinned host memory.  scratch: >= shine_pool_scratch_bytes of
+ * size + n_new, 8-byte aligned, device memory of the pool's GPU; cleared on `stream` by this call. */
+int shine_pool_window_append(const shine_sample_pool* pool, const float* coord, const float* label, const float* weight,
+                             int64_t n_new, float ox, float oy, float oz, float radius, int64_t* size_out, void* scratch,
+                             int64_t scratch_bytes, void* stream);
+
 /* ---- multi-GPU exchange (SURVEY.md 8e, 8b export (6); the reference is single-GPU) --------------------------------
  * One process per GPU.  The map is partitioned by Morton prefix at the coarsest featured level; every rank owns the
  * rows reachable from its blocks, so corner rows on a face between two blocks exist on both ranks.  Their gradients

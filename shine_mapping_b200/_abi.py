@@ -92,6 +92,11 @@ class ShineBoundaryInverse(C.Structure):
                 ("holders", C.c_void_p * MAX_LEVELS)]
 
 
+class ShineSamplePool(C.Structure):
+    _fields_ = [("coord", C.c_void_p), ("label", C.c_void_p), ("weight", C.c_void_p), ("size", C.c_int64),
+                ("capacity", C.c_int64)]
+
+
 # name -> (restype, argtypes); every symbol declared in include/shine_b200.h
 _vp, _i64, _i32, _u32, _f32 = C.c_void_p, C.c_int64, C.c_int32, C.c_uint32, C.c_float
 _OCT, _DEC = C.POINTER(ShineOctree), C.POINTER(ShineDecoder)
@@ -136,6 +141,9 @@ SYMBOLS = {
     "shine_p2p_destroy": (C.c_int, [_vp]),
     "shine_adam_step": (C.c_int, [C.POINTER(ShineAdamTensor), _i32, _f32, _f32, _f32, _i32, _i32, _vp]),
     "shine_adam_step_dev": (C.c_int, [C.POINTER(ShineAdamTensor), _i32, _f32, _f32, _f32, _vp, _i32, _vp]),
+    "shine_pool_scratch_bytes": (C.c_int64, [_i64]),
+    "shine_pool_window_append": (C.c_int, [C.POINTER(ShineSamplePool), _vp, _vp, _vp, _i64, _f32, _f32, _f32, _f32, _vp,
+                                           _vp, _i64, _vp]),
 }
 
 _lib = None

@@ -11,6 +11,14 @@ With `ekional_loss_on` (the reference's replay configs set it) the step is the f
 The BCE part is the fused sm_90a step; the regulariser (model/feature_octree.py:246-255) and the importance update touch
 only the rows the batch touched: `shine_mark_touched` collects them (bitmap + compact list, no unique()/sort) and
 `shine_regularization_apply` / `shine_importance_accumulate` run over that list.
+
+With `continual_learning_reg: False` the reference replays instead (the other half of its shipped incremental configs,
+`*_incre_replay.yaml`): the pool keeps every earlier frame's samples, minus, with `window_replay_on`, those outside a
+sliding window around the new sensor origin; pass a `synth.ReplayPool` as `pool`.
+
+    python -m shine_mapping_b200.incre_loop config.yaml [--synthetic-azimuth N --frames F --frame-step-m S --iters I]
+
+runs either mode, as the config selects it, on a synthetic drive along +x and prints the per-frame history.
 """
 from __future__ import annotations
 
@@ -112,29 +120,46 @@ def cal_feature_importance(trainer: SdfTrainer, octree: FeatureOctree, coord_poo
 
 
 def run_shine_mapping_incremental(config: SHINEConfig, octree: FeatureOctree, decoder: Decoder, frames, iters=None,
-                                  log=None):
+                                  log=None, pool=None):
     """frames: iterable of (coord, sdf_label, weight) sample sets, one per scan (what `process_frame` leaves in the
-    pools).  Returns per-frame dicts with first/last loss (and first/last eikonal mean with ekional_loss_on)."""
+    pools).  Returns per-frame dicts with first/last loss (and first/last eikonal mean with ekional_loss_on).
+
+    pool: a `synth.ReplayPool` (or anything with its `add_frame` / `get_batch` / `len`) selects the reference's replay mode
+    (`continual_learning_reg: False`, dataset/lidar_dataset.py:235-271): frames are then (coord, sdf_label, weight,
+    origin_scaled), the pool keeps the earlier frames' samples, dropping with `window_replay_on` those `window_radius`
+    metres or more from the new frame's origin, and batches are drawn from the whole pool.  The history also records
+    the pool size."""
+    if pool is not None and config.continual_learning_reg:
+        raise ValueError("continual_learning_reg keeps the current frame's samples only; a replay pool is the other "
+                         "incremental mode (dataset/lidar_dataset.py:223 vs :235): pass pool=None or turn the "
+                         "regularisation off")
     if config.continual_learning_reg:
         config.loss_reduction = "sum"          # reference shine_incre.py:77-78
     iters = config.iters if iters is None else iters
+    window = config.window_radius * config.scale if config.window_replay_on else None    # lidar_dataset.py:237-239
     dev = None
     history = []
-    for fid, (coord, label, weight) in enumerate(frames):
+    for fid, frame in enumerate(frames):
+        coord, label, weight = frame[:3]
         if fid == config.freeze_after_frame:   # reference shine_incre.py:97-101
             for child in decoder.children():
                 for p in child.parameters():
                     p.requires_grad = False
         surface = coord[weight > 0, :]
         octree.update(surface, incremental_on=config.continual_learning_reg)        # lidar_dataset.py:212-218
+        if pool is not None:
+            pool.add_frame(coord, label, weight, frame[3], window)                  # lidar_dataset.py:235-271
         trainer = SdfTrainer(config, octree, decoder)                               # fresh Adam state per frame
         dev = trainer.flat_grad.device
         trainer.zero_grad()
         first = last = None
         n = coord.shape[0]
         for it in range(iters):
-            index = torch.randint(0, n, (config.bs,), device=dev)
-            c, l, w = coord[index], label[index], weight[index]
+            if pool is not None:
+                c, l, w = pool.get_batch(config.bs)                                 # lidar_dataset.py:431-448
+            else:
+                index = torch.randint(0, n, (config.bs,), device=dev)
+                c, l, w = coord[index], label[index], weight[index]
             if config.ekional_loss_on:                                              # shine_incre.py:159-165
                 loss, eik = trainer.forward_backward_eikonal(c, l, w)
                 total = loss + config.weight_e * eik
@@ -153,8 +178,45 @@ def run_shine_mapping_incremental(config: SHINEConfig, octree: FeatureOctree, de
             cal_feature_importance(trainer, octree, coord, label, config.bs, config.cal_importance_weight_down_rate)
         history.append({"frame": fid, "loss_first": first, "loss_last": last, "bce_first": bce_first, "bce_last": bce_last,
                         "rows": [int(p.shape[0]) for p in octree.hier_features]})
+        if pool is not None:
+            history[-1]["pool"] = len(pool)
         if config.ekional_loss_on:
             history[-1].update(eik_first=eik_first, eik_last=eik_last)
         if log:
             log(history[-1])
     return history
+
+
+def main(argv=None):
+    import argparse
+    from . import synth
+    from .batch_loop import check_supported
+    ap = argparse.ArgumentParser(description="Incremental mapping on a synthetic drive along +x (regularisation or replay, "
+                                             "as the config selects)")
+    ap.add_argument("config")
+    ap.add_argument("--synthetic-azimuth", type=int, default=1024)
+    ap.add_argument("--frames", type=int, default=10)
+    ap.add_argument("--frame-step-m", type=float, default=2.0)
+    ap.add_argument("--iters", type=int, default=None)
+    args = ap.parse_args(argv)
+    config = SHINEConfig()
+    config.load(args.config)
+    check_supported(config)
+    torch.manual_seed(config.seed)
+    octree, decoder = FeatureOctree(config), Decoder(config)
+    dev = config.device
+    # shine_incre.py:106: the regularisation mode keeps the current frame's samples only, the other mode replays
+    pool = None if config.continual_learning_reg else synth.ReplayPool(dev)
+    scans = synth.generate_scans(config, args.synthetic_azimuth, args.frames, args.frame_step_m, seed=config.seed,
+                                 device=dev)
+    frames = [(coord, label, weight, torch.tensor([f * args.frame_step_m, 0.0, 0.0]) * config.scale)
+              for f, (coord, label, weight, _) in enumerate(scans)]
+    print("Begin mapping:", "replay" + (f" (window {config.window_radius} m)" if config.window_replay_on else "")
+          if pool is not None else "regularisation")
+    history = run_shine_mapping_incremental(config, octree, decoder, frames, iters=args.iters, log=print, pool=pool)
+    octree.print_detail()
+    return history
+
+
+if __name__ == "__main__":
+    main()

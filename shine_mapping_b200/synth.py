@@ -9,10 +9,13 @@
                       +1 for surface samples, -1 for free-space samples (:104); ray-wise output order (:123-134).
 * `SamplePool`      — the device sample pools and `get_batch()` of `LiDARDataset`
                       (dataset/lidar_dataset.py:104-113,431-448): `torch.randint` gather.
+* `ReplayPool`      — the pool of incremental mapping with replay: earlier frames' samples kept, those outside the
+                      sliding window dropped on the GPU before the frame is appended (dataset/lidar_dataset.py:235-271).
 * `build_scene_map` — scans -> samples -> `octree.update(surface samples)` (dataset/lidar_dataset.py:204-218).
 """
 from __future__ import annotations
 
+import ctypes as C
 import math
 
 import torch
@@ -146,6 +149,91 @@ class SamplePool:
         elif ordered:
             raise ValueError("ordered batches need a pool in Morton order: call sort_morton() first")
         return self.coord_pool[index, :], self.sdf_label_pool[index], self.weight_pool[index]
+
+
+class ReplayPool(SamplePool):
+    """The pool of incremental mapping with replay (`continual_learning_reg: False`, dataset/lidar_dataset.py:235-271):
+    every earlier frame's samples stay; with a window (`window_replay_on`) the ones `window_radius * scale` or more from
+    the new sensor origin are dropped before the new frame is appended behind the survivors, in the reference's order.
+
+    The samples live in capacity buffers that grow by about 1.5x; `coord_pool` / `sdf_label_pool` / `weight_pool` are
+    views `[:size]` of them, so `get_batch` is SamplePool's: the reference's `torch.randint` draw, in the order drawn.
+    With a window, `add_frame` is one launch of `shine_pool_window_append` (filter and append in place) and reading the
+    new size back is its only host synchronisation; without one, the frame is copied behind the old samples."""
+
+    GROWTH = 1.5
+
+    def __init__(self, device, capacity: int = 0):
+        super().__init__(device)
+        self._coord = torch.empty(capacity, 3, device=device)
+        self._label = torch.empty(capacity, device=device)
+        self._weight = torch.empty(capacity, device=device)
+        self._scratch = None
+        self._size_out = None
+        self._set_size(0)
+
+    @property
+    def capacity(self) -> int:
+        return self._label.shape[0]
+
+    def _set_size(self, n: int) -> None:
+        self.size = n
+        self.coord_pool, self.sdf_label_pool, self.weight_pool = self._coord[:n], self._label[:n], self._weight[:n]
+
+    def _reserve(self, need: int) -> None:
+        if need <= self.capacity:
+            return
+        cap = max(need, int(self.capacity * self.GROWTH))
+        n = self.size
+        self.coord_pool = self.sdf_label_pool = self.weight_pool = None     # the views would keep the old buffers alive
+        for name, shape in (("_coord", (cap, 3)), ("_label", (cap,)), ("_weight", (cap,))):
+            old = getattr(self, name)
+            new = torch.empty(shape, device=self.device)
+            new[:n] = old[:n]
+            setattr(self, name, new)
+            del old                  # one array at a time: the pool is never held twice
+        self._set_size(n)
+
+    def add_frame(self, coord, label, weight, origin_scaled=None, window_radius_scaled: float | None = None):
+        """Append one frame's samples.  window_radius_scaled (`window_radius * scale`, a Python float): first drop the
+        samples whose distance to origin_scaled (the frame's sensor origin in scaled coordinates, 3 values on the host)
+        is not below it; None: keep every earlier sample (`window_replay_on: False`)."""
+        coord = coord.to(self.device, torch.float32).reshape(-1, 3).contiguous()
+        label = label.to(self.device, torch.float32).reshape(-1).contiguous()
+        weight = weight.to(self.device, torch.float32).reshape(-1).contiguous()
+        n_new = coord.shape[0]
+        if label.shape[0] != n_new or weight.shape[0] != n_new:
+            raise ValueError("coord, label and weight of a frame must have the same number of samples")
+        self._reserve(self.size + n_new)
+        self.ordered = False
+        if window_radius_scaled is None:                 # lidar_dataset.py:260-270: simply keep all previous samples
+            self._coord[self.size:self.size + n_new] = coord
+            self._label[self.size:self.size + n_new] = label
+            self._weight[self.size:self.size + n_new] = weight
+            self._set_size(self.size + n_new)
+            return self
+        from . import _abi
+        _abi.require_cuda(self._coord, "ReplayPool.add_frame")
+        o = torch.as_tensor(origin_scaled, dtype=torch.float32).reshape(3).tolist()
+        lib = _abi.lib()
+        need = int(lib.shine_pool_scratch_bytes(self.size + n_new))
+        if self._scratch is None or self._scratch.numel() < need:
+            self._scratch = torch.empty(need, dtype=torch.uint8, device=self.device)
+            self._size_out = torch.empty(1, dtype=torch.int64, device=self.device)
+        desc = _abi.ShineSamplePool(self._coord.data_ptr(), self._label.data_ptr(), self._weight.data_ptr(), self.size,
+                                    self.capacity)
+        _abi.check(lib.shine_pool_window_append(C.byref(desc), _abi.ptr(coord), _abi.ptr(label), _abi.ptr(weight), n_new,
+                                                o[0], o[1], o[2], float(window_radius_scaled), _abi.ptr(self._size_out),
+                                                _abi.ptr(self._scratch), self._scratch.numel(),
+                                                _abi.stream_ptr(self._coord.device)), "shine_pool_window_append")
+        self._set_size(int(self._size_out.item()))      # randint needs the size on the host
+        return self
+
+    def append(self, coord, label, weight):
+        return self.add_frame(coord, label, weight)
+
+    def sort_morton(self, level: int = 16, octree=None):
+        raise NotImplementedError("ReplayPool keeps the reference's sample order (the window filter preserves it)")
 
 
 def generate_scans(config: SHINEConfig, n_azimuth: int, n_frames: int = 1, frame_step_m: float = 1.0, seed: int = 42,
