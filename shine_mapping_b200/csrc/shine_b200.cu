@@ -57,7 +57,7 @@
 // The per-point training kernels with decoder gradients keep 56 accumulators per lane live through the whole tile: at 2
 // blocks/SM (128 registers) they spill ~0.5 KB per thread, at 1 block/SM (255) they do not, and on H100 the spill-free
 // build is faster (C2 batch in the order drawn, kernel: 0.460 vs 0.564 ms).  The grouped kernel timed on Morton-ordered batches
-// splits the weight-gradient contraction across the block (block-wide rounds) and fits SHINE_TRAIN_MINB without spilling.
+// splits the weight-gradient contraction across groups of 4 warps (rounds) and fits SHINE_TRAIN_MINB without spilling.
 #ifndef SHINE_TRAIN_DECGRAD_MINB
 #define SHINE_TRAIN_DECGRAD_MINB 1
 #endif
@@ -323,24 +323,58 @@ __device__ __forceinline__ void from_cfrag(const float (&c)[4], int odd, float (
     else      { v[0] = r0;   v[1] = r1;   v[2] = c[2]; v[3] = c[3]; }
 }
 
-// Sums 24 per-lane values over the 8 lanes of equal t (lane bits 2-4) and leaves lane (g, t) the sums of slots 3g .. 3g+2:
-// a butterfly that halves the values it keeps at each step (21 shuffles instead of 72 for a full all-reduce).
-__device__ __forceinline__ void reduce_scatter_g(const float (&v)[24], float (&out)[3], int lane) {
-    float a[12], b[6];
-    const bool b4 = (lane & 16) != 0, b3 = (lane & 8) != 0, b2 = (lane & 4) != 0;
-#pragma unroll
-    for (int i = 0; i < 12; ++i) a[i] = (b4 ? v[12 + i] : v[i]) + __shfl_xor_sync(kFull, b4 ? v[i] : v[12 + i], 16);
-#pragma unroll
-    for (int i = 0; i < 6; ++i) b[i] = (b3 ? a[6 + i] : a[i]) + __shfl_xor_sync(kFull, b3 ? a[i] : a[6 + i], 8);
-#pragma unroll
-    for (int i = 0; i < 3; ++i) out[i] = (b2 ? b[3 + i] : b[i]) + __shfl_xor_sync(kFull, b2 ? b[i] : b[3 + i], 4);
-}
-
 // decoder-gradient accumulators of a lane in the per-point kernels (mma.sync C fragments): dW2[2][4][4], dW1[2][4], and the
 // per-column partial sums of db2, db1, dw3 ([4][2]: columns 8j + 2t + q)
 #define SHINE_ACC_DECL float dW2[2][4][4], dW1[2][4], db2p[4][2], db1p[4][2], dw3p[4][2]
 
-__device__ __forceinline__ void round_bar(int id) { asm volatile("bar.sync %0, 256;" ::"r"(id) : "memory"); }
+// Sums 8 per-lane values over the 8 lanes of equal t and leaves lane (g, t) the sum of slot g (7 shuffles)
+__device__ __forceinline__ float reduce_scatter_g8(const float (&v)[8], int lane) {
+    float a[4], b[2];
+    const bool b4 = (lane & 16) != 0, b3 = (lane & 8) != 0, b2 = (lane & 4) != 0;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) a[i] = (b4 ? v[4 + i] : v[i]) + __shfl_xor_sync(kFull, b4 ? v[i] : v[4 + i], 16);
+#pragma unroll
+    for (int i = 0; i < 2; ++i) b[i] = (b3 ? a[2 + i] : a[i]) + __shfl_xor_sync(kFull, b3 ? a[i] : a[2 + i], 8);
+    return (b2 ? b[1] : b[0]) + __shfl_xor_sync(kFull, b2 ? b[0] : b[1], 4);
+}
+// named barrier of one round group: the 4 warps (128 threads) that share their staged tiles
+__device__ __forceinline__ void round_bar(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+
+// Decoder-weight-gradient operands are staged in mma fragment order: a consumer lane builds an A fragment with one LDS.128
+// and a B fragment with one LDS.64.  The contraction runs over a tile's 16 points in an order of our choosing (A and B
+// agree on it): points g and g + 8 are k-step g >> 2, k-slots (g & 3) and (g & 3) + 4, so that the producer lane of a
+// C-fragment row pair (rows g, g + 8) holds both k-slots of a fragment register pair.  The 32 lane chunks of a fragment
+// are stored at frag_chunk(lane), a permutation inside each group of 8 lanes: a consumer's 8 (LDS.128) or 16 (LDS.64)
+// consecutive lanes still read whole 128-byte lines, and the producers' stores, where lane (g, t) writes the chunk of
+// consumer lane 8t + 4q + (g & 3), land on distinct banks because the XOR with 2t separates the four values of t.
+// Bank conflicts stay at zero by this layout, without padding.
+__device__ __forceinline__ int frag_chunk(int lane) { return lane ^ ((lane >> 2) & 6); }
+// A fragment ([32][4] block) / B fragment ([32][2] block) of chunk c, split for 3xTF32
+template <int NTF>
+__device__ __forceinline__ void load_afrag(const float* blk, int c, AFrag<NTF>& a) {
+    const float4 v = *reinterpret_cast<const float4*>(blk + 4 * c);
+    a.set_packed(v.x, v.y, v.z, v.w);
+}
+__device__ __forceinline__ void load_bfrag(const float* blk, int c, uint2& bh, uint2& bl) {
+    const float2 v = *reinterpret_cast<const float2*>(blk + 2 * c);
+    split_fast2(v.x, v.y, bh.x, bh.y, bl.x, bl.y);
+}
+// C fragments of a [16 points][32] tile (rows g, g + 8) -> the A fragments [m-tile 2][32][4] of this lane's k-step:
+// column pairs 8j + 2t + q and 8j + 8 + 2t + q of both rows are one chunk
+__device__ __forceinline__ void stage_afrags(float* blk, const int (&sq)[2], const float (&c)[4][4]) {
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+        for (int q = 0; q < 2; ++q)
+            *reinterpret_cast<float4*>(blk + 128 * mt + 4 * sq[q]) = make_float4(c[2 * mt][q], c[2 * mt + 1][q], c[2 * mt][2 + q], c[2 * mt + 1][2 + q]);
+}
+// feat fragments [k-step 2][32][2]: each lane stores single elements, so k-step 1 also flips chunk bit 3 (16 banks) to
+// keep the two k-steps' stores apart
+__device__ __forceinline__ int xfrag_word(int ks, int c) { return 64 * ks + 2 * (c ^ (8 * ks)); }
+__device__ __forceinline__ void load_xfrag(const float* sx, int ks, int c, uint2& bh, uint2& bl) {
+    const float2 v = *reinterpret_cast<const float2*>(sx + xfrag_word(ks, c));
+    split_fast2(v.x, v.y, bh.x, bh.y, bl.x, bl.y);
+}
 
 // ------------------------------------------------------------------------------------------------------
 // the fused kernel: hash walk + gather + blend + MLP (+ BCE loss) (+ full backward with scatter-add)
@@ -359,13 +393,18 @@ struct SmemPlan {
     static constexpr int B1 = W2T + 2 * kH * kWS;      // [32]
     static constexpr int B2 = B1 + kH;
     static constexpr int W3 = B2 + kH;
-    static constexpr int B3 = W3 + kH;                 // [1] (+3 pad)
+    static constexpr int B3 = W3 + kH;                 // [1]
+    static constexpr int GSCALE = B3 + 1;              // [1] (+2 pad) dL/dpred scale: read per tile, not held in a register
     static constexpr int kDecGradFloats = kH * kF + kH + kH * kH + kH + kH + 1;   // 1377 (a warp's partial goes to its staging area)
     static constexpr int RND = B3 + 4;                 // [8] per warp: 1 if its tile of the current round is staged
     static constexpr int PRE = RND + 8;                // per-warp input prefetch: [16][3] coord | [16] label | [16] weight
     static constexpr int kPrePerWarp = 5 * kTile;
-    static constexpr int STAGE = PRE + 8 * kPrePerWarp;   // per-warp staging: 3 x [16][kWS] + [16][8]
-    static constexpr int kStagePerWarp = 3 * kTile * kWS + kTile * kF;   // dh2 | h1 | dh1 | feat tiles
+    static constexpr int STAGE = PRE + 8 * kPrePerWarp;   // per-warp staging of one tile, in mma fragment order (below)
+    static constexpr int SA2 = 0;                      // dh2: A fragments of dW2, [k-step 2][m-tile 2][32 lanes][4]
+    static constexpr int SB2 = SA2 + kTile * kH;       // h1:  B fragments of dW2, [k-step 2][n-tile 4][32 lanes][2]
+    static constexpr int SA1 = SB2 + kTile * kH;       // dh1: A fragments of dW1, [k-step 2][m-tile 2][32 lanes][4]
+    static constexpr int SX = SA1 + kTile * kH;        // feat: B fragments of dW1, [k-step 2][32 lanes][2]
+    static constexpr int kStagePerWarp = SX + kTile * kF;
     // GROUPED only, after the staging area: per warp and level [tx | ty | tz | node slot] x 16 points, and (frozen decoder:
     // no staging area to borrow from) the [16][8] dL/dfeature tile
     static constexpr int kGroupPerLevel = 4 * kTile;
@@ -522,7 +561,10 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
         smem[SmemPlan::B2 + tid] = P.dec.b2 ? P.dec.b2[tid] : 0.f;
         smem[SmemPlan::W3 + tid] = P.dec.w3[tid];
     }
-    if (tid == 0) smem[SmemPlan::B3] = P.dec.b3 ? P.dec.b3[0] : 0.f;
+    if (tid == 0) {
+        smem[SmemPlan::B3] = P.dec.b3 ? P.dec.b3[0] : 0.f;
+        smem[SmemPlan::GSCALE] = P.loss_scale * ((TRAIN && P.d_loss) ? __ldg(P.d_loss) : 1.0f);
+    }
     constexpr int kPark = LMAX <= 4 ? 16 : 32;                           // blend factors of every level, per lane
     constexpr int kIdPark = 4 * LMAX;                                    // this lane's 4 corner rows of every level
     __syncthreads();
@@ -536,15 +578,20 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
     }
 #pragma unroll
     for (int j = 0; j < 4; ++j) { db2p[j][0] = db2p[j][1] = db1p[j][0] = db1p[j][1] = dw3p[j][0] = dw3p[j][1] = 0.f; }
-    // Grouped kernel (kRounds): the block's warps advance in rounds of one tile each; a round's staged operands are
-    // contracted by the whole block, each warp owning a slice of the outputs (K = the up to 128 points of the round), so that
-    // the kernel fits 2 blocks/SM without spilling.  (At 1 block/SM, the per-point kernels lose more to the round
-    // barriers than they gain: C2 batch in the order drawn, kernel 0.56 vs 0.46 ms on H100.)
-    //   dW2 [32 x 32]: m16n8 fragment (warp >> 2, warp & 3), over every staged tile;
+    // Grouped kernel (kRounds): the block's warps advance in rounds of one tile each.  A round's staged operands are
+    // contracted by the warp's group (warps 0-3 and 4-7; each group synchronises on its own named barriers, so it waits
+    // only for its own slowest warp), each warp owning a slice of the outputs (K = the up to 64 points of the group's
+    // round), so that the kernel fits 2 blocks/SM without spilling.  (At 1 block/SM, the per-point kernels lose more to the
+    // round barriers than they gain: C2 batch in the order drawn, kernel 0.56 vs 0.46 ms on H100.)
+    //   dW2 [32 x 32]: m16n16 block (warp & 1, (warp >> 1) & 1) over the tiles of group warp >> 2, 4 (warp >> 2) ..
+    //                  4 (warp >> 2) + 3 (one A and two B fragments per k-step; the two groups' partials are summed in the
+    //                  epilogue);
     //   dW1 [32 x 8]:  m16n8 fragment warp & 1, over the tiles 2 (warp >> 1) and 2 (warp >> 1) + 1 (4 partial sums each);
-    //   db1, db2, dw3: this warp's own tiles, reduced per tile to 3 columns per lane (reduce_scatter_g); db3: lane sums.
-    float dW2acc[4] = {0.f, 0.f, 0.f, 0.f}, dW1acc[4] = {0.f, 0.f, 0.f, 0.f};
-    float vecacc[3] = {0.f, 0.f, 0.f};
+    //   db1, db2: sums of the A fragments of dW1 / dW2 (dW2: the warps with (warp >> 1) & 1 == 0), reduced over the lanes
+    //             in the epilogue; dw3: this warp's own tiles, reduced per tile to 1 column per lane (reduce_scatter_g8);
+    //   db3: lane sums.
+    float dW2acc[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}}, dW1acc[4] = {0.f, 0.f, 0.f, 0.f};
+    float dw3acc = 0.f, db2acc[2] = {0.f, 0.f}, db1acc[2] = {0.f, 0.f};
     constexpr bool kRounds = DEC_GRAD && GROUPED;
 
     constexpr bool kSectorProbe = TRAIN ? (SHINE_SECTOR_PROBE_TRAIN != 0) : (SHINE_SECTOR_PROBE_INFER != 0);
@@ -552,17 +599,16 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
     constexpr bool kZeroSkip = (SHINE_ZERO_TILE_SKIP != 0) && (SHINE_CPASYNC_PREFETCH == 0);
     const bool poly = P.oct.poly_interp != 0;
     const int L = P.oct.num_levels;
-    const float up = (TRAIN && P.d_loss) ? __ldg(P.d_loss) : 1.0f;
-    const float gscale = P.loss_scale * up;
 
     float db3p = 0.f;
     float loss_acc = 0.f;
 
     float* stage = smem + SmemPlan::STAGE + warp * SmemPlan::kStagePerWarp;   // only touched when DEC_GRAD
-    float* stA = stage;                       // [16][kWS]
-    float* stB = stage + kTile * kWS;         // [16][kWS]
-    float* stC = stage + 2 * kTile * kWS;     // [16][kWS]
-    float* stX = stage + 3 * kTile * kWS;     // [16][8]
+    float* stX = stage + SmemPlan::SX;
+    // fragment-order staging (frag_chunk): this lane's points g, g + 8 are k-step kp, and its C-fragment columns 2t + q
+    // are the chunks sq[q] of that k-step's fragments; the consumer side reads chunk fc
+    const int kp = g >> 2, fc = frag_chunk(lane);
+    const int sq[2] = {frag_chunk(8 * t + (g & 3)), frag_chunk(8 * t + 4 + (g & 3))};
     // GROUPED: per-warp level tables behind the staging area; the dL/dfeature tile borrows stX (dead after the wgrad section)
     float* gpt = smem + SmemPlan::STAGE + (DEC_GRAD ? 8 * SmemPlan::kStagePerWarp : 0) +
                  warp * (LMAX * SmemPlan::kGroupPerLevel + (DEC_GRAD ? 0 : kTile * kF));
@@ -570,49 +616,51 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
 
     // End of a round (kRounds): every warp of the block arrives here once per round, `staged` telling whether its staging
     // area holds a tile (zero tiles, tiles past the end and the idle warps of the virtual backward round do not).  The
-    // second barrier releases the staging areas (the grouped scatter reuses stX right after).
+    // group's first barrier publishes its staging areas, the second releases them (the grouped scatter reuses stX right
+    // after).  Only the flags of the warp's own group are used.
     auto wgrad_round = [&](bool staged) {
         if (lane == 0) smu[SmemPlan::RND + warp] = staged ? 1u : 0u;
-        round_bar(1);
+        round_bar(1 + 2 * (threadIdx.x >> 7));
         uint32_t present = 0;
 #pragma unroll
         for (int v = 0; v < kWarps; ++v) present |= (smu[SmemPlan::RND + v] != 0u ? 1u : 0u) << v;
-        const int mt = warp >> 2, nt = warp & 3;
+        const int mt = warp & 1, np = (warp >> 1) & 1, kh = warp >> 2;
 #pragma unroll
-        for (int v = 0; v < kWarps; ++v) {
+        for (int i = 0; i < kWarps / 2; ++i) {
+            const int v = 4 * kh + i;
             if (!((present >> v) & 1u)) continue;
-            const float* sA = smem + SmemPlan::STAGE + v * SmemPlan::kStagePerWarp;   // dh2
-            const float* sB = sA + kTile * kWS;                                       // h1
+            const float* s = smem + SmemPlan::STAGE + v * SmemPlan::kStagePerWarp;
             // dW2[n2][k1] += sum_rows dh2[row][n2] * h1[row][k1]
 #pragma unroll
             for (int ks = 0; ks < 2; ++ks) {
-                uint2 bh, bl;
-                split_fast2(sB[(8 * ks + t) * kWS + 8 * nt + g], sB[(8 * ks + t + 4) * kWS + 8 * nt + g], bh.x, bh.y, bl.x, bl.y);
+                uint2 bh[2], bl[2];
+#pragma unroll
+                for (int n = 0; n < 2; ++n) load_bfrag(s + SmemPlan::SB2 + (4 * ks + 2 * np + n) * 64, fc, bh[n], bl[n]);
                 AFrag<NTF> a;
-                a.set_packed(sA[(8 * ks + t) * kWS + 16 * mt + g], sA[(8 * ks + t) * kWS + 16 * mt + g + 8],
-                             sA[(8 * ks + t + 4) * kWS + 16 * mt + g], sA[(8 * ks + t + 4) * kWS + 16 * mt + g + 8]);
-                mma3<NTF>(dW2acc, a, bh, bl);
+                const float4 av = *reinterpret_cast<const float4*>(s + SmemPlan::SA2 + (2 * ks + mt) * 128 + 4 * fc);
+                a.set_packed(av.x, av.y, av.z, av.w);
+                if (np == 0) { db2acc[0] += av.x + av.z; db2acc[1] += av.y + av.w; }   // db2 rows 16 mt + g, + 8
+                mma3x2<NTF>(dW2acc[0], dW2acc[1], a, a, bh[0], bl[0], bh[1], bl[1]);
             }
         }
-        const int m1 = warp & 1;
 #pragma unroll
         for (int vv = 0; vv < 2; ++vv) {
             const int v = 2 * (warp >> 1) + vv;
             if (!((present >> v) & 1u)) continue;
-            const float* sC = smem + SmemPlan::STAGE + v * SmemPlan::kStagePerWarp + 2 * kTile * kWS;   // dh1
-            const float* sX = sC + kTile * kWS;                                                       // feat
+            const float* s = smem + SmemPlan::STAGE + v * SmemPlan::kStagePerWarp;
             // dW1[n1][ch] += sum_rows dh1[row][n1] * feat[row][ch]
 #pragma unroll
             for (int ks = 0; ks < 2; ++ks) {
                 uint2 bh, bl;
-                split_fast2(sX[(8 * ks + t) * kF + g], sX[(8 * ks + t + 4) * kF + g], bh.x, bh.y, bl.x, bl.y);
+                load_xfrag(s + SmemPlan::SX, ks, fc, bh, bl);
                 AFrag<NTF> a;
-                a.set_packed(sC[(8 * ks + t) * kWS + 16 * m1 + g], sC[(8 * ks + t) * kWS + 16 * m1 + g + 8],
-                             sC[(8 * ks + t + 4) * kWS + 16 * m1 + g], sC[(8 * ks + t + 4) * kWS + 16 * m1 + g + 8]);
+                const float4 av = *reinterpret_cast<const float4*>(s + SmemPlan::SA1 + (2 * ks + mt) * 128 + 4 * fc);
+                a.set_packed(av.x, av.y, av.z, av.w);
+                db1acc[0] += av.x + av.z; db1acc[1] += av.y + av.w;                  // db1 rows 16 mt + g, + 8
                 mma3<NTF>(dW1acc, a, bh, bl);
             }
         }
-        round_bar(2);
+        round_bar(2 + 2 * (threadIdx.x >> 7));
     };
 
     const int warp_global = blockIdx.x * kWarps + warp;
@@ -739,7 +787,7 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
         if (TRAIN) {
             const float rs = __fdividef(1.0f, 1.0f + e);
             const float sg = pv >= 0.f ? rs : e * rs;                                   // sigmoid(pred)
-            dp = (sg - zt) * wg * gscale;
+            dp = (sg - zt) * wg * smem[SmemPlan::GSCALE];
         }
     };
     // tile schedule: the first tile of a warp is its global index; every further one is drawn from P.tile_counter (counter
@@ -976,10 +1024,13 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
             float a[4]; to_afrag(feat, odd, a);
             ax.set(a[0], a[1], a[2], a[3]);
         }
-        // operands of the weight-gradient contraction go to this warp's shared-memory staging the moment they are
-        // produced (feat -> stX, h1 -> stB, dh2 -> stA, dh1 -> stC) so that they do not pin registers
-        if (DEC_GRAD)
-            *reinterpret_cast<float4*>(stX + (g + 8 * odd) * kF + 4 * half) = make_float4(feat[0], feat[1], feat[2], feat[3]);
+        // operands of the weight-gradient contraction go to this warp's shared-memory staging (fragment order) the moment
+        // they are produced (feat -> SX, h1 -> SB2, dh2 -> SA2, dh1 -> SA1) so that they do not pin registers.
+        // feat (row-half layout): point g + 8 odd is k-slot odd of chunk (4 half + q) * 4 + (g & 3) of k-step kp.
+        if (DEC_GRAD) {
+#pragma unroll
+            for (int q = 0; q < 4; ++q) stX[xfrag_word(kp, frag_chunk(16 * half + 4 * q + (g & 3))) + odd] = feat[q];
+        }
         float h1[4][4];
         uint32_t m1 = 0;   // ReLU mask of h1: bit 4j+r
         {
@@ -1001,8 +1052,9 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
                     h1[j][r] = fmaxf(h1[j][r], 0.f);
                 }
                 if (DEC_GRAD) {
-                    *reinterpret_cast<float2*>(stB + g * kWS + 8 * j + 2 * t) = make_float2(h1[j][0], h1[j][1]);
-                    *reinterpret_cast<float2*>(stB + (g + 8) * kWS + 8 * j + 2 * t) = make_float2(h1[j][2], h1[j][3]);
+#pragma unroll
+                    for (int q = 0; q < 2; ++q)
+                        *reinterpret_cast<float2*>(stage + SmemPlan::SB2 + (4 * kp + j) * 64 + 2 * sq[q]) = make_float2(h1[j][q], h1[j][2 + q]);
                 }
             }
         }
@@ -1070,7 +1122,7 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
             if (TRAIN) {
                 const float rs = __fdividef(1.0f, 1.0f + e);
                 const float sg = pown >= 0.f ? rs : e * rs;                               // sigmoid(pred)
-                dpo = (sg - zt) * wgt * gscale;
+                dpo = (sg - zt) * wgt * smem[SmemPlan::GSCALE];
             }
 #endif
         }
@@ -1083,7 +1135,7 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
         const float dpx = __shfl_xor_sync(kFull, dpo, 1);
         const float dp0 = odd ? dpx : dpo, dp8 = odd ? dpo : dpx;
         float dh2[4][4];
-        float db2t[4][2], db1t[4][2], dw3t[4][2];   // this tile's partials (rows g, g+8), folded into vecacc before the round
+        float db2t[4][2], db1t[4][2], dw3t[4][2];   // this tile's partials (rows g, g+8)
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             dh2[j][0] = h2[j][0] > 0.f ? dp0 * w3a[j] : 0.f; dh2[j][1] = h2[j][1] > 0.f ? dp0 * w3b[j] : 0.f;
@@ -1091,10 +1143,9 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
             if (DEC_GRAD) {
                 dw3t[j][0] = dp0 * h2[j][0] + dp8 * h2[j][2];  dw3t[j][1] = dp0 * h2[j][1] + dp8 * h2[j][3];
                 db2t[j][0] = dh2[j][0] + dh2[j][2];            db2t[j][1] = dh2[j][1] + dh2[j][3];
-                *reinterpret_cast<float2*>(stA + g * kWS + 8 * j + 2 * t) = make_float2(dh2[j][0], dh2[j][1]);
-                *reinterpret_cast<float2*>(stA + (g + 8) * kWS + 8 * j + 2 * t) = make_float2(dh2[j][2], dh2[j][3]);
             }
         }
+        if (DEC_GRAD) stage_afrags(stage + SmemPlan::SA2 + 256 * kp, sq, dh2);
         if (DEC_GRAD && t == 0) db3p += dp0 + dp8;
 
         float dh1[4][4];
@@ -1117,12 +1168,9 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
             for (int j = 0; j < 4; ++j) {
 #pragma unroll
                 for (int r = 0; r < 4; ++r) dh1[j][r] = ((m1 >> (4 * j + r)) & 1u) ? dh1[j][r] : 0.f;
-                if (DEC_GRAD) {
-                    db1t[j][0] = dh1[j][0] + dh1[j][2]; db1t[j][1] = dh1[j][1] + dh1[j][3];
-                    *reinterpret_cast<float2*>(stC + g * kWS + 8 * j + 2 * t) = make_float2(dh1[j][0], dh1[j][1]);
-                    *reinterpret_cast<float2*>(stC + (g + 8) * kWS + 8 * j + 2 * t) = make_float2(dh1[j][2], dh1[j][3]);
-                }
+                if (DEC_GRAD) { db1t[j][0] = dh1[j][0] + dh1[j][2]; db1t[j][1] = dh1[j][1] + dh1[j][3]; }
             }
+            if (DEC_GRAD) stage_afrags(stage + SmemPlan::SA1 + 256 * kp, sq, dh1);
         }
         float dxc[4] = {0.f, 0.f, 0.f, 0.f};
         {
@@ -1157,15 +1205,11 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
             for (int ks = 0; ks < 2; ++ks) {
                 uint2 bh[4], bl[4];
 #pragma unroll
-                for (int nt = 0; nt < 4; ++nt) {
-                    const float b0 = stB[(8 * ks + t) * kWS + 8 * nt + g], b1 = stB[(8 * ks + t + 4) * kWS + 8 * nt + g];
-                    split_fast2(b0, b1, bh[nt].x, bh[nt].y, bl[nt].x, bl[nt].y);
-                }
+                for (int nt = 0; nt < 4; ++nt) load_bfrag(stage + SmemPlan::SB2 + (4 * ks + nt) * 64, fc, bh[nt], bl[nt]);
 #pragma unroll
                 for (int mt = 0; mt < 2; ++mt) {
                     AFrag<NTF> a;
-                    a.set_packed(stA[(8 * ks + t) * kWS + 16 * mt + g], stA[(8 * ks + t) * kWS + 16 * mt + g + 8],
-                          stA[(8 * ks + t + 4) * kWS + 16 * mt + g], stA[(8 * ks + t + 4) * kWS + 16 * mt + g + 8]);
+                    load_afrag(stage + SmemPlan::SA2 + (2 * ks + mt) * 128, fc, a);
                     mma3x4<NTF>(dW2[mt], a, bh, bl);
                 }
             }
@@ -1173,27 +1217,19 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
 #pragma unroll
             for (int ks = 0; ks < 2; ++ks) {
                 uint2 bh, bl;
-                split_fast2(stX[(8 * ks + t) * kF + g], stX[(8 * ks + t + 4) * kF + g], bh.x, bh.y, bl.x, bl.y);
+                load_xfrag(stX, ks, fc, bh, bl);
                 AFrag<NTF> a0, a1;
-                a0.set_packed(stC[(8 * ks + t) * kWS + g], stC[(8 * ks + t) * kWS + g + 8],
-                              stC[(8 * ks + t + 4) * kWS + g], stC[(8 * ks + t + 4) * kWS + g + 8]);
-                a1.set_packed(stC[(8 * ks + t) * kWS + 16 + g], stC[(8 * ks + t) * kWS + 16 + g + 8],
-                              stC[(8 * ks + t + 4) * kWS + 16 + g], stC[(8 * ks + t + 4) * kWS + 16 + g + 8]);
+                load_afrag(stage + SmemPlan::SA1 + (2 * ks) * 128, fc, a0);
+                load_afrag(stage + SmemPlan::SA1 + (2 * ks + 1) * 128, fc, a1);
                 mma3x2<NTF>(dW1[0], dW1[1], a0, a1, bh, bl, bh, bl);
             }
             __syncwarp();
-                }
+        }
         if (kRounds) {                    // bias / output-layer columns here, the weight matrices by the round
-            float cols[24];   // slot 8k + 2j + q: column 8j + 2t + q of db1 (k = 0), db2 (k = 1), dw3 (k = 2)
+            float cols[8];   // slot 2j + q: column 8j + 2t + q of dw3 (db1, db2: sums of the round's A fragments)
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {
-#pragma unroll
-                for (int q = 0; q < 2; ++q) { cols[2 * j + q] = db1t[j][q]; cols[8 + 2 * j + q] = db2t[j][q]; cols[16 + 2 * j + q] = dw3t[j][q]; }
-            }
-            float sums[3];
-            reduce_scatter_g(cols, sums, lane);
-#pragma unroll
-            for (int i = 0; i < 3; ++i) vecacc[i] += sums[i];
+            for (int j = 0; j < 4; ++j) { cols[2 * j] = dw3t[j][0]; cols[2 * j + 1] = dw3t[j][1]; }
+            dw3acc += reduce_scatter_g8(cols, lane);    // column 8 (g >> 1) + 2t + (g & 1)
             wgrad_round(true);
         }
 
@@ -1256,29 +1292,38 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
         if (lane == 0 && loss_acc != 0.f) atomicAdd(P.loss, loss_acc * P.loss_scale);
     }
     if (kRounds) {
-        // dW2: this warp is the only owner of its fragment, one global atomic per non-zero element
-        {
-            const int mt = warp >> 2, nt = warp & 3;
-#pragma unroll
-            for (int r = 0; r < 4; ++r)
-                if (dW2acc[r] != 0.f) atomicAdd(P.dec.gw2 + (16 * mt + g + 8 * (r >> 1)) * kH + 8 * nt + 2 * t + (r & 1), dW2acc[r]);
-        }
-        // the rest: per-warp partials [dW1 fragment warp & 1: 128 | gb1 32 | gb2 32 | gw3 32 | gb3 1] in the staging area
-        // (free after the last round), summed by the block, one global atomic per non-zero element
+        // per-warp partials [dW1 fragment warp & 1: 128 | gb1 32 | gb2 32 | gw3 32 | gb3 1 | pad | dW2 block (warp & 1,
+        // (warp >> 1) & 1) over half the tiles: [16][16]] in the staging area (free after the last round), summed by the
+        // block, one global atomic per non-zero element
         float* part = stage;
-        constexpr int oB1 = 128, oB3 = 224, kParts = 225;
+        constexpr int oB1 = 128, oB3 = 224, kParts = 225, oW2 = 256, kW2Block = 16 * 16;
+#pragma unroll
+        for (int n = 0; n < 2; ++n) {
+            *reinterpret_cast<float2*>(part + oW2 + g * 16 + 8 * n + 2 * t) = make_float2(dW2acc[n][0], dW2acc[n][1]);
+            *reinterpret_cast<float2*>(part + oW2 + (g + 8) * 16 + 8 * n + 2 * t) = make_float2(dW2acc[n][2], dW2acc[n][3]);
+        }
         *reinterpret_cast<float2*>(part + g * kF + 2 * t) = make_float2(dW1acc[0], dW1acc[1]);
         *reinterpret_cast<float2*>(part + (g + 8) * kF + 2 * t) = make_float2(dW1acc[2], dW1acc[3]);
+        part[oB1 + 2 * kH + 8 * (g >> 1) + 2 * t + (g & 1)] = dw3acc;
+        {   // db1 / db2 rows 16 mt + g (+ 8): sums over this warp's k-slots, then over the 4 lanes of equal g
+            const int mt = warp & 1, np = (warp >> 1) & 1;
 #pragma unroll
-        for (int i = 0; i < 3; ++i) {
-            const int s = 3 * g + i, k = s >> 3, j = (s & 7) >> 1, q = s & 1;
-            part[oB1 + 32 * k + 8 * j + 2 * t + q] = vecacc[i];
+            for (int r = 0; r < 2; ++r) {
+                float d1 = db1acc[r], d2 = db2acc[r];
+#pragma unroll
+                for (int o = 1; o < 4; o <<= 1) { d1 += __shfl_xor_sync(kFull, d1, o); d2 += __shfl_xor_sync(kFull, d2, o); }
+                if (t == 0) {
+                    part[oB1 + 16 * mt + g + 8 * r] = d1;           part[oB1 + 16 * (1 - mt) + g + 8 * r] = 0.f;
+                    part[oB1 + kH + 16 * mt + g + 8 * r] = np == 0 ? d2 : 0.f;   part[oB1 + kH + 16 * (1 - mt) + g + 8 * r] = 0.f;
+                }
+            }
         }
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) db3p += __shfl_xor_sync(kFull, db3p, o);
         if (lane == 0) part[oB3] = db3p;
         __syncthreads();
-        for (int i = tid; i < 2 * oB1 + (kParts - oB1); i += blockDim.x) {
+        constexpr int kVecEnd = 2 * oB1 + (kParts - oB1);
+        for (int i = tid; i < kVecEnd + 4 * kW2Block; i += blockDim.x) {
             float v = 0.f;
             float* dst;
             if (i < 2 * oB1) {      // dW1 row 16 m + r: the partials of warps m, m + 2, m + 4, m + 6
@@ -1286,6 +1331,11 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
 #pragma unroll
                 for (int c = 0; c < kWarps / 2; ++c) v += smem[SmemPlan::STAGE + (2 * c + m) * SmemPlan::kStagePerWarp + e];
                 dst = P.dec.gw1 + 16 * m * kF + e;
+            } else if (i >= kVecEnd) {      // dW2 block b = (row block b & 1, column block b >> 1): warps b and b + 4
+                const int b = (i - kVecEnd) / kW2Block, e = (i - kVecEnd) % kW2Block;
+                const float* p0 = smem + SmemPlan::STAGE + b * SmemPlan::kStagePerWarp + oW2 + e;
+                v = p0[0] + p0[4 * SmemPlan::kStagePerWarp];
+                dst = P.dec.gw2 + (16 * (b & 1) + e / 16) * kH + 16 * (b >> 1) + e % 16;
             } else {
                 const int e = i - oB1;
 #pragma unroll
