@@ -57,7 +57,7 @@
 // The per-point training kernels with decoder gradients keep 56 accumulators per lane live through the whole tile: at 2
 // blocks/SM (128 registers) they spill ~0.5 KB per thread, at 1 block/SM (255) they do not, and on H100 the spill-free
 // build is faster (C2 batch in the order drawn, kernel: 0.460 vs 0.564 ms).  The grouped kernel timed on Morton-ordered batches
-// splits the weight-gradient contraction across groups of 4 warps (rounds) and fits SHINE_TRAIN_MINB without spilling.
+// keeps its dW2 partial in shared memory and fits SHINE_TRAIN_MINB without spilling.
 #ifndef SHINE_TRAIN_DECGRAD_MINB
 #define SHINE_TRAIN_DECGRAD_MINB 1
 #endif
@@ -337,8 +337,6 @@ __device__ __forceinline__ float reduce_scatter_g8(const float (&v)[8], int lane
     for (int i = 0; i < 2; ++i) b[i] = (b3 ? a[2 + i] : a[i]) + __shfl_xor_sync(kFull, b3 ? a[i] : a[2 + i], 8);
     return (b2 ? b[1] : b[0]) + __shfl_xor_sync(kFull, b2 ? b[0] : b[1], 4);
 }
-// named barrier of one round group: the 4 warps (128 threads) that share their staged tiles
-__device__ __forceinline__ void round_bar(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
 
 // Decoder-weight-gradient operands are staged in mma fragment order: a consumer lane builds an A fragment with one LDS.128
 // and a B fragment with one LDS.64.  The contraction runs over a tile's 16 points in an order of our choosing (A and B
@@ -396,18 +394,24 @@ struct SmemPlan {
     static constexpr int B3 = W3 + kH;                 // [1]
     static constexpr int GSCALE = B3 + 1;              // [1] (+2 pad) dL/dpred scale: read per tile, not held in a register
     static constexpr int kDecGradFloats = kH * kF + kH + kH * kH + kH + kH + 1;   // 1377 (a warp's partial goes to its staging area)
-    static constexpr int RND = B3 + 4;                 // [8] per warp: 1 if its tile of the current round is staged
-    static constexpr int PRE = RND + 8;                // per-warp input prefetch: [16][3] coord | [16] label | [16] weight
+    static constexpr int PRE = B3 + 4;                 // per-warp input prefetch: [16][3] coord | [16] label | [16] weight
     static constexpr int kPrePerWarp = 5 * kTile;
     static constexpr int STAGE = PRE + 8 * kPrePerWarp;   // per-warp staging of one tile, in mma fragment order (below)
-    static constexpr int SA2 = 0;                      // dh2: A fragments of dW2, [k-step 2][m-tile 2][32 lanes][4]
-    static constexpr int SB2 = SA2 + kTile * kH;       // h1:  B fragments of dW2, [k-step 2][n-tile 4][32 lanes][2]
+    static constexpr int SB2 = 0;                      // h1:  B fragments of dW2, [k-step 2][n-tile 4][32 lanes][2]
     static constexpr int SA1 = SB2 + kTile * kH;       // dh1: A fragments of dW1, [k-step 2][m-tile 2][32 lanes][4]
     static constexpr int SX = SA1 + kTile * kH;        // feat: B fragments of dW1, [k-step 2][32 lanes][2]
-    static constexpr int kStagePerWarp = SX + kTile * kF;
+    static constexpr int SA2 = SX + kTile * kF;        // per-point kernels: dh2, A fragments of dW2, [k-step 2][m-tile 2][32 lanes][4]
+    static constexpr int SDP = SA2;                    // GROUPED: [16 points] {dL/dpred, ReLU mask of h2 (bit n)}, from
+                                                       // which the contraction rebuilds dh2
+    static constexpr int kStagePerWarp = SA2 + kTile * kH;
+    static constexpr int kStageGrouped = SDP + 2 * kTile;
+    __host__ __device__ static constexpr int stage_per_warp(bool grouped) { return grouped ? kStageGrouped : kStagePerWarp; }
     // GROUPED only, after the staging area: per warp and level [tx | ty | tz | node slot] x 16 points, and (frozen decoder:
     // no staging area to borrow from) the [16][8] dL/dfeature tile
     static constexpr int kGroupPerLevel = 4 * kTile;
+    // GROUPED with decoder gradients, after the level tables: per warp its dW2 partial as the image of the C fragments
+    // [m-tile 2][n-tile 4][32 lanes][4]
+    static constexpr int kW2Part = kH * kH;
 };
 
 // ---- voxel-grouped scatter (GROUPED kernels: batches in Morton order) ---------------------------------------------
@@ -537,6 +541,11 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
     static_assert(!GROUPED || TRAIN, "the grouped scatter belongs to the training kernels");
     static_assert(!DEC_GRAD || TRAIN, "decoder gradients belong to the training kernels");
     static_assert(SmemPlan::kStagePerWarp >= SmemPlan::kDecGradFloats, "a warp's staging area holds its partial decoder gradient");
+    static_assert(SmemPlan::kStageGrouped >= kH * kF + 3 * kH + 1, "a grouped warp's staging area holds its partial bias / dW1 gradients");
+    static_assert(!(GROUPED && DEC_GRAD) ||
+                      (SmemPlan::STAGE + 8 * (SmemPlan::kStageGrouped + LMAX * SmemPlan::kGroupPerLevel + SmemPlan::kW2Part)) * 4 + 1024 <=
+                          227 * 1024 / SHINE_TRAIN_MINB,
+                  "the grouped kernel's shared memory fits SHINE_TRAIN_MINB blocks/SM");
     extern __shared__ __align__(16) float smem[];
     uint32_t* smu = reinterpret_cast<uint32_t*>(smem);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -578,21 +587,12 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
     }
 #pragma unroll
     for (int j = 0; j < 4; ++j) { db2p[j][0] = db2p[j][1] = db1p[j][0] = db1p[j][1] = dw3p[j][0] = dw3p[j][1] = 0.f; }
-    // Grouped kernel (kRounds): the block's warps advance in rounds of one tile each.  A round's staged operands are
-    // contracted by the warp's group (warps 0-3 and 4-7; each group synchronises on its own named barriers, so it waits
-    // only for its own slowest warp), each warp owning a slice of the outputs (K = the up to 64 points of the group's
-    // round), so that the kernel fits 2 blocks/SM without spilling.  (At 1 block/SM, the per-point kernels lose more to the
-    // round barriers than they gain: C2 batch in the order drawn, kernel 0.56 vs 0.46 ms on H100.)
-    //   dW2 [32 x 32]: m16n16 block (warp & 1, (warp >> 1) & 1) over the tiles of group warp >> 2, 4 (warp >> 2) ..
-    //                  4 (warp >> 2) + 3 (one A and two B fragments per k-step; the two groups' partials are summed in the
-    //                  epilogue);
-    //   dW1 [32 x 8]:  m16n8 fragment warp & 1, over the tiles 2 (warp >> 1) and 2 (warp >> 1) + 1 (4 partial sums each);
-    //   db1, db2: sums of the A fragments of dW1 / dW2 (dW2: the warps with (warp >> 1) & 1 == 0), reduced over the lanes
-    //             in the epilogue; dw3: this warp's own tiles, reduced per tile to 1 column per lane (reduce_scatter_g8);
-    //   db3: lane sums.
-    float dW2acc[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}}, dW1acc[4] = {0.f, 0.f, 0.f, 0.f};
-    float dw3acc = 0.f, db2acc[2] = {0.f, 0.f}, db1acc[2] = {0.f, 0.f};
-    constexpr bool kRounds = DEC_GRAD && GROUPED;
+    // Grouped kernel: every warp contracts the tile it has just staged.  Only dW2 does not fit the registers at 2 blocks/SM:
+    // it is a per-warp partial in shared memory (SmemPlan::kW2Part), read, updated and written back once per tile.
+    //   dW1: dW1[2][4] as in the per-point kernels;
+    //   db1, db2: sums of the A fragments of dW1 / dW2 (rows 16 mt + g, + 8), reduced over the lanes in the epilogue;
+    //   dw3: reduced per tile to 1 column per lane (reduce_scatter_g8);  db3: lane sums.
+    float dw3acc = 0.f, db2acc[2][2] = {{0.f, 0.f}, {0.f, 0.f}}, db1acc[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
 
     constexpr bool kSectorProbe = TRAIN ? (SHINE_SECTOR_PROBE_TRAIN != 0) : (SHINE_SECTOR_PROBE_INFER != 0);
     constexpr bool kSlotPrefetch = TRAIN && !kSectorProbe && (SHINE_SLOT_PREFETCH != 0) && (SHINE_CPASYNC_PREFETCH == 0);
@@ -603,65 +603,24 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
     float db3p = 0.f;
     float loss_acc = 0.f;
 
-    float* stage = smem + SmemPlan::STAGE + warp * SmemPlan::kStagePerWarp;   // only touched when DEC_GRAD
+    constexpr int kStage = SmemPlan::stage_per_warp(GROUPED);
+    float* stage = smem + SmemPlan::STAGE + warp * kStage;   // only touched when DEC_GRAD
     float* stX = stage + SmemPlan::SX;
     // fragment-order staging (frag_chunk): this lane's points g, g + 8 are k-step kp, and its C-fragment columns 2t + q
     // are the chunks sq[q] of that k-step's fragments; the consumer side reads chunk fc
     const int kp = g >> 2, fc = frag_chunk(lane);
     const int sq[2] = {frag_chunk(8 * t + (g & 3)), frag_chunk(8 * t + 4 + (g & 3))};
     // GROUPED: per-warp level tables behind the staging area; the dL/dfeature tile borrows stX (dead after the wgrad section)
-    float* gpt = smem + SmemPlan::STAGE + (DEC_GRAD ? 8 * SmemPlan::kStagePerWarp : 0) +
+    float* gpt = smem + SmemPlan::STAGE + (DEC_GRAD ? 8 * kStage : 0) +
                  warp * (LMAX * SmemPlan::kGroupPerLevel + (DEC_GRAD ? 0 : kTile * kF));
     float* gdx = DEC_GRAD ? stX : gpt + LMAX * SmemPlan::kGroupPerLevel;
-
-    // End of a round (kRounds): every warp of the block arrives here once per round, `staged` telling whether its staging
-    // area holds a tile (zero tiles, tiles past the end and the idle warps of the virtual backward round do not).  The
-    // group's first barrier publishes its staging areas, the second releases them (the grouped scatter reuses stX right
-    // after).  Only the flags of the warp's own group are used.
-    auto wgrad_round = [&](bool staged) {
-        if (lane == 0) smu[SmemPlan::RND + warp] = staged ? 1u : 0u;
-        round_bar(1 + 2 * (threadIdx.x >> 7));
-        uint32_t present = 0;
+    // GROUPED with decoder gradients: this warp's dW2 partial behind the level tables; a lane only ever touches its own
+    // float4 of each fragment, so no synchronisation guards it until the epilogue
+    float* w2p = smem + SmemPlan::STAGE + 8 * kStage + 8 * LMAX * SmemPlan::kGroupPerLevel + warp * SmemPlan::kW2Part;
+    if (DEC_GRAD && GROUPED) {
 #pragma unroll
-        for (int v = 0; v < kWarps; ++v) present |= (smu[SmemPlan::RND + v] != 0u ? 1u : 0u) << v;
-        const int mt = warp & 1, np = (warp >> 1) & 1, kh = warp >> 2;
-#pragma unroll
-        for (int i = 0; i < kWarps / 2; ++i) {
-            const int v = 4 * kh + i;
-            if (!((present >> v) & 1u)) continue;
-            const float* s = smem + SmemPlan::STAGE + v * SmemPlan::kStagePerWarp;
-            // dW2[n2][k1] += sum_rows dh2[row][n2] * h1[row][k1]
-#pragma unroll
-            for (int ks = 0; ks < 2; ++ks) {
-                uint2 bh[2], bl[2];
-#pragma unroll
-                for (int n = 0; n < 2; ++n) load_bfrag(s + SmemPlan::SB2 + (4 * ks + 2 * np + n) * 64, fc, bh[n], bl[n]);
-                AFrag<NTF> a;
-                const float4 av = *reinterpret_cast<const float4*>(s + SmemPlan::SA2 + (2 * ks + mt) * 128 + 4 * fc);
-                a.set_packed(av.x, av.y, av.z, av.w);
-                if (np == 0) { db2acc[0] += av.x + av.z; db2acc[1] += av.y + av.w; }   // db2 rows 16 mt + g, + 8
-                mma3x2<NTF>(dW2acc[0], dW2acc[1], a, a, bh[0], bl[0], bh[1], bl[1]);
-            }
-        }
-#pragma unroll
-        for (int vv = 0; vv < 2; ++vv) {
-            const int v = 2 * (warp >> 1) + vv;
-            if (!((present >> v) & 1u)) continue;
-            const float* s = smem + SmemPlan::STAGE + v * SmemPlan::kStagePerWarp;
-            // dW1[n1][ch] += sum_rows dh1[row][n1] * feat[row][ch]
-#pragma unroll
-            for (int ks = 0; ks < 2; ++ks) {
-                uint2 bh, bl;
-                load_xfrag(s + SmemPlan::SX, ks, fc, bh, bl);
-                AFrag<NTF> a;
-                const float4 av = *reinterpret_cast<const float4*>(s + SmemPlan::SA1 + (2 * ks + mt) * 128 + 4 * fc);
-                a.set_packed(av.x, av.y, av.z, av.w);
-                db1acc[0] += av.x + av.z; db1acc[1] += av.y + av.w;                  // db1 rows 16 mt + g, + 8
-                mma3<NTF>(dW1acc, a, bh, bl);
-            }
-        }
-        round_bar(2 + 2 * (threadIdx.x >> 7));
-    };
+        for (int f = 0; f < 8; ++f) *reinterpret_cast<float4*>(w2p + 128 * f + 4 * lane) = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
 
     const int warp_global = blockIdx.x * kWarps + warp;
     const int warp_stride = gridDim.x * kWarps;
@@ -735,8 +694,7 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
     };
     prefetch_inputs(warp_global);
 
-    // kRounds: the block's warps run the same rounds; a tile past the end has no valid point and contributes zeros
-    for (int tile = warp_global; tile - (kRounds ? warp : 0) < P.num_tiles; tile += warp_stride) {
+    for (int tile = warp_global; tile < P.num_tiles; tile += warp_stride) {
         const int64_t base = (int64_t)tile * kTile;
         const int64_t myp = base + g + 8 * odd;
         asm volatile("cp.async.wait_group 0;" ::: "memory");
@@ -773,8 +731,7 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
     // linear in dL/dpred.  In a Morton-ordered batch free-space samples fill whole tiles (35 % of the C2 tiles): such a tile
     // only walks the hash, evaluates its loss terms against pred0 and adds its dL/dpred to a sum.  Pass 0 of the loop below
     // is one virtual tile (no points: features 0) run through the forward to get pred0; after the block's real tiles, warp 0
-    // runs one more virtual tile whose first point carries the block's dL/dpred sum through the ordinary backward (with
-    // DEC_GRAD: one more round, in which the other warps stage nothing).
+    // runs one more virtual tile whose first point carries the block's dL/dpred sum through the ordinary backward.
     int phase = kZeroSkip ? 0 : 1;          // 0: virtual forward, 1: this warp's tiles, 2: virtual backward (warp 0)
     bool advance = false, last_pass = false;
     float pred0 = 0.f, zsum = 0.f;
@@ -792,22 +749,20 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
     };
     // tile schedule: the first tile of a warp is its global index; every further one is drawn from P.tile_counter (counter
     // value k <-> tile warp_stride + k), requested a whole tile ahead so that the atomic's latency is never waited for
-    // (kRounds keeps the static schedule: its warps run in block-wide rounds)
-    const bool dynamic = (SHINE_DYNAMIC_TILES != 0) && !kRounds && P.tile_counter != nullptr;
+    const bool dynamic = (SHINE_DYNAMIC_TILES != 0) && P.tile_counter != nullptr;
     int next_tile = 0, pending = 0;
     if (dynamic && lane == 0) pending = atomicAdd(P.tile_counter, 1);
     for (int seq = warp_global;; seq = !advance ? seq : (dynamic ? next_tile : seq + warp_stride)) {
         if (last_pass) break;
         const int tile = tile_of(seq);
-        // kRounds: the rounds go on while warp 0 of the block has a tile; a later warp's tile past the end is a zero tile
-        if (phase == 1 && seq - (kRounds ? warp : 0) >= P.num_tiles) {
+        if (phase == 1 && seq >= P.num_tiles) {
             if constexpr (kZeroSkip && DEC_GRAD) {
                 // hand the all-miss dL/dpred sums of the block's warps to warp 0 (every warp passes here exactly once)
 #pragma unroll
                 for (int o = 16; o > 0; o >>= 1) zsum += __shfl_xor_sync(kFull, zsum, o);
                 if (lane == 0) smem[SmemPlan::PRE + warp] = zsum;
                 __syncthreads();
-                if (!kRounds && warp != 0) break;
+                if (warp != 0) break;
                 float tot = 0.f;
 #pragma unroll
                 for (int w = 0; w < kWarps; ++w) tot += smem[SmemPlan::PRE + w];
@@ -821,7 +776,6 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
         const bool virt = phase != 1;
         last_pass = phase == 2;
         advance = !virt;
-        if (kRounds && phase == 2 && warp != 0) { wgrad_round(false); continue; }
         const int64_t base = (int64_t)tile * kTile;
         const int64_t myp = base + g + 8 * odd;
         const bool valid = virt ? false : nvalid;
@@ -1007,7 +961,6 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
                 bce_point(pred0, lab, wgt, li, dpz);
                 if (half == 0) { loss_acc += wgt * li; zsum += dpz; }
             }
-            if (kRounds) wgrad_round(false);
             continue;
         }
 #endif
@@ -1102,10 +1055,7 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
 #endif
         if (P.pred && half == 0 && valid) P.pred[myp] = pown;
 
-        if (P.label == nullptr) {   // pure inference
-            if (kRounds) wgrad_round(false);
-            continue;
-        }
+        if (P.label == nullptr) continue;   // pure inference
 
         // ---- sdf_bce_loss (utils/loss.py:17-24) + dL/dpred ---------------------------------------------
         float dpo = 0.f;
@@ -1145,7 +1095,25 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
                 db2t[j][0] = dh2[j][0] + dh2[j][2];            db2t[j][1] = dh2[j][1] + dh2[j][3];
             }
         }
-        if (DEC_GRAD) stage_afrags(stage + SmemPlan::SA2 + 256 * kp, sq, dh2);
+        if (DEC_GRAD && !GROUPED) stage_afrags(stage + SmemPlan::SA2 + 256 * kp, sq, dh2);
+        if (DEC_GRAD && GROUPED) {
+            // dh2 = dL/dpred * w3 where h2 > 0: per point its dL/dpred and the 32-bit ReLU mask of its h2 row are staged
+            // instead of the 512 values of dh2 (the four lanes of equal g hold 8 columns each of rows g and g + 8)
+            uint32_t mg = 0, mg8 = 0;
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+#pragma unroll
+                for (int q = 0; q < 2; ++q) {
+                    mg |= (h2[j][q] > 0.f ? 1u : 0u) << (8 * j + 2 * t + q);
+                    mg8 |= (h2[j][2 + q] > 0.f ? 1u : 0u) << (8 * j + 2 * t + q);
+                }
+            mg |= __shfl_xor_sync(kFull, mg, 1); mg8 |= __shfl_xor_sync(kFull, mg8, 1);
+            mg |= __shfl_xor_sync(kFull, mg, 2); mg8 |= __shfl_xor_sync(kFull, mg8, 2);
+            if (t == 0) {
+                *reinterpret_cast<float2*>(stage + SmemPlan::SDP + 2 * g) = make_float2(dp0, __uint_as_float(mg));
+                *reinterpret_cast<float2*>(stage + SmemPlan::SDP + 2 * (g + 8)) = make_float2(dp8, __uint_as_float(mg8));
+            }
+        }
         if (DEC_GRAD && t == 0) db3p += dp0 + dp8;
 
         float dh1[4][4];
@@ -1192,7 +1160,7 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
         }
 
         // ---- backward: decoder weight grads ------------------------------------------------------------------------
-        if (DEC_GRAD && !kRounds) {       // contraction over the tile's 16 points
+        if (DEC_GRAD && !GROUPED) {       // contraction over the tile's 16 points
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
                 db2p[j][0] += db2t[j][0]; db2p[j][1] += db2t[j][1];
@@ -1225,12 +1193,59 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
             }
             __syncwarp();
         }
-        if (kRounds) {                    // bias / output-layer columns here, the weight matrices by the round
-            float cols[8];   // slot 2j + q: column 8j + 2t + q of dw3 (db1, db2: sums of the round's A fragments)
+        if (DEC_GRAD && GROUPED) {        // the same contraction, dW2 accumulated into this warp's shared-memory partial
+            float cols[8];   // slot 2j + q: column 8j + 2t + q of dw3
 #pragma unroll
             for (int j = 0; j < 4; ++j) { cols[2 * j] = dw3t[j][0]; cols[2 * j + 1] = dw3t[j][1]; }
             dw3acc += reduce_scatter_g8(cols, lane);    // column 8 (g >> 1) + 2t + (g & 1)
-            wgrad_round(true);
+            __syncwarp();
+            // dW2[n2][k1] += sum_rows dh2[row][n2] * h1[row][k1], one m-tile at a time (16 accumulators); the A fragment
+            // (rows n2 = 16 mt + g, + 8; k-slots = points 4 ks + t, + 8) is rebuilt with the product dp * w3 of the
+            // forward's dh2, so it is bit-identical to it
+#pragma unroll
+            for (int mt = 0; mt < 2; ++mt) {
+                const int n = 16 * mt + g;
+                const float wn = smem[SmemPlan::W3 + n], wn8 = smem[SmemPlan::W3 + n + 8];
+                float acc[4][4];
+#pragma unroll
+                for (int nt = 0; nt < 4; ++nt) {
+                    const float4 v = *reinterpret_cast<const float4*>(w2p + 128 * (4 * mt + nt) + 4 * lane);
+                    acc[nt][0] = v.x; acc[nt][1] = v.y; acc[nt][2] = v.z; acc[nt][3] = v.w;
+                }
+#pragma unroll
+                for (int ks = 0; ks < 2; ++ks) {
+                    uint2 bh[4], bl[4];
+#pragma unroll
+                    for (int nt = 0; nt < 4; ++nt) load_bfrag(stage + SmemPlan::SB2 + (4 * ks + nt) * 64, fc, bh[nt], bl[nt]);
+                    const float2 e0 = *reinterpret_cast<const float2*>(stage + SmemPlan::SDP + 2 * (4 * ks + t));
+                    const float2 e8 = *reinterpret_cast<const float2*>(stage + SmemPlan::SDP + 2 * (4 * ks + t + 8));
+                    const uint32_t k0 = __float_as_uint(e0.y), k8 = __float_as_uint(e8.y);
+                    const float ax = (k0 >> n) & 1u ? e0.x * wn : 0.f, ay = (k0 >> (n + 8)) & 1u ? e0.x * wn8 : 0.f;
+                    const float az = (k8 >> n) & 1u ? e8.x * wn : 0.f, aw = (k8 >> (n + 8)) & 1u ? e8.x * wn8 : 0.f;
+                    db2acc[mt][0] += ax + az; db2acc[mt][1] += ay + aw;
+                    AFrag<NTF> af;
+                    af.set_packed(ax, ay, az, aw);
+                    mma3x4<NTF>(acc, af, bh, bl);
+                }
+#pragma unroll
+                for (int nt = 0; nt < 4; ++nt)
+                    *reinterpret_cast<float4*>(w2p + 128 * (4 * mt + nt) + 4 * lane) = make_float4(acc[nt][0], acc[nt][1], acc[nt][2], acc[nt][3]);
+            }
+            // dW1[n1][ch] += sum_rows dh1[row][n1] * feat[row][ch]
+#pragma unroll
+            for (int ks = 0; ks < 2; ++ks) {
+                uint2 bh, bl;
+                load_xfrag(stX, ks, fc, bh, bl);
+                AFrag<NTF> a[2];
+#pragma unroll
+                for (int mt = 0; mt < 2; ++mt) {
+                    const float4 av = *reinterpret_cast<const float4*>(stage + SmemPlan::SA1 + (2 * ks + mt) * 128 + 4 * fc);
+                    db1acc[mt][0] += av.x + av.z; db1acc[mt][1] += av.y + av.w;
+                    a[mt].set_packed(av.x, av.y, av.z, av.w);
+                }
+                mma3x2<NTF>(dW1[0], dW1[1], a[0], a[1], bh, bl, bh, bl);
+            }
+            __syncwarp();
         }
 
         // ---- backward: scatter-add into the corner-feature tables (index_put_ accumulate) -------------
@@ -1291,64 +1306,51 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
         for (int o = 16; o > 0; o >>= 1) loss_acc += __shfl_xor_sync(kFull, loss_acc, o);
         if (lane == 0 && loss_acc != 0.f) atomicAdd(P.loss, loss_acc * P.loss_scale);
     }
-    if (kRounds) {
-        // per-warp partials [dW1 fragment warp & 1: 128 | gb1 32 | gb2 32 | gw3 32 | gb3 1 | pad | dW2 block (warp & 1,
-        // (warp >> 1) & 1) over half the tiles: [16][16]] in the staging area (free after the last round), summed by the
-        // block, one global atomic per non-zero element
+    if (DEC_GRAD && GROUPED) {
+        // per-warp partials [gw1 256 | gb1 32 | gb2 32 | gw3 32 | gb3 1] in the staging area (each element has exactly one
+        // owner lane) and dW2 in its C-fragment image; the block sums the eight partials of each element and issues one
+        // global atomic per non-zero element
         float* part = stage;
-        constexpr int oB1 = 128, oB3 = 224, kParts = 225, oW2 = 256, kW2Block = 16 * 16;
+        constexpr int oB1 = 256, oB2 = 288, oW3 = 320, oB3 = 352, kVec = 353;
 #pragma unroll
-        for (int n = 0; n < 2; ++n) {
-            *reinterpret_cast<float2*>(part + oW2 + g * 16 + 8 * n + 2 * t) = make_float2(dW2acc[n][0], dW2acc[n][1]);
-            *reinterpret_cast<float2*>(part + oW2 + (g + 8) * 16 + 8 * n + 2 * t) = make_float2(dW2acc[n][2], dW2acc[n][3]);
-        }
-        *reinterpret_cast<float2*>(part + g * kF + 2 * t) = make_float2(dW1acc[0], dW1acc[1]);
-        *reinterpret_cast<float2*>(part + (g + 8) * kF + 2 * t) = make_float2(dW1acc[2], dW1acc[3]);
-        part[oB1 + 2 * kH + 8 * (g >> 1) + 2 * t + (g & 1)] = dw3acc;
-        {   // db1 / db2 rows 16 mt + g (+ 8): sums over this warp's k-slots, then over the 4 lanes of equal g
-            const int mt = warp & 1, np = (warp >> 1) & 1;
+        for (int mt = 0; mt < 2; ++mt) {
+            *reinterpret_cast<float2*>(part + (16 * mt + g) * kF + 2 * t) = make_float2(dW1[mt][0], dW1[mt][1]);
+            *reinterpret_cast<float2*>(part + (16 * mt + g + 8) * kF + 2 * t) = make_float2(dW1[mt][2], dW1[mt][3]);
 #pragma unroll
-            for (int r = 0; r < 2; ++r) {
-                float d1 = db1acc[r], d2 = db2acc[r];
+            for (int r = 0; r < 2; ++r) {   // db1 / db2 rows 16 mt + g + 8 r: sums over this lane's k-slots, then over the
+                float d1 = db1acc[mt][r], d2 = db2acc[mt][r];   // 4 lanes of equal g
 #pragma unroll
                 for (int o = 1; o < 4; o <<= 1) { d1 += __shfl_xor_sync(kFull, d1, o); d2 += __shfl_xor_sync(kFull, d2, o); }
-                if (t == 0) {
-                    part[oB1 + 16 * mt + g + 8 * r] = d1;           part[oB1 + 16 * (1 - mt) + g + 8 * r] = 0.f;
-                    part[oB1 + kH + 16 * mt + g + 8 * r] = np == 0 ? d2 : 0.f;   part[oB1 + kH + 16 * (1 - mt) + g + 8 * r] = 0.f;
-                }
+                if (t == 0) { part[oB1 + 16 * mt + g + 8 * r] = d1; part[oB2 + 16 * mt + g + 8 * r] = d2; }
             }
         }
+        part[oW3 + 8 * (g >> 1) + 2 * t + (g & 1)] = dw3acc;
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) db3p += __shfl_xor_sync(kFull, db3p, o);
         if (lane == 0) part[oB3] = db3p;
         __syncthreads();
-        constexpr int kVecEnd = 2 * oB1 + (kParts - oB1);
-        for (int i = tid; i < kVecEnd + 4 * kW2Block; i += blockDim.x) {
+        for (int i = tid; i < kVec + kH * kH; i += blockDim.x) {
             float v = 0.f;
             float* dst;
-            if (i < 2 * oB1) {      // dW1 row 16 m + r: the partials of warps m, m + 2, m + 4, m + 6
-                const int m = i / oB1, e = i % oB1;
+            if (i < kVec) {
 #pragma unroll
-                for (int c = 0; c < kWarps / 2; ++c) v += smem[SmemPlan::STAGE + (2 * c + m) * SmemPlan::kStagePerWarp + e];
-                dst = P.dec.gw1 + 16 * m * kF + e;
-            } else if (i >= kVecEnd) {      // dW2 block b = (row block b & 1, column block b >> 1): warps b and b + 4
-                const int b = (i - kVecEnd) / kW2Block, e = (i - kVecEnd) % kW2Block;
-                const float* p0 = smem + SmemPlan::STAGE + b * SmemPlan::kStagePerWarp + oW2 + e;
-                v = p0[0] + p0[4 * SmemPlan::kStagePerWarp];
-                dst = P.dec.gw2 + (16 * (b & 1) + e / 16) * kH + 16 * (b >> 1) + e % 16;
-            } else {
-                const int e = i - oB1;
-#pragma unroll
-                for (int w = 0; w < kWarps; ++w) v += smem[SmemPlan::STAGE + w * SmemPlan::kStagePerWarp + e];
-                if (e < oB1 + kH) dst = P.dec.gb1 ? P.dec.gb1 + (e - oB1) : nullptr;
-                else if (e < oB1 + 2 * kH) dst = P.dec.gb2 ? P.dec.gb2 + (e - oB1 - kH) : nullptr;
-                else if (e < oB3) dst = P.dec.gw3 + (e - oB1 - 2 * kH);
+                for (int w = 0; w < kWarps; ++w) v += smem[SmemPlan::STAGE + w * kStage + i];
+                if (i < oB1) dst = P.dec.gw1 + i;
+                else if (i < oB2) dst = P.dec.gb1 ? P.dec.gb1 + (i - oB1) : nullptr;
+                else if (i < oW3) dst = P.dec.gb2 ? P.dec.gb2 + (i - oB2) : nullptr;
+                else if (i < oB3) dst = P.dec.gw3 + (i - oW3);
                 else dst = P.dec.gb3;
+            } else {   // dW2[r][c]: fragment (r >> 4, c >> 3), lane 4 (r & 7) + ((c & 7) >> 1), register 2 ((r >> 3) & 1) + (c & 1)
+                const int e = i - kVec, r = e / kH, c = e % kH;
+                const int f = 128 * (4 * (r >> 4) + (c >> 3)) + 4 * (4 * (r & 7) + ((c & 7) >> 1)) + 2 * ((r >> 3) & 1) + (c & 1);
+#pragma unroll
+                for (int w = 0; w < kWarps; ++w) v += w2p[(w - warp) * SmemPlan::kW2Part + f];
+                dst = P.dec.gw2 + e;
             }
             if (v != 0.f && dst) atomicAdd(dst, v);
         }
     }
-    if (DEC_GRAD && !kRounds) {
+    if (DEC_GRAD && !GROUPED) {
         // every warp writes its complete partial gradient vector [gw1 256 | gb1 32 | gw2 1024 | gb2 32 | gw3 32 | gb3 1]
         // into its own staging area (each element has exactly one owner lane: plain stores, no shared-memory atomics),
         // then the block sums the eight vectors and issues one global atomic per non-zero element
@@ -1388,7 +1390,7 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
         for (int i = tid; i < SmemPlan::kDecGradFloats; i += blockDim.x) {
             float v = 0.f;
 #pragma unroll
-            for (int w = 0; w < kWarps; ++w) v += smem[SmemPlan::STAGE + w * SmemPlan::kStagePerWarp + i];
+            for (int w = 0; w < kWarps; ++w) v += smem[SmemPlan::STAGE + w * kStage + i];
             if (v == 0.f) continue;
             float* dst;
             if (i < oB1) dst = P.dec.gw1 + i;
@@ -1723,8 +1725,8 @@ int check_decoder(const shine_decoder* d, const shine_octree* o) {
 template <int NTF, bool TRAIN, bool DEC_GRAD, int LMAX, bool GROUPED = false>
 int launch_fused_t(const StepParams& P, cudaStream_t st) {
     auto kern = sdf_fused_kernel<NTF, TRAIN, DEC_GRAD, LMAX, GROUPED>;
-    const int smem_floats = SmemPlan::STAGE + (DEC_GRAD ? 8 * SmemPlan::kStagePerWarp : 0) +
-                            (GROUPED ? 8 * (LMAX * SmemPlan::kGroupPerLevel + (DEC_GRAD ? 0 : kTile * kF)) : 0);
+    const int smem_floats = SmemPlan::STAGE + (DEC_GRAD ? 8 * SmemPlan::stage_per_warp(GROUPED) : 0) +
+                            (GROUPED ? 8 * (LMAX * SmemPlan::kGroupPerLevel + (DEC_GRAD ? SmemPlan::kW2Part : kTile * kF)) : 0);
     const size_t smem_bytes = (size_t)smem_floats * sizeof(float);
     static int per_sm_by_dev[kMaxDevices] = {0};   // per template instantiation AND per device: the >48 KB dynamic
     int& per_sm_cached = per_sm_by_dev[current_device()];   // shared-memory opt-in is a per-device function attribute
