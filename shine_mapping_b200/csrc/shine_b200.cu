@@ -21,35 +21,9 @@
 
 #include "shine_b200.h"
 
-// tuning switches.  Front-end of the fused kernel: reading key + 4 corner rows as one 32-byte sector per level (every
-// lane probes every level) is used for inference; the training kernel keeps the level-split key probe + ids load, which
-// issues fewer instructions.
-#ifndef SHINE_SECTOR_PROBE_TRAIN
-#define SHINE_SECTOR_PROBE_TRAIN 0
-#endif
-#ifndef SHINE_SECTOR_PROBE_INFER
-#define SHINE_SECTOR_PROBE_INFER 1
-#endif
-#ifndef SHINE_CPASYNC_PREFETCH
-#define SHINE_CPASYNC_PREFETCH 0  // 1: next tile's inputs via cp.async to shared memory; 0: register prefetch (timing-neutral)
-#endif
+// tuning constants
 #ifndef SHINE_GATHER_GROUP
 #define SHINE_GATHER_GROUP 2  // levels whose first-probe sectors are in flight together (register pressure vs parallelism)
-#endif
-#ifndef SHINE_SLOT_PREFETCH
-#define SHINE_SLOT_PREFETCH 0  // training kernel: hash + L1 prefetch of the NEXT tile's home slots before this tile's scatter
-#endif
-#ifndef SHINE_ZERO_TILE_SKIP
-#define SHINE_ZERO_TILE_SKIP 1   // tiles whose 16 points miss every level: prediction of the zero feature vector, decoder gradients by linearity
-#endif
-#ifndef SHINE_DYNAMIC_TILES
-#define SHINE_DYNAMIC_TILES 0    // 1: warps draw their tiles from a device counter (measured slower: concurrent warps then share rows)
-#endif
-#ifndef SHINE_PERMUTE_TILES
-#define SHINE_PERMUTE_TILES 0    // 1: multiplicative permutation of the tile order (measured slower: a block loses its adjacent tiles)
-#endif
-#ifndef SHINE_EXPERIMENT_NO_RED
-#define SHINE_EXPERIMENT_NO_RED 0
 #endif
 #ifndef SHINE_TRAIN_MINB
 #define SHINE_TRAIN_MINB 2    // min resident blocks/SM of the training kernels (register cap 65536/(256*MINB))
@@ -57,7 +31,7 @@
 // The per-point training kernels with decoder gradients keep 56 accumulators per lane live through the whole tile: at 2
 // blocks/SM (128 registers) they spill ~0.5 KB per thread, at 1 block/SM (255) they do not, and on H100 the spill-free
 // build is faster (C2 batch in the order drawn, kernel: 0.460 vs 0.564 ms).  The grouped kernel timed on Morton-ordered batches
-// keeps its dW2 partial in shared memory and fits SHINE_TRAIN_MINB without spilling.
+// keeps its dW2 partial in shared memory and fits SHINE_TRAIN_MINB with a 4-byte spill.
 #ifndef SHINE_TRAIN_DECGRAD_MINB
 #define SHINE_TRAIN_DECGRAD_MINB 1
 #endif
@@ -394,9 +368,10 @@ struct SmemPlan {
     static constexpr int B3 = W3 + kH;                 // [1]
     static constexpr int GSCALE = B3 + 1;              // [1] (+2 pad) dL/dpred scale: read per tile, not held in a register
     static constexpr int kDecGradFloats = kH * kF + kH + kH * kH + kH + kH + 1;   // 1377 (a warp's partial goes to its staging area)
-    static constexpr int PRE = B3 + 4;                 // per-warp input prefetch: [16][3] coord | [16] label | [16] weight
-    static constexpr int kPrePerWarp = 5 * kTile;
-    static constexpr int STAGE = PRE + 8 * kPrePerWarp;   // per-warp staging of one tile, in mma fragment order (below)
+    static constexpr int ZSUM = B3 + 4;                // [8] the warps' dL/dpred sums of their zero tiles (zero-tile shortcut)
+    static constexpr int kZsumFloats = 8 * 5 * kTile;  // more than the 8 sums need: the offsets below and the block's
+                                                       // shared-memory footprint were timed with this size
+    static constexpr int STAGE = ZSUM + kZsumFloats;   // per-warp staging of one tile, in mma fragment order (below)
     static constexpr int SB2 = 0;                      // h1:  B fragments of dW2, [k-step 2][n-tile 4][32 lanes][2]
     static constexpr int SA1 = SB2 + kTile * kH;       // dh1: A fragments of dW1, [k-step 2][m-tile 2][32 lanes][4]
     static constexpr int SX = SA1 + kTile * kH;        // feat: B fragments of dW1, [k-step 2][32 lanes][2]
@@ -594,9 +569,9 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
     //   dw3: reduced per tile to 1 column per lane (reduce_scatter_g8);  db3: lane sums.
     float dw3acc = 0.f, db2acc[2][2] = {{0.f, 0.f}, {0.f, 0.f}}, db1acc[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
 
-    constexpr bool kSectorProbe = TRAIN ? (SHINE_SECTOR_PROBE_TRAIN != 0) : (SHINE_SECTOR_PROBE_INFER != 0);
-    constexpr bool kSlotPrefetch = TRAIN && !kSectorProbe && (SHINE_SLOT_PREFETCH != 0) && (SHINE_CPASYNC_PREFETCH == 0);
-    constexpr bool kZeroSkip = (SHINE_ZERO_TILE_SKIP != 0) && (SHINE_CPASYNC_PREFETCH == 0);
+    // hash walk: inference reads key + its 4 corner rows as one 32-byte sector per level (every lane probes every level);
+    // training uses the level-split walk, because the grouped scatter needs the node slots it resolves
+    constexpr bool kSectorProbe = !TRAIN;
     const bool poly = P.oct.poly_interp != 0;
     const int L = P.oct.num_levels;
 
@@ -632,90 +607,11 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
     for (int i = 1; i < LMAX; ++i)
         if (i < L && P.oct.lv[i].level != P.oct.lv[0].level - i) consecutive = false;
 
-    // staged one tile ahead (kSlotPrefetch): leaf Morton key and home-slot indices of this lane's levels; both 32-byte
-    // sectors of each home slot are pulled into L1 while the previous tile scatters, so the key and corner-id loads of the
-    // walk below hit L1 and only the row gather pays an L2 round trip
-    unsigned long long skey0 = 0ull;
-    int smine[LMAX / 2];
-    uint4 skf[LMAX / 2];
-#pragma unroll
-    for (int j = 0; j < LMAX / 2; ++j) smine[j] = -1;
-    auto stage_slots = [&](bool v, float sx, float sy, float sz) {
-        skey0 = v ? morton_of(sx, sy, sz, P.oct.lv[0].level) : 0ull;
-#pragma unroll
-        for (int j = 0; j < LMAX / 2; ++j) {
-            const int i = 2 * j + half;
-            smine[j] = -1;
-            if (i < L && v) {
-                const shine_level& lv = P.oct.lv[i];
-                const unsigned long long kq = consecutive ? (skey0 >> (3 * i)) : morton_of(sx, sy, sz, lv.level);
-                smine[j] = (int)(hash_key(kq) & (lv.hash_capacity - 1));
-                const HashSlot* sp = reinterpret_cast<const HashSlot*>(lv.hash_slots) + smine[j];
-                if (SHINE_SLOT_PREFETCH == 2) {          // the home-slot load itself is issued a scatter phase early
-                    skf[j] = __ldg(reinterpret_cast<const uint4*>(sp));
-                } else {
-                    asm volatile("prefetch.global.L1 [%0];" ::"l"(sp));
-                    asm volatile("prefetch.global.L1 [%0];" ::"l"(reinterpret_cast<const char*>(sp) + 32));
-                }
-            }
-        }
-    };
-
-    // sequence number of a warp's work item -> tile index (identity, or a multiplicative permutation of the tiles)
-    auto tile_of = [&](int seq) -> int {
-        if constexpr (SHINE_PERMUTE_TILES != 0)
-            return (P.tile_perm_mul > 1 && seq < P.num_tiles) ? (int)(((long long)seq * P.tile_perm_mul) % P.num_tiles) : seq;
-        else
-            return seq;
-    };
-
-#if SHINE_CPASYNC_PREFETCH
-    // software pipeline, depth 1: the next tile's coordinates / label / weight travel global -> shared memory with
-    // cp.async (no registers pinned, nothing to spill) while this tile computes
-    float* pre = smem + SmemPlan::PRE + warp * SmemPlan::kPrePerWarp;
-    const uint32_t pre_s = (uint32_t)__cvta_generic_to_shared(pre);
-    auto prefetch_inputs = [&](int tl) {
-        if (tl < P.num_tiles) {
-            const int64_t base = (int64_t)tl * kTile;
-            const int64_t left = P.n - base;                      // > 0
-            const int npts = left < kTile ? (int)left : kTile;
-            // words 0..47: coord, 48..63: label, 64..79: weight
-#pragma unroll
-            for (int r = 0; r < 3; ++r) {
-                const int wd = lane + 32 * r;
-                const float* src = nullptr;
-                if (wd < 48) { if (wd < 3 * npts) src = P.coord + 3 * base + wd; }
-                else if (wd < 64) { if (P.label && wd - 48 < npts) src = P.label + base + (wd - 48); }
-                else if (wd < 80) { if (P.weighted && wd - 64 < npts) src = P.weight + base + (wd - 64); }
-                if (src) asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(pre_s + 4u * (uint32_t)wd), "l"(src) : "memory");
-            }
-        }
-        asm volatile("cp.async.commit_group;" ::: "memory");
-    };
-    prefetch_inputs(warp_global);
-
-    for (int tile = warp_global; tile < P.num_tiles; tile += warp_stride) {
-        const int64_t base = (int64_t)tile * kTile;
-        const int64_t myp = base + g + 8 * odd;
-        asm volatile("cp.async.wait_group 0;" ::: "memory");
-        __syncwarp();
-        const bool valid = myp < P.n;
-        float x = 0.f, y = 0.f, z = 0.f, lab = 0.f, wgt = 1.f;
-        if (valid) {
-            const int lp = g + 8 * odd;
-            x = pre[3 * lp]; y = pre[3 * lp + 1]; z = pre[3 * lp + 2];
-            if (P.label) lab = pre[48 + lp];
-            if (P.weighted) wgt = fabsf(pre[64 + lp]);   // shine_batch.py:172 abs()
-        }
-        __syncwarp();
-        prefetch_inputs(tile + warp_stride);
-
-#else
     // software pipeline, depth 1: the next tile's coordinates / label are in flight (registers) while this tile computes
     float nx = 0.f, ny = 0.f, nz = 0.f, nlab = 0.f, nwgt = 1.f;
     bool nvalid = false;
     auto prefetch_inputs = [&](int tl) {
-        const int64_t p = (int64_t)tile_of(tl) * kTile + g + 8 * odd;
+        const int64_t p = (int64_t)tl * kTile + g + 8 * odd;
         nvalid = tl < P.num_tiles && p < P.n;
         if (nvalid) {
             nx = __ldg(P.coord + 3 * p); ny = __ldg(P.coord + 3 * p + 1); nz = __ldg(P.coord + 3 * p + 2);
@@ -724,15 +620,14 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
         }
     };
     prefetch_inputs(warp_global);
-    if (kSlotPrefetch) stage_slots(nvalid, nx, ny, nz);   // first tile
 
-    // Zero-tile shortcut (kZeroSkip).  A point that misses every level has the feature vector 0, so every such point gets the
+    // Zero-tile shortcut.  A point that misses every level has the feature vector 0, so every such point gets the
     // SAME prediction pred0 = Decoder.sdf(0), and its decoder gradients are dL/dpred times the gradients of that one forward:
     // linear in dL/dpred.  In a Morton-ordered batch free-space samples fill whole tiles (35 % of the C2 tiles): such a tile
     // only walks the hash, evaluates its loss terms against pred0 and adds its dL/dpred to a sum.  Pass 0 of the loop below
     // is one virtual tile (no points: features 0) run through the forward to get pred0; after the block's real tiles, warp 0
     // runs one more virtual tile whose first point carries the block's dL/dpred sum through the ordinary backward.
-    int phase = kZeroSkip ? 0 : 1;          // 0: virtual forward, 1: this warp's tiles, 2: virtual backward (warp 0)
+    int phase = 0;                          // 0: virtual forward, 1: this warp's tiles, 2: virtual backward (warp 0)
     bool advance = false, last_pass = false;
     float pred0 = 0.f, zsum = 0.f;
     auto bce_point = [&](float pv, float lb, float wg, float& li, float& dp) {
@@ -747,25 +642,20 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
             dp = (sg - zt) * wg * smem[SmemPlan::GSCALE];
         }
     };
-    // tile schedule: the first tile of a warp is its global index; every further one is drawn from P.tile_counter (counter
-    // value k <-> tile warp_stride + k), requested a whole tile ahead so that the atomic's latency is never waited for
-    const bool dynamic = (SHINE_DYNAMIC_TILES != 0) && P.tile_counter != nullptr;
-    int next_tile = 0, pending = 0;
-    if (dynamic && lane == 0) pending = atomicAdd(P.tile_counter, 1);
-    for (int seq = warp_global;; seq = !advance ? seq : (dynamic ? next_tile : seq + warp_stride)) {
+    for (int seq = warp_global;; seq = advance ? seq + warp_stride : seq) {
         if (last_pass) break;
-        const int tile = tile_of(seq);
+        const int tile = seq;
         if (phase == 1 && seq >= P.num_tiles) {
-            if constexpr (kZeroSkip && DEC_GRAD) {
+            if constexpr (DEC_GRAD) {
                 // hand the all-miss dL/dpred sums of the block's warps to warp 0 (every warp passes here exactly once)
 #pragma unroll
                 for (int o = 16; o > 0; o >>= 1) zsum += __shfl_xor_sync(kFull, zsum, o);
-                if (lane == 0) smem[SmemPlan::PRE + warp] = zsum;
+                if (lane == 0) smem[SmemPlan::ZSUM + warp] = zsum;
                 __syncthreads();
                 if (warp != 0) break;
                 float tot = 0.f;
 #pragma unroll
-                for (int w = 0; w < kWarps; ++w) tot += smem[SmemPlan::PRE + w];
+                for (int w = 0; w < kWarps; ++w) tot += smem[SmemPlan::ZSUM + w];
                 if (tot == 0.f) break;
                 zsum = tot;
                 phase = 2;
@@ -780,17 +670,8 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
         const int64_t myp = base + g + 8 * odd;
         const bool valid = virt ? false : nvalid;
         const float x = nx, y = ny, z = nz, lab = nlab, wgt = nwgt;
-        if (!virt) {
-            if (dynamic) {
-                next_tile = warp_stride + __shfl_sync(kFull, pending, 0);
-                prefetch_inputs(next_tile);
-                if (lane == 0) pending = atomicAdd(P.tile_counter, 1);
-            } else {
-                prefetch_inputs(seq + warp_stride);
-            }
-        }
+        if (!virt) prefetch_inputs(seq + warp_stride);
 
-#endif
         float feat[4];
         float pk[kPark];      // [3i..3i+2] = tx,ty,tz of level i (kept over the MLP phase for the scatter)
         float idp[kIdPark];   // [4i..4i+3] = rows of this lane's corners (z bit == half) of level i, -1 on a miss
@@ -863,7 +744,7 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
         int slot[LMAX];
         {
             constexpr int LH = LMAX / 2;
-            const unsigned long long key0 = kSlotPrefetch ? skey0 : (valid ? morton_of(x, y, z, P.oct.lv[0].level) : 0ull);
+            const unsigned long long key0 = valid ? morton_of(x, y, z, P.oct.lv[0].level) : 0ull;
             unsigned long long kq[LH];
             uint4 kf[LH];          // home slot: {key lo, key hi, node, maxdisp}
             int mine[LH];
@@ -875,8 +756,8 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
                     const shine_level& lv = P.oct.lv[i];
                     const HashSlot* slots = reinterpret_cast<const HashSlot*>(lv.hash_slots);
                     kq[j] = consecutive ? (key0 >> (3 * i)) : morton_of(x, y, z, lv.level);
-                    mine[j] = kSlotPrefetch ? smine[j] : (int)(hash_key(kq[j]) & (lv.hash_capacity - 1));
-                    kf[j] = (kSlotPrefetch && SHINE_SLOT_PREFETCH == 2) ? skf[j] : __ldg(reinterpret_cast<const uint4*>(slots + mine[j]));
+                    mine[j] = (int)(hash_key(kq[j]) & (lv.hash_capacity - 1));
+                    kf[j] = __ldg(reinterpret_cast<const uint4*>(slots + mine[j]));
                 }
             }
 #pragma unroll
@@ -950,8 +831,7 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
             }
         }
         }
-#if !SHINE_CPASYNC_PREFETCH
-        if (kZeroSkip && phase == 1 && __ballot_sync(kFull, hitmask != 0u) == 0u) {
+        if (phase == 1 && __ballot_sync(kFull, hitmask != 0u) == 0u) {
             // no point of this tile sees a node on any level: features 0, prediction pred0, no table gradient; the decoder
             // gradients follow by linearity from the sum of dL/dpred (virtual backward tile at the end of the block)
             if (!TRAIN && P.mask && half == 0 && valid) P.mask[myp] = 0;
@@ -963,7 +843,6 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
             }
             continue;
         }
-#endif
         if (!TRAIN && P.mask) {
             bool present = false;
 #pragma unroll
@@ -1050,9 +929,7 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
         const float b3 = smem[SmemPlan::B3];
         p0 += b3; p8 += b3;
         const float pown = odd ? p8 : p0;
-#if !SHINE_CPASYNC_PREFETCH
-        if (kZeroSkip && phase == 0) { pred0 = pown; phase = 1; continue; }     // the virtual forward: every row is Decoder.sdf(0)
-#endif
+        if (phase == 0) { pred0 = pown; phase = 1; continue; }     // the virtual forward: every row is Decoder.sdf(0)
         if (P.pred && half == 0 && valid) P.pred[myp] = pown;
 
         if (P.label == nullptr) continue;   // pure inference
@@ -1060,26 +937,12 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
         // ---- sdf_bce_loss (utils/loss.py:17-24) + dL/dpred ---------------------------------------------
         float dpo = 0.f;
         if (valid) {
-#if !SHINE_CPASYNC_PREFETCH
             float li;
             bce_point(pown, lab, wgt, li, dpo);
             if (half == 0) loss_acc += wgt * li;
-#else
-            const float zt = __fdividef(1.0f, 1.0f + __expf(-__fdividef(lab, P.sigma)));   // sigmoid(label / sigma)
-            const float e = __expf(-fabsf(pown));
-            const float li = fmaxf(pown, 0.f) - pown * zt + __logf(1.0f + e);              // log1p(e), e in (0, 1]
-            if (half == 0) loss_acc += wgt * li;
-            if (TRAIN) {
-                const float rs = __fdividef(1.0f, 1.0f + e);
-                const float sg = pown >= 0.f ? rs : e * rs;                               // sigmoid(pred)
-                dpo = (sg - zt) * wgt * smem[SmemPlan::GSCALE];
-            }
-#endif
         }
         if (!TRAIN) continue;
-#if !SHINE_CPASYNC_PREFETCH
-        if (kZeroSkip && phase == 2) dpo = (g == 0 && odd == 0) ? zsum : 0.f;   // point 0 of the virtual tile carries the block's sum
-#endif
+        if (phase == 2) dpo = (g == 0 && odd == 0) ? zsum : 0.f;   // point 0 of the virtual tile carries the block's sum
 
         // ---- backward: MLP dgrad on tensor cores ------------------------------------------------------
         const float dpx = __shfl_xor_sync(kFull, dpo, 1);
@@ -1249,11 +1112,7 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
         }
 
         // ---- backward: scatter-add into the corner-feature tables (index_put_ accumulate) -------------
-#if !SHINE_CPASYNC_PREFETCH
-        if (kSlotPrefetch) stage_slots(nvalid, nx, ny, nz);   // next tile's hash + slot prefetch rides under the scatter
-#endif
         if constexpr (GROUPED) {
-            static_assert(!GROUPED || !kSectorProbe, "the grouped scatter reads the node slots of the level-split walk");
             grouped_scatter<LMAX>(P, L, tile, gpt, gdx, dxc, lane);
             continue;
         }
@@ -1290,9 +1149,6 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
                         const f2_t wk = f2_pack(w[k], w[k]);
                         float g0, g1, g2, g3;
                         f2_unpack(f2_mul(wk, dx01), g0, g1); f2_unpack(f2_mul(wk, dx23), g2, g3);
-#if SHINE_EXPERIMENT_NO_RED      // bound experiment: what the step costs without the scatter's memory traffic
-                        if (P.sigma == -12345.f)
-#endif
                         red_add_f4(gb + (int64_t)ids[c + k] * kF, g0, g1, g2, g3);
                     }
                 }
@@ -1756,36 +1612,7 @@ int launch_fused_t(const StepParams& P, cudaStream_t st) {
     int grid = sm_count() * per_sm;
     if (grid > blocks_needed) grid = blocks_needed;
     if (grid < 1) grid = 1;
-    // dynamic tile schedule: the warps draw tile indices from a device counter (tiles differ a lot in cost once whole tiles
-    // of free-space samples take the zero-tile shortcut).  A small ring of counters per device: a launch zeroes its own.
-    StepParams Q = P;
-    Q.tile_counter = nullptr;
-    Q.tile_perm_mul = 0;
-#if SHINE_PERMUTE_TILES
-    if (P.num_tiles > 4 * grid * 8) {        // several rounds of tiles per warp: decorrelate what an SM gets from the batch order
-        auto gcd = [](long long a, long long b) { while (b) { const long long t = a % b; a = b; b = t; } return a; };
-        long long m = (long long)(0.6180339887 * (double)P.num_tiles) | 1;
-        while (gcd(m, P.num_tiles) != 1) m += 2;
-        Q.tile_perm_mul = (int32_t)m;
-    }
-#endif
-#if SHINE_DYNAMIC_TILES
-    {
-        static int32_t* ring_by_dev[kMaxDevices] = {nullptr};
-        static unsigned next_by_dev[kMaxDevices] = {0};
-        constexpr unsigned kRing = 64;
-        const int dev = current_device();
-        if (!ring_by_dev[dev]) {
-            e = cudaMalloc(reinterpret_cast<void**>(&ring_by_dev[dev]), kRing * 64);      // one 64-byte line per counter
-            if (e != cudaSuccess) return (int)e;
-        }
-        int32_t* ctr = ring_by_dev[dev] + 16 * (next_by_dev[dev]++ % kRing);
-        e = cudaMemsetAsync(ctr, 0, sizeof(int32_t), st);
-        if (e != cudaSuccess) return (int)e;
-        Q.tile_counter = ctr;
-    }
-#endif
-    kern<<<grid, 256, smem_bytes, st>>>(Q);
+    kern<<<grid, 256, smem_bytes, st>>>(P);
     return (int)cudaGetLastError();
 }
 
@@ -1835,7 +1662,7 @@ int fill_params(StepParams& P, const shine_octree* oct, const shine_decoder* dec
     P.oct = *oct; P.dec = *dec; P.coord = coord; P.n = n;
     P.num_tiles = (int32_t)((n + kTile - 1) / kTile);
     P.label = nullptr; P.weight = nullptr; P.d_loss = nullptr; P.pred = nullptr; P.loss = nullptr; P.mask = nullptr;
-    P.mask_level = 0; P.sigma = 1.f; P.loss_scale = 1.f; P.weighted = 0; P.debug_dx = nullptr; P.tile_counter = nullptr; P.tile_perm_mul = 0;
+    P.mask_level = 0; P.sigma = 1.f; P.loss_scale = 1.f; P.weighted = 0; P.debug_dx = nullptr;
     return SHINE_OK;
 }
 

@@ -29,9 +29,6 @@ struct StepParams {
     float loss_scale;
     int32_t weighted;
     float* debug_dx;         // development aid: dL/dfeature rows [n, 8] of the tcgen05 training kernel (NULL in normal use)
-    int32_t* tile_counter;   // fused kernels: zeroed device counter the warps draw their tiles from (NULL: static round-robin)
-    int32_t tile_perm_mul;   // > 1: the k-th tile taken is tile (k * mul) mod num_tiles (mul coprime to num_tiles): spreads the
-                             // work of concurrently running warps over the whole batch whatever its order
 };
 
 // shine_train_tc.cu: the warp-specialised tcgen05 training kernel (SHINE_FLAG_TCGEN05 on shine_sdf_bce_step)
