@@ -295,6 +295,29 @@ int shine_pool_window_append(const shine_sample_pool* pool, const float* coord, 
                              int64_t n_new, float ox, float oy, float oz, float radius, int64_t* size_out, void* scratch,
                              int64_t scratch_bytes, void* stream);
 
+/* ---- the batch-mode sample pool in pinned host memory (more than `pc_count_gpu_limit` scans) ------------------------
+ * Replaces the CPU pools of dataset/lidar_dataset.py:94-101 and the CPU-side gather + copy of get_batch (:431-448).
+ * Record i is 32 bytes, 32-byte aligned, {x, y, z, label, weight, 0, 0, 0} fp32, at byte (i & (2^chunk_shift - 1)) * 32 of
+ * chunk i >> chunk_shift.  Chunks are pinned (page-locked) host memory the GPU addresses directly (unified addressing);
+ * `chunks` is a DEVICE array of num_chunks such pointers, on the GPU that runs the kernels. */
+typedef struct shine_host_pool {
+    void* const* chunks;      /* device [num_chunks] pointers to pinned host chunks of 2^chunk_shift records each        */
+    int32_t chunk_shift;      /* 5 .. 31                                                                                  */
+    int32_t num_chunks;
+    int64_t size;             /* records in the pool: gather indices must lie in [0, size); <= num_chunks << chunk_shift   */
+} shine_host_pool;
+
+/* Pack a frame's device samples (coord [n,3], label [n], weight [n] fp32) into records at + 0 .. at + n - 1 (one launch;
+ * the run may cross chunk boundaries).  at + n must not exceed num_chunks << chunk_shift; `size` is not read or changed. */
+int shine_host_pool_append(const shine_host_pool* pool, int64_t at, const float* coord, const float* label,
+                           const float* weight, int64_t n, void* stream);
+
+/* The batch of get_batch: coord_out[t] = (x, y, z), label_out[t], weight_out[t] of record index[t], t < n (int64 device
+ * indices; device outputs [n,3], [n], [n]).  One launch, no host synchronisation: capturable in a CUDA graph.  An index
+ * outside [0, size) gives NaN coordinates and label = weight = 0. */
+int shine_host_pool_gather(const shine_host_pool* pool, const int64_t* index, int64_t n, float* coord_out,
+                           float* label_out, float* weight_out, void* stream);
+
 /* ---- multi-GPU exchange (SURVEY.md 8e, 8b export (6); the reference is single-GPU) --------------------------------
  * One process per GPU.  The map is partitioned by Morton prefix at the coarsest featured level; every rank owns the
  * rows reachable from its blocks, so corner rows on a face between two blocks exist on both ranks.  Their gradients

@@ -97,6 +97,10 @@ class ShineSamplePool(C.Structure):
                 ("capacity", C.c_int64)]
 
 
+class ShineHostPool(C.Structure):
+    _fields_ = [("chunks", C.c_void_p), ("chunk_shift", C.c_int32), ("num_chunks", C.c_int32), ("size", C.c_int64)]
+
+
 # name -> (restype, argtypes); every symbol declared in include/shine_b200.h
 _vp, _i64, _i32, _u32, _f32 = C.c_void_p, C.c_int64, C.c_int32, C.c_uint32, C.c_float
 _OCT, _DEC = C.POINTER(ShineOctree), C.POINTER(ShineDecoder)
@@ -144,6 +148,8 @@ SYMBOLS = {
     "shine_pool_scratch_bytes": (C.c_int64, [_i64]),
     "shine_pool_window_append": (C.c_int, [C.POINTER(ShineSamplePool), _vp, _vp, _vp, _i64, _f32, _f32, _f32, _f32, _vp,
                                            _vp, _i64, _vp]),
+    "shine_host_pool_append": (C.c_int, [C.POINTER(ShineHostPool), _i64, _vp, _vp, _vp, _i64, _vp]),
+    "shine_host_pool_gather": (C.c_int, [C.POINTER(ShineHostPool), _vp, _i64, _vp, _vp, _vp, _vp]),
 }
 
 _lib = None

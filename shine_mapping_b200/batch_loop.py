@@ -180,7 +180,10 @@ def main(argv=None):
     torch.manual_seed(config.seed)
     octree, decoder = FeatureOctree(config), Decoder(config)
     print("Load, preprocess and sample data (synthetic scans)")
-    pool = synth.build_scene_map(config, octree, args.synthetic_azimuth, args.frames, seed=config.seed)
+    # more than pc_count_gpu_limit scans: the pool lives in pinned host memory (dataset/lidar_dataset.py:94-101)
+    pool = synth.build_scene_map(config, octree, args.synthetic_azimuth, args.frames, seed=config.seed, pool="auto")
+    where = "pinned host memory" if isinstance(pool, synth.HostSamplePool) else "device memory"
+    print(f"Sample pool: {type(pool).__name__} in {where}, {len(pool)} samples")
     octree.print_detail()
     print("Begin mapping")
     out = run_shine_mapping_batch(config, octree, decoder, pool, iters=args.iters, log_every=1000)

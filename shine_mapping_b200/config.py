@@ -66,6 +66,8 @@ _YAML_MAP = {
     "setting.first_frame_ref": ("first_frame_ref", None), "setting.begin_frame": ("begin_frame", None),
     "setting.end_frame": ("end_frame", None), "setting.every_frame": ("every_frame", None),
     "setting.device": ("device", None), "setting.gpu_id": ("gpu_id", None),
+    # not read from YAML by the reference (utils/config.py:35 keeps the default 500); accepted here so a config can set it
+    "setting.pc_count_gpu_limit": ("pc_count_gpu_limit", int),
     "process.min_range_m": ("min_range", None), "process.pc_radius_m": ("pc_radius", None),
     "process.rand_downsample": ("rand_downsample", None), "process.vox_down_m": ("vox_down_m", None),
     "process.rand_down_r": ("rand_down_r", None), "process.min_z_m": ("min_z", None),

@@ -11,6 +11,8 @@
                       (dataset/lidar_dataset.py:104-113,431-448): `torch.randint` gather.
 * `ReplayPool`      — the pool of incremental mapping with replay: earlier frames' samples kept, those outside the
                       sliding window dropped on the GPU before the frame is appended (dataset/lidar_dataset.py:235-271).
+* `HostSamplePool`  — the batch-mode pool in pinned host memory past `pc_count_gpu_limit` scans (dataset/lidar_dataset.py:
+                      94-101), gathered on the GPU; `use_host_pool` states the reference's rule.
 * `build_scene_map` — scans -> samples -> `octree.update(surface samples)` (dataset/lidar_dataset.py:204-218).
 """
 from __future__ import annotations
@@ -236,6 +238,120 @@ class ReplayPool(SamplePool):
         raise NotImplementedError("ReplayPool keeps the reference's sample order (the window filter preserves it)")
 
 
+class HostSamplePool:
+    """The batch-mode pool in pinned host memory, for maps of more scans than `pc_count_gpu_limit`
+    (dataset/lidar_dataset.py:94-101: the reference then keeps its pools in CPU memory).  Same contract as SamplePool:
+    `append`, `len`, `get_batch(bs, generator=None, ordered=None)`, `ordered = False`.
+
+    Samples are 32-byte records {x, y, z, label, weight, pad x3} in pinned chunks of 2^chunk_shift records (a power of two
+    in bytes, which is what torch's pinned allocator hands out); the pool grows by adding chunks, never by copying.
+    `append` is one launch of `shine_host_pool_append` that packs a frame's device samples straight into the chunks.
+    `get_batch` draws the indices exactly like SamplePool (`torch.randint` on the device, same generator calls), then one
+    launch of `shine_host_pool_gather` reads the drawn records over PCIe: a host pool and a device pool filled with the same
+    frames give bit-identical batches for the same generator state.  The reference instead draws and indexes on the CPU and
+    copies the batch (:431-448); the distribution is the same (uniform, with replacement) and here the draw stays on the
+    device, so `get_batch` has no host synchronisation and can be captured in a CUDA graph (capture it after the last
+    append: a captured batch draws from the pool size at capture time)."""
+
+    RECORD_FLOATS = 8
+    DEFAULT_CHUNK_SHIFT = 22          # 4 Mi records = 128 MiB per chunk
+
+    def __init__(self, device, chunk_shift: int = DEFAULT_CHUNK_SHIFT):
+        if not 5 <= chunk_shift <= 31:
+            raise ValueError("chunk_shift must lie in [5, 31]")
+        self.device = torch.device(device)
+        if self.device.type != "cuda":
+            raise ValueError("HostSamplePool feeds a GPU: device must be a CUDA device")
+        if self.device.index is None:
+            self.device = torch.device("cuda", torch.cuda.current_device())
+        self.chunk_shift = chunk_shift
+        self.size = 0
+        self.ordered = False
+        self.last_index = None        # the indices of the last get_batch (a graph's static tensor when captured)
+        self._chunks: list[torch.Tensor] = []
+        self._table = torch.empty(0, dtype=torch.int64, device=self.device)   # device array of the chunks' addresses
+
+    @property
+    def chunk_records(self) -> int:
+        return 1 << self.chunk_shift
+
+    @property
+    def capacity(self) -> int:
+        return len(self._chunks) << self.chunk_shift
+
+    def __len__(self):
+        return self.size
+
+    def _descriptor(self):
+        from . import _abi
+        return _abi.ShineHostPool(self._table.data_ptr() if self._chunks else None, self.chunk_shift, len(self._chunks),
+                                  self.size)
+
+    def _reserve(self, need: int) -> None:
+        if self.capacity >= need:
+            return
+        while self.capacity < need:
+            self._chunks.append(torch.empty(self.chunk_records * self.RECORD_FLOATS, dtype=torch.float32, pin_memory=True))
+        self._table = torch.tensor([c.data_ptr() for c in self._chunks], dtype=torch.int64, device=self.device)
+
+    def append(self, coord, label, weight):
+        from . import _abi
+        for t in (coord, label, weight):
+            _abi.require_cuda(t, "HostSamplePool.append")
+            if t.device != self.device:
+                raise ValueError(f"HostSamplePool.append: frame on {t.device}, pool fed to {self.device}")
+        coord = coord.to(torch.float32).reshape(-1, 3).contiguous()
+        label = label.to(torch.float32).reshape(-1).contiguous()
+        weight = weight.to(torch.float32).reshape(-1).contiguous()
+        n = coord.shape[0]
+        if label.shape[0] != n or weight.shape[0] != n:
+            raise ValueError("coord, label and weight of a frame must have the same number of samples")
+        if n == 0:
+            return self
+        self._reserve(self.size + n)
+        desc = self._descriptor()
+        _abi.check(_abi.lib().shine_host_pool_append(C.byref(desc), self.size, _abi.ptr(coord), _abi.ptr(label),
+                                                     _abi.ptr(weight), n, _abi.stream_ptr(self.device)),
+                   "shine_host_pool_append")
+        self.size += n
+        return self
+
+    def gather(self, index: torch.Tensor):
+        """-> coord [n,3], sdf_label [n], weight [n] on the device: the samples at `index` (int64 device tensor)."""
+        from . import _abi
+        _abi.require_cuda(index, "HostSamplePool.gather")
+        index = index.to(torch.int64).reshape(-1).contiguous()
+        n = index.shape[0]
+        coord = torch.empty(n, 3, device=self.device)
+        label = torch.empty(n, device=self.device)
+        weight = torch.empty(n, device=self.device)
+        if n:
+            desc = self._descriptor()
+            _abi.check(_abi.lib().shine_host_pool_gather(C.byref(desc), _abi.ptr(index), n, _abi.ptr(coord),
+                                                         _abi.ptr(label), _abi.ptr(weight),
+                                                         _abi.stream_ptr(self.device)), "shine_host_pool_gather")
+        return coord, label, weight
+
+    def get_batch(self, bs: int, generator: torch.Generator | None = None, ordered: bool | None = None):
+        """ordered: None or False = the order drawn; True raises (the host pool is never in Morton order)."""
+        if ordered:
+            raise ValueError("HostSamplePool hands batches out in the order drawn; it has no Morton order")
+        if self.size == 0:
+            raise ValueError("get_batch on an empty HostSamplePool")
+        index = torch.randint(0, self.size, (bs,), device=self.device, generator=generator)
+        self.last_index = index
+        return self.gather(index)
+
+    def sort_morton(self, level: int = 16, octree=None):
+        raise NotImplementedError("HostSamplePool keeps the samples in the order appended")
+
+
+def use_host_pool(config: SHINEConfig, n_frames: int) -> bool:
+    """The reference's rule for the pool's place in batch mode (dataset/lidar_dataset.py:94): pinned host memory iff the
+    run uses more than `pc_count_gpu_limit` scans and neither continual-learning mode is on."""
+    return n_frames > config.pc_count_gpu_limit and not config.continual_learning_reg and not config.window_replay_on
+
+
 def generate_scans(config: SHINEConfig, n_azimuth: int, n_frames: int = 1, frame_step_m: float = 1.0, seed: int = 42,
                    device=None, origin_x0: float = 0.0):
     """Scan the analytic scene from `n_frames` poses along +x and sample every scan like the reference's sampler.
@@ -257,11 +373,18 @@ def generate_scans(config: SHINEConfig, n_azimuth: int, n_frames: int = 1, frame
 
 
 def build_scene_map(config: SHINEConfig, octree, n_azimuth: int, n_frames: int = 1, frame_step_m: float = 1.0,
-                    seed: int = 42, device=None, origin_x0: float = 0.0):
+                    seed: int = 42, device=None, origin_x0: float = 0.0, pool=None):
     """Scan the analytic scene from `n_frames` poses along +x, sample every scan, grow the octree from the
-    surface samples (weight > 0; dataset/lidar_dataset.py:212-218) and return the SamplePool."""
+    surface samples (weight > 0; dataset/lidar_dataset.py:212-218) and return the pool.
+    pool: None = a new SamplePool; "auto" = a new HostSamplePool if `use_host_pool(config, n_frames)`, else a new
+    SamplePool; or the (Host)SamplePool to fill."""
     device = device or config.device
-    pool = SamplePool(device)
+    if pool is None:
+        pool = SamplePool(device)
+    elif isinstance(pool, str):
+        if pool != "auto":
+            raise ValueError(f"pool must be None, 'auto' or a pool object, not {pool!r}")
+        pool = HostSamplePool(device) if use_host_pool(config, n_frames) else SamplePool(device)
     for coord, label, weight, hits in generate_scans(config, n_azimuth, n_frames, frame_step_m, seed, device, origin_x0):
         if config.octree_from_surface_samples:
             octree.update(coord[weight > 0, :])
