@@ -361,8 +361,8 @@ struct SmemPlan {
     static constexpr int W1 = 0;                       // [32][8]   W1[n][k]
     static constexpr int W1T = W1 + 2 * kH * kF;       // [8][kWS]  W1T[k][n]
     static constexpr int W2 = W1T + 2 * kF * kWS;      // [32][kWS] W2[n][k]
-    static constexpr int W2T = W2 + 2 * kH * kWS;      // [32][kWS] W2T[k][n]
-    static constexpr int B1 = W2T + 2 * kH * kWS;      // [32]
+    static constexpr int W3W2T = W2 + 2 * kH * kWS;    // [32][kWS] w3[n] * W2[n][k] at [k][n] (layer-2 dgrad through the mask)
+    static constexpr int B1 = W3W2T + 2 * kH * kWS;    // [32]
     static constexpr int B2 = B1 + kH;
     static constexpr int W3 = B2 + kH;
     static constexpr int B3 = W3 + kH;                 // [1]
@@ -373,11 +373,13 @@ struct SmemPlan {
                                                        // shared-memory footprint were timed with this size
     static constexpr int STAGE = ZSUM + kZsumFloats;   // per-warp staging of one tile, in mma fragment order (below)
     static constexpr int SB2 = 0;                      // h1:  B fragments of dW2, [k-step 2][n-tile 4][32 lanes][2]
+    static constexpr int SU = SB2;                     // GROUPED: h1 as A fragments of T = (dp h1)^T M2 (rows = layer-1
+                                                       // units, k = points), [k-step 2][m-tile 2][32 lanes][4]
     static constexpr int SA1 = SB2 + kTile * kH;       // dh1: A fragments of dW1, [k-step 2][m-tile 2][32 lanes][4]
     static constexpr int SX = SA1 + kTile * kH;        // feat: B fragments of dW1, [k-step 2][32 lanes][2]
     static constexpr int SA2 = SX + kTile * kF;        // per-point kernels: dh2, A fragments of dW2, [k-step 2][m-tile 2][32 lanes][4]
-    static constexpr int SDP = SA2;                    // GROUPED: [16 points] {dL/dpred, ReLU mask of h2 (bit n)}, from
-                                                       // which the contraction rebuilds dh2
+    static constexpr int SDP = SA2;                    // GROUPED: [16 points] {dL/dpred, ReLU mask of h2 (bit n)}: the
+                                                       // scale of u = dp h1 and the B operand M2 of T
     static constexpr int kStagePerWarp = SA2 + kTile * kH;
     static constexpr int kStageGrouped = SDP + 2 * kTile;
     __host__ __device__ static constexpr int stage_per_warp(bool grouped) { return grouped ? kStageGrouped : kStagePerWarp; }
@@ -536,9 +538,11 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
     }
     for (int i = tid; i < kH * kH; i += blockDim.x) {
         const int nrow = i / kH, k = i % kH;
-        uint32_t hi, lo; split_tf32(P.dec.w2[i], hi, lo);
+        const float w = P.dec.w2[i];
+        uint32_t hi, lo; split_tf32(w, hi, lo);
         smu[SmemPlan::W2 + nrow * kWS + k] = hi; smu[SmemPlan::W2 + kH * kWS + nrow * kWS + k] = lo;
-        smu[SmemPlan::W2T + k * kWS + nrow] = hi; smu[SmemPlan::W2T + kH * kWS + k * kWS + nrow] = lo;
+        split_tf32(__fmul_rn(P.dec.w3[nrow], w), hi, lo);
+        smu[SmemPlan::W3W2T + k * kWS + nrow] = hi; smu[SmemPlan::W3W2T + kH * kWS + k * kWS + nrow] = lo;
     }
     if (tid < kH) {
         smem[SmemPlan::B1 + tid] = P.dec.b1 ? P.dec.b1[tid] : 0.f;
@@ -565,9 +569,10 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
     // Grouped kernel: every warp contracts the tile it has just staged.  Only dW2 does not fit the registers at 2 blocks/SM:
     // it is a per-warp partial in shared memory (SmemPlan::kW2Part), read, updated and written back once per tile.
     //   dW1: dW1[2][4] as in the per-point kernels;
-    //   db1, db2: sums of the A fragments of dW1 / dW2 (rows 16 mt + g, + 8), reduced over the lanes in the epilogue;
+    //   db1: sums of the A fragments of dW1 (rows 16 mt + g, + 8), reduced over the lanes in the epilogue;
+    //   db2 / w3: sums of dp over the B fragments of T (columns 8 nt + g), reduced over the lanes in the epilogue;
     //   dw3: reduced per tile to 1 column per lane (reduce_scatter_g8);  db3: lane sums.
-    float dw3acc = 0.f, db2acc[2][2] = {{0.f, 0.f}, {0.f, 0.f}}, db1acc[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
+    float dw3acc = 0.f, db2acc[4] = {0.f, 0.f, 0.f, 0.f}, db1acc[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
 
     // hash walk: inference reads key + its 4 corner rows as one 32-byte sector per level (every lane probes every level);
     // training uses the level-split walk, because the grouped scatter needs the node slots it resolves
@@ -857,7 +862,7 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
             ax.set(a[0], a[1], a[2], a[3]);
         }
         // operands of the weight-gradient contraction go to this warp's shared-memory staging (fragment order) the moment
-        // they are produced (feat -> SX, h1 -> SB2, dh2 -> SA2, dh1 -> SA1) so that they do not pin registers.
+        // they are produced (feat -> SX, h1 -> SB2 or, grouped, SU, dh2 -> SA2, dh1 -> SA1) so that they do not pin registers.
         // feat (row-half layout): point g + 8 odd is k-slot odd of chunk (4 half + q) * 4 + (g & 3) of k-step kp.
         if (DEC_GRAD) {
 #pragma unroll
@@ -883,12 +888,13 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
                     if (TRAIN && h1[j][r] > 0.f) m1 |= 1u << (4 * j + r);
                     h1[j][r] = fmaxf(h1[j][r], 0.f);
                 }
-                if (DEC_GRAD) {
+                if (DEC_GRAD && !GROUPED) {
 #pragma unroll
                     for (int q = 0; q < 2; ++q)
                         *reinterpret_cast<float2*>(stage + SmemPlan::SB2 + (4 * kp + j) * 64 + 2 * sq[q]) = make_float2(h1[j][q], h1[j][2 + q]);
                 }
             }
+            if (DEC_GRAD && GROUPED) stage_afrags(stage + SmemPlan::SU + 256 * kp, sq, h1);
         }
         float h2[4][4];
         {
@@ -947,21 +953,25 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
         // ---- backward: MLP dgrad on tensor cores ------------------------------------------------------
         const float dpx = __shfl_xor_sync(kFull, dpo, 1);
         const float dp0 = odd ? dpx : dpo, dp8 = odd ? dpo : dpx;
-        float dh2[4][4];
-        float db2t[4][2], db1t[4][2], dw3t[4][2];   // this tile's partials (rows g, g+8)
+        float db1t[4][2], dw3t[4][2];   // this tile's partials (rows g, g+8)
+        if (DEC_GRAD) {
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            dh2[j][0] = h2[j][0] > 0.f ? dp0 * w3a[j] : 0.f; dh2[j][1] = h2[j][1] > 0.f ? dp0 * w3b[j] : 0.f;
-            dh2[j][2] = h2[j][2] > 0.f ? dp8 * w3a[j] : 0.f; dh2[j][3] = h2[j][3] > 0.f ? dp8 * w3b[j] : 0.f;
-            if (DEC_GRAD) {
-                dw3t[j][0] = dp0 * h2[j][0] + dp8 * h2[j][2];  dw3t[j][1] = dp0 * h2[j][1] + dp8 * h2[j][3];
-                db2t[j][0] = dh2[j][0] + dh2[j][2];            db2t[j][1] = dh2[j][1] + dh2[j][3];
-            }
+            for (int j = 0; j < 4; ++j) { dw3t[j][0] = dp0 * h2[j][0] + dp8 * h2[j][2];  dw3t[j][1] = dp0 * h2[j][1] + dp8 * h2[j][3]; }
         }
-        if (DEC_GRAD && !GROUPED) stage_afrags(stage + SmemPlan::SA2 + 256 * kp, sq, dh2);
+        if (DEC_GRAD && !GROUPED) {
+            // dh2 = dL/dpred * w3 where h2 > 0, the A operand of this kernel's dW2 contraction
+            float dh2[4][4];
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                dh2[j][0] = h2[j][0] > 0.f ? dp0 * w3a[j] : 0.f; dh2[j][1] = h2[j][1] > 0.f ? dp0 * w3b[j] : 0.f;
+                dh2[j][2] = h2[j][2] > 0.f ? dp8 * w3a[j] : 0.f; dh2[j][3] = h2[j][3] > 0.f ? dp8 * w3b[j] : 0.f;
+                db2p[j][0] += dh2[j][0] + dh2[j][2]; db2p[j][1] += dh2[j][1] + dh2[j][3];
+            }
+            stage_afrags(stage + SmemPlan::SA2 + 256 * kp, sq, dh2);
+        }
         if (DEC_GRAD && GROUPED) {
-            // dh2 = dL/dpred * w3 where h2 > 0: per point its dL/dpred and the 32-bit ReLU mask of its h2 row are staged
-            // instead of the 512 values of dh2 (the four lanes of equal g hold 8 columns each of rows g and g + 8)
+            // per point its dL/dpred and the 32-bit ReLU mask of its h2 row are staged instead of the 512 values of dh2
+            // (the four lanes of equal g hold 8 columns each of rows g and g + 8)
             uint32_t mg = 0, mg8 = 0;
 #pragma unroll
             for (int j = 0; j < 4; ++j)
@@ -979,24 +989,28 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
         }
         if (DEC_GRAD && t == 0) db3p += dp0 + dp8;
 
+        // dh1 = dp * (M2 W2') with M2 = [h2 > 0] and W2' = diag(w3) W2 (SmemPlan::W3W2T): M2 is exact in tf32, so 3xTF32
+        // takes two products, and each row is scaled by its dL/dpred afterwards
         float dh1[4][4];
         {
 #pragma unroll
             for (int j = 0; j < 4; ++j) { dh1[j][0] = dh1[j][1] = dh1[j][2] = dh1[j][3] = 0.f; }
 #pragma unroll
             for (int kk = 0; kk < 4; ++kk) {
-                AFrag<NTF> a; a.set(dh2[kk][0], dh2[kk][2], dh2[kk][1], dh2[kk][3]);
+                const uint32_t a[4] = {h2[kk][0] > 0.f ? kTf32One : 0u, h2[kk][2] > 0.f ? kTf32One : 0u,
+                                       h2[kk][1] > 0.f ? kTf32One : 0u, h2[kk][3] > 0.f ? kTf32One : 0u};
                 uint2 bh[4], bl[4];
 #pragma unroll
                 for (int j = 0; j < 4; ++j) {
                     const int off = (8 * j + g) * kWS + 8 * kk + 2 * t;
-                    bh[j] = *reinterpret_cast<const uint2*>(smu + SmemPlan::W2T + off);
-                    bl[j] = *reinterpret_cast<const uint2*>(smu + SmemPlan::W2T + kH * kWS + off);
+                    bh[j] = *reinterpret_cast<const uint2*>(smu + SmemPlan::W3W2T + off);
+                    bl[j] = *reinterpret_cast<const uint2*>(smu + SmemPlan::W3W2T + kH * kWS + off);
                 }
-                mma3x4<NTF>(dh1, a, bh, bl);
+                mma2x4_exact_a<NTF>(dh1, a, bh, bl);
             }
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
+                dh1[j][0] *= dp0; dh1[j][1] *= dp0; dh1[j][2] *= dp8; dh1[j][3] *= dp8;
 #pragma unroll
                 for (int r = 0; r < 4; ++r) dh1[j][r] = ((m1 >> (4 * j + r)) & 1u) ? dh1[j][r] : 0.f;
                 if (DEC_GRAD) { db1t[j][0] = dh1[j][0] + dh1[j][2]; db1t[j][1] = dh1[j][1] + dh1[j][3]; }
@@ -1026,7 +1040,6 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
         if (DEC_GRAD && !GROUPED) {       // contraction over the tile's 16 points
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
-                db2p[j][0] += db2t[j][0]; db2p[j][1] += db2t[j][1];
                 db1p[j][0] += db1t[j][0]; db1p[j][1] += db1t[j][1];
                 dw3p[j][0] += dw3t[j][0]; dw3p[j][1] += dw3t[j][1];
             }
@@ -1062,13 +1075,24 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
             for (int j = 0; j < 4; ++j) { cols[2 * j] = dw3t[j][0]; cols[2 * j + 1] = dw3t[j][1]; }
             dw3acc += reduce_scatter_g8(cols, lane);    // column 8 (g >> 1) + 2t + (g & 1)
             __syncwarp();
-            // dW2[n2][k1] += sum_rows dh2[row][n2] * h1[row][k1], one m-tile at a time (16 accumulators); the A fragment
-            // (rows n2 = 16 mt + g, + 8; k-slots = points 4 ks + t, + 8) is rebuilt with the product dp * w3 of the
-            // forward's dh2, so it is bit-identical to it
+            // dW2[n2][k1] = w3[n2] T[k1][n2] with T[k1][n2] = sum_rows u[row][k1] M2[row][n2], u = dp h1, M2 = [h2 > 0];
+            // w3 is applied in the epilogue.  T runs one m-tile at a time (16 accumulators).  A (rows k1 = 16 mt + g, + 8;
+            // k-slots = points 4 ks + t, + 8) is the forward's h1, scaled by the two points' dp as it is loaded; B (same
+            // k-slots, n2 = 8 nt + g) is the 0/1 mask, exact in tf32, so 3xTF32 takes two products
+            float dpk[2][2];
+            uint32_t mk[2][2];   // the points' masks, shifted to column g
+#pragma unroll
+            for (int ks = 0; ks < 2; ++ks) {
+                const float2 e0 = *reinterpret_cast<const float2*>(stage + SmemPlan::SDP + 2 * (4 * ks + t));
+                const float2 e8 = *reinterpret_cast<const float2*>(stage + SmemPlan::SDP + 2 * (4 * ks + t + 8));
+                dpk[ks][0] = e0.x; dpk[ks][1] = e8.x;
+                mk[ks][0] = __float_as_uint(e0.y) >> g; mk[ks][1] = __float_as_uint(e8.y) >> g;
+#pragma unroll
+                for (int nt = 0; nt < 4; ++nt)   // db2[n2] / w3[n2]: the mask's column sums weighted by dp
+                    db2acc[nt] += ((mk[ks][0] >> (8 * nt)) & 1u ? dpk[ks][0] : 0.f) + ((mk[ks][1] >> (8 * nt)) & 1u ? dpk[ks][1] : 0.f);
+            }
 #pragma unroll
             for (int mt = 0; mt < 2; ++mt) {
-                const int n = 16 * mt + g;
-                const float wn = smem[SmemPlan::W3 + n], wn8 = smem[SmemPlan::W3 + n + 8];
                 float acc[4][4];
 #pragma unroll
                 for (int nt = 0; nt < 4; ++nt) {
@@ -1077,18 +1101,16 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
                 }
 #pragma unroll
                 for (int ks = 0; ks < 2; ++ks) {
-                    uint2 bh[4], bl[4];
+                    uint2 b[4];
 #pragma unroll
-                    for (int nt = 0; nt < 4; ++nt) load_bfrag(stage + SmemPlan::SB2 + (4 * ks + nt) * 64, fc, bh[nt], bl[nt]);
-                    const float2 e0 = *reinterpret_cast<const float2*>(stage + SmemPlan::SDP + 2 * (4 * ks + t));
-                    const float2 e8 = *reinterpret_cast<const float2*>(stage + SmemPlan::SDP + 2 * (4 * ks + t + 8));
-                    const uint32_t k0 = __float_as_uint(e0.y), k8 = __float_as_uint(e8.y);
-                    const float ax = (k0 >> n) & 1u ? e0.x * wn : 0.f, ay = (k0 >> (n + 8)) & 1u ? e0.x * wn8 : 0.f;
-                    const float az = (k8 >> n) & 1u ? e8.x * wn : 0.f, aw = (k8 >> (n + 8)) & 1u ? e8.x * wn8 : 0.f;
-                    db2acc[mt][0] += ax + az; db2acc[mt][1] += ay + aw;
+                    for (int nt = 0; nt < 4; ++nt) {
+                        b[nt].x = (mk[ks][0] >> (8 * nt)) & 1u ? kTf32One : 0u;
+                        b[nt].y = (mk[ks][1] >> (8 * nt)) & 1u ? kTf32One : 0u;
+                    }
+                    const float4 v = *reinterpret_cast<const float4*>(stage + SmemPlan::SU + (2 * ks + mt) * 128 + 4 * fc);
                     AFrag<NTF> af;
-                    af.set_packed(ax, ay, az, aw);
-                    mma3x4<NTF>(acc, af, bh, bl);
+                    af.set_packed(v.x * dpk[ks][0], v.y * dpk[ks][0], v.z * dpk[ks][1], v.w * dpk[ks][1]);
+                    mma2x4_exact_b<NTF>(acc, af, b);
                 }
 #pragma unroll
                 for (int nt = 0; nt < 4; ++nt)
@@ -1173,11 +1195,11 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
             *reinterpret_cast<float2*>(part + (16 * mt + g) * kF + 2 * t) = make_float2(dW1[mt][0], dW1[mt][1]);
             *reinterpret_cast<float2*>(part + (16 * mt + g + 8) * kF + 2 * t) = make_float2(dW1[mt][2], dW1[mt][3]);
 #pragma unroll
-            for (int r = 0; r < 2; ++r) {   // db1 / db2 rows 16 mt + g + 8 r: sums over this lane's k-slots, then over the
-                float d1 = db1acc[mt][r], d2 = db2acc[mt][r];   // 4 lanes of equal g
+            for (int r = 0; r < 2; ++r) {   // db1 rows 16 mt + g + 8 r / db2 columns 8 (2 mt + r) + g: sums over this lane's
+                float d1 = db1acc[mt][r], d2 = db2acc[2 * mt + r];   // k-slots, then over the 4 lanes of equal g
 #pragma unroll
                 for (int o = 1; o < 4; o <<= 1) { d1 += __shfl_xor_sync(kFull, d1, o); d2 += __shfl_xor_sync(kFull, d2, o); }
-                if (t == 0) { part[oB1 + 16 * mt + g + 8 * r] = d1; part[oB2 + 16 * mt + g + 8 * r] = d2; }
+                if (t == 0) { part[oB1 + 16 * mt + g + 8 * r] = d1; part[oB2 + 8 * (2 * mt + r) + g] = d2; }
             }
         }
         part[oW3 + 8 * (g >> 1) + 2 * t + (g & 1)] = dw3acc;
@@ -1193,14 +1215,16 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
                 for (int w = 0; w < kWarps; ++w) v += smem[SmemPlan::STAGE + w * kStage + i];
                 if (i < oB1) dst = P.dec.gw1 + i;
                 else if (i < oB2) dst = P.dec.gb1 ? P.dec.gb1 + (i - oB1) : nullptr;
-                else if (i < oW3) dst = P.dec.gb2 ? P.dec.gb2 + (i - oB2) : nullptr;
+                else if (i < oW3) { v *= smem[SmemPlan::W3 + (i - oB2)]; dst = P.dec.gb2 ? P.dec.gb2 + (i - oB2) : nullptr; }
                 else if (i < oB3) dst = P.dec.gw3 + (i - oW3);
                 else dst = P.dec.gb3;
-            } else {   // dW2[r][c]: fragment (r >> 4, c >> 3), lane 4 (r & 7) + ((c & 7) >> 1), register 2 ((r >> 3) & 1) + (c & 1)
+            } else {   // dW2[r][c] = w3[r] T[c][r]: fragment (c >> 4, r >> 3), lane 4 (c & 7) + ((r & 7) >> 1), register
+                       // 2 ((c >> 3) & 1) + (r & 1)
                 const int e = i - kVec, r = e / kH, c = e % kH;
-                const int f = 128 * (4 * (r >> 4) + (c >> 3)) + 4 * (4 * (r & 7) + ((c & 7) >> 1)) + 2 * ((r >> 3) & 1) + (c & 1);
+                const int f = 128 * (4 * (c >> 4) + (r >> 3)) + 4 * (4 * (c & 7) + ((r & 7) >> 1)) + 2 * ((c >> 3) & 1) + (r & 1);
 #pragma unroll
                 for (int w = 0; w < kWarps; ++w) v += w2p[(w - warp) * SmemPlan::kW2Part + f];
+                v *= smem[SmemPlan::W3 + r];
                 dst = P.dec.gw2 + e;
             }
             if (v != 0.f && dst) atomicAdd(dst, v);

@@ -363,6 +363,29 @@ __device__ __forceinline__ void mma3x2(float (&d0)[4], float (&d1)[4], const AFr
     }
     mma_tf32(d0, a0.hi, bh0.x, bh0.y); mma_tf32(d1, a1.hi, bh1.x, bh1.y);
 }
+// The same for an operand that is exact in tf32 (a 0/1 ReLU mask): its lo word is zero, so 3xTF32 takes two products.
+// 1.0f as an mma operand word
+constexpr uint32_t kTf32One = 0x3f800000u;
+// exact A (one word per element), four accumulators: D[j] += A Bh[j] + A Bl[j]
+template <int NTF>
+__device__ __forceinline__ void mma2x4_exact_a(float (&d)[4][4], const uint32_t (&a)[4], const uint2 (&bh)[4], const uint2 (&bl)[4]) {
+    if (NTF == 3) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) mma_tf32(d[j], a, bl[j].x, bl[j].y);
+    }
+#pragma unroll
+    for (int j = 0; j < 4; ++j) mma_tf32(d[j], a, bh[j].x, bh[j].y);
+}
+// exact B, four accumulators sharing one A fragment: D[j] += Al B[j] + Ah B[j]
+template <int NTF>
+__device__ __forceinline__ void mma2x4_exact_b(float (&d)[4][4], const AFrag<NTF>& a, const uint2 (&b)[4]) {
+    if (NTF == 3) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) mma_tf32(d[j], a.lo, b[j].x, b[j].y);
+    }
+#pragma unroll
+    for (int j = 0; j < 4; ++j) mma_tf32(d[j], a.hi, b[j].x, b[j].y);
+}
 
 // ------------------------------------------------------------------------------------------------------
 // wgmma (sm_90a warpgroup MMA, kind tf32, fp32 accumulate) with shared-memory descriptors, mbarrier wait
