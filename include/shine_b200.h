@@ -295,6 +295,42 @@ int shine_pool_window_append(const shine_sample_pool* pool, const float* coord, 
                              int64_t n_new, float ox, float oy, float oz, float radius, int64_t* size_out, void* scratch,
                              int64_t scratch_bytes, void* stream);
 
+/* ---- one LiDAR frame from its file's records to training samples ---------------------------------------------------
+ * Replaces dataset/lidar_dataset.py:115-218 (process_frame: preprocess_kitti :334-339, open3d crop :139-142, voxel
+ * down-sampling :158, transform :179 and scale :189) and utils/data_sampler.py:18-139 (dataSampler.sample).
+ * Records are the file's bytes as read: n records of stride_bytes, x y z first, float32 (fp64 = 0) or float64 (fp64 = 1).
+ * The four calls run in order on one scratch (>= shine_scan_scratch_bytes(n), 256-byte aligned, device memory) and the
+ * same records; only the voxel count has to reach the host between the second and the third. */
+typedef struct shine_scan_input {
+    const void* records;    /* device [n * stride_bytes] */
+    int64_t n;
+    int32_t stride_bytes;
+    int32_t fp64;
+} shine_scan_input;
+
+int64_t shine_scan_scratch_bytes(int64_t n);
+/* Keeps, in fp64, z > min_z, sqrt((x*x + y*y) + z*z) >= min_range and -r <= x, y <= r, min_z <= z <= max_z (NaN and inf
+ * points fail); takes the per-axis bounds of the kept points and their voxel keys floor((p - (min - v/2)) / v), 21 bits
+ * per axis.  A crop box wider than 2^21 - 2 voxels on an axis is SHINE_ERR_INVALID_ARG. */
+int shine_scan_filter_keys(const shine_scan_input* in, double min_z, double max_z, double min_range, double pc_radius,
+                           double voxel, void* scratch, int64_t scratch_bytes, void* stream);
+/* Stable radix sort of (key, input index); the number of voxels goes to the device int64 *voxel_count. */
+int shine_scan_sort_voxels(int64_t n, int64_t* voxel_count, void* scratch, int64_t scratch_bytes, void* stream);
+/* Voxel i (ascending key) = fp64 sum of its points in input order / their count -> voxels_out[i] (nullable, [n_voxels,3]
+ * fp64); then q = pose·[p,1] (row-major 4x4, host memory; rows ((m0*x + m1*y) + m2*z) + m3, no FMA), q.xyz / q.w, times
+ * scale, rounded to nearest fp32 -> points_out [n_voxels,3]. */
+int shine_scan_average_transform(const shine_scan_input* in, const double* pose, double scale, int64_t n_voxels,
+                                 double* voxels_out, float* points_out, void* scratch, int64_t scratch_bytes,
+                                 void* stream);
+/* dataSampler.sample in fp32 without contraction, for n_rays points and the sensor origin (ox, oy, oz).  Uniforms are
+ * sample-major like the reference's torch.rand(R*n, 1): u_surface[s*R + i] is surface sample s of ray i.
+ * Per ray i, output rows i*(surface_n + free_n) + s: surface samples then free-space samples; coord = shift*ratio + o,
+ * label = displacement, weight = +1 (surface) / -1 (free).  surface_range, free_end: the fp32 values of
+ * surface_sample_range_m * scale and free_sample_end_dist_m * scale. */
+int shine_scan_sample(const float* points, int64_t n_rays, float ox, float oy, float oz, const float* u_surface,
+                      int32_t surface_n, const float* u_free, int32_t free_n, float surface_range, float free_end,
+                      float free_begin_ratio, float* coord, float* label, float* weight, void* stream);
+
 /* ---- the batch-mode sample pool in pinned host memory (more than `pc_count_gpu_limit` scans) ------------------------
  * Replaces the CPU pools of dataset/lidar_dataset.py:94-101 and the CPU-side gather + copy of get_batch (:431-448).
  * Record i is 32 bytes, 32-byte aligned, {x, y, z, label, weight, 0, 0, 0} fp32, at byte (i & (2^chunk_shift - 1)) * 32 of

@@ -101,6 +101,10 @@ class ShineHostPool(C.Structure):
     _fields_ = [("chunks", C.c_void_p), ("chunk_shift", C.c_int32), ("num_chunks", C.c_int32), ("size", C.c_int64)]
 
 
+class ShineScanInput(C.Structure):
+    _fields_ = [("records", C.c_void_p), ("n", C.c_int64), ("stride_bytes", C.c_int32), ("fp64", C.c_int32)]
+
+
 # name -> (restype, argtypes); every symbol declared in include/shine_b200.h
 _vp, _i64, _i32, _u32, _f32 = C.c_void_p, C.c_int64, C.c_int32, C.c_uint32, C.c_float
 _OCT, _DEC = C.POINTER(ShineOctree), C.POINTER(ShineDecoder)
@@ -150,6 +154,14 @@ SYMBOLS = {
                                            _vp, _i64, _vp]),
     "shine_host_pool_append": (C.c_int, [C.POINTER(ShineHostPool), _i64, _vp, _vp, _vp, _i64, _vp]),
     "shine_host_pool_gather": (C.c_int, [C.POINTER(ShineHostPool), _vp, _i64, _vp, _vp, _vp, _vp]),
+    "shine_scan_scratch_bytes": (C.c_int64, [_i64]),
+    "shine_scan_filter_keys": (C.c_int, [C.POINTER(ShineScanInput), C.c_double, C.c_double, C.c_double, C.c_double,
+                                         C.c_double, _vp, _i64, _vp]),
+    "shine_scan_sort_voxels": (C.c_int, [_i64, _vp, _vp, _i64, _vp]),
+    "shine_scan_average_transform": (C.c_int, [C.POINTER(ShineScanInput), C.POINTER(C.c_double), C.c_double, _i64, _vp,
+                                               _vp, _vp, _i64, _vp]),
+    "shine_scan_sample": (C.c_int, [_vp, _i64, _f32, _f32, _f32, _vp, _i32, _vp, _i32, _f32, _f32, _f32, _vp, _vp, _vp,
+                                    _vp]),
 }
 
 _lib = None

@@ -174,14 +174,24 @@ def main(argv=None):
     ap.add_argument("--synthetic-azimuth", type=int, default=2048)
     ap.add_argument("--frames", type=int, default=10)
     ap.add_argument("--iters", type=int, default=None)
+    ap.add_argument("--scans", action="store_true",
+                    help="map the sequence of the config's pc_path / pose_path / calib_path instead of synthetic scans")
     args = ap.parse_args(argv)
     config = SHINEConfig()
     config.load(args.config)
     torch.manual_seed(config.seed)
     octree, decoder = FeatureOctree(config), Decoder(config)
-    print("Load, preprocess and sample data (synthetic scans)")
-    # more than pc_count_gpu_limit scans: the pool lives in pinned host memory (dataset/lidar_dataset.py:94-101)
-    pool = synth.build_scene_map(config, octree, args.synthetic_azimuth, args.frames, seed=config.seed, pool="auto")
+    if args.scans:
+        from .scans import LiDARDataset
+        print(f"Load, preprocess and sample data ({config.pc_path})")
+        dataset = LiDARDataset(config, octree)                                      # shine_batch.py:58-76
+        for frame_id in dataset.used_frames:
+            dataset.process_frame(frame_id)
+        pool = dataset.pool
+    else:
+        print("Load, preprocess and sample data (synthetic scans)")
+        # more than pc_count_gpu_limit scans: the pool lives in pinned host memory (dataset/lidar_dataset.py:94-101)
+        pool = synth.build_scene_map(config, octree, args.synthetic_azimuth, args.frames, seed=config.seed, pool="auto")
     where = "pinned host memory" if isinstance(pool, synth.HostSamplePool) else "device memory"
     print(f"Sample pool: {type(pool).__name__} in {where}, {len(pool)} samples")
     octree.print_detail()

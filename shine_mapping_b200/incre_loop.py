@@ -198,6 +198,8 @@ def main(argv=None):
     ap.add_argument("--frames", type=int, default=10)
     ap.add_argument("--frame-step-m", type=float, default=2.0)
     ap.add_argument("--iters", type=int, default=None)
+    ap.add_argument("--scans", action="store_true",
+                    help="map the sequence of the config's pc_path / pose_path / calib_path instead of the synthetic drive")
     args = ap.parse_args(argv)
     config = SHINEConfig()
     config.load(args.config)
@@ -207,10 +209,14 @@ def main(argv=None):
     dev = config.device
     # shine_incre.py:106: the regularisation mode keeps the current frame's samples only, the other mode replays
     pool = None if config.continual_learning_reg else synth.ReplayPool(dev)
-    scans = synth.generate_scans(config, args.synthetic_azimuth, args.frames, args.frame_step_m, seed=config.seed,
-                                 device=dev)
-    frames = [(coord, label, weight, torch.tensor([f * args.frame_step_m, 0.0, 0.0]) * config.scale)
-              for f, (coord, label, weight, _) in enumerate(scans)]
+    if args.scans:
+        from .scans import LiDARDataset
+        frames = LiDARDataset(config).frames()            # read and sampled one frame at a time, as the loop asks
+    else:
+        scans = synth.generate_scans(config, args.synthetic_azimuth, args.frames, args.frame_step_m, seed=config.seed,
+                                     device=dev)
+        frames = [(coord, label, weight, torch.tensor([f * args.frame_step_m, 0.0, 0.0]) * config.scale)
+                  for f, (coord, label, weight, _) in enumerate(scans)]
     print("Begin mapping:", "replay" + (f" (window {config.window_radius} m)" if config.window_replay_on else "")
           if pool is not None else "regularisation")
     history = run_shine_mapping_incremental(config, octree, decoder, frames, iters=args.iters, log=print, pool=pool)
