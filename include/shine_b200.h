@@ -30,7 +30,7 @@
 extern "C" {
 #endif
 
-#define SHINE_ABI_VERSION 3
+#define SHINE_ABI_VERSION 4
 #define SHINE_MAX_LEVELS 8
 #define SHINE_HASH_SLOT_BYTES 64
 
@@ -38,13 +38,11 @@ extern "C" {
 #define SHINE_ERR_INVALID_ARG (-1)
 #define SHINE_ERR_UNSUPPORTED (-2)
 
-/* flags of shine_sdf_* calls */
+/* flags of shine_sdf_* calls; shine_sdf_infer, shine_sdf_bce_fwd and shine_sdf_bce_step return SHINE_ERR_UNSUPPORTED
+ * for any other bit (ABI version 3 also defined bit 8) */
 #define SHINE_FLAG_REDUCTION_SUM 1u   /* loss_reduction == "sum" (shine_incre.py:77-78); default mean   */
 #define SHINE_FLAG_WEIGHTED 2u        /* loss_weight_on (utils/loss.py:18-19): per-sample weight applied */
 #define SHINE_FLAG_TF32X1 4u          /* decoder contractions in plain TF32 (default: 3xTF32 ~ fp32)     */
-#define SHINE_FLAG_TCGEN05 8u         /* shine_sdf_infer / shine_sdf_bce_step: decoder on warpgroup MMAs (wgmma)
-                                         (128-point tiles, warp-specialised gather / epilogue warps) instead of
-                                         warp-level mma.sync                                                  */
 #define SHINE_FLAG_MORTON_ORDERED 16u  /* shine_sdf_bce_step: the batch is in Morton order of its coordinates (the order the
                                          Morton-sorted sample pool hands batches out in).  A hint, never a requirement:
                                          neighbouring points then share nodes, and the step sums the gradients of each run of

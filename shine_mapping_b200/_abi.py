@@ -13,14 +13,13 @@ import torch
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("SHINE_B200_LIB") or os.path.join(_HERE, "csrc", "libshine_b200.so")
 
-ABI_VERSION = 3
+ABI_VERSION = 4
 MAX_LEVELS = 8
 HASH_SLOT_BYTES = 64
 ADAM_MAX_TENSORS = 16
 FLAG_REDUCTION_SUM = 1
 FLAG_WEIGHTED = 2
 FLAG_TF32X1 = 4
-FLAG_TCGEN05 = 8
 FLAG_MORTON_ORDERED = 16
 
 

@@ -1284,218 +1284,6 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
     }
 }
 
-
-// ------------------------------------------------------------------------------------------------------
-// Warpgroup-MMA inference kernel (SHINE_FLAG_TCGEN05): query_feature -> Decoder.sdf with the decoder on wgmma.
-// Two threads per point walk the hash, gather the 8 x L rows and blend all 8 channels; the block's 128 feature vectors
-// become the A operand (M = 128 points, two m64 instructions) of
-//     D1[128x32] = X[128x8] * W1^T      (wgmma kind tf32, 3xTF32: hi*hi + lo*hi + hi*lo)
-//     D2[128x32] = relu(D1+b1)[128x32] * W2^T
-// with operands in shared memory (canonical K-major, no swizzle: 8-row x 16-byte core matrices, LBO = 128 B between
-// the two K-chunks of one MMA, SBO = stride of an 8-row group) and the accumulators in registers (mma.sync C-fragment
-// layout); bias / ReLU / the 32->1 output layer work on the fragments, a row's dot product is summed over its lane quad.
-// ------------------------------------------------------------------------------------------------------
-
-struct TcPlan {                                   // byte offsets in dynamic shared memory
-    static constexpr int A2H = 0;                 // H1  hi  [16 groups][8 chunks][8 rows][16 B]   = 16 KB
-    static constexpr int A2L = A2H + 16384;
-    static constexpr int A1H = A2H;               // X   hi  [16 groups][2 chunks][8 rows][16 B]   = 4 KB; aliases the
-    static constexpr int A1L = A2H + 4096;        //     H1 tile: X is dead once layer 1's MMAs have completed
-    static constexpr int W1H = A2L + 16384;       // W1  hi  [4 groups][2 chunks][8][16 B]         = 1 KB
-    static constexpr int W1L = W1H + 1024;
-    static constexpr int W2H = W1L + 1024;        // W2  hi  [4 groups][8 chunks][8][16 B]         = 4 KB
-    static constexpr int W2L = W2H + 4096;
-    static constexpr int VEC = W2L + 4096;        // b1[32] b2[32] w3[32] b3 (floats)
-    static constexpr int BYTES = VEC + 100 * 4;
-};
-
-template <int LMAX>
-__global__ void __launch_bounds__(128, 5) sdf_infer_tc_kernel(const __grid_constant__ StepParams P) {
-    extern __shared__ __align__(128) unsigned char tsm[];
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const uint32_t sbase = (uint32_t)__cvta_generic_to_shared(tsm);
-    float* vec = reinterpret_cast<float*>(tsm + TcPlan::VEC);
-
-    // ---- prologue: weights (hi/lo) into the canonical K-major layout ---------------------------------------
-    for (int i = tid; i < kH * kF; i += 128) {
-        const int n = i / kF, k = i % kF;
-        uint32_t hi, lo; split_tf32(P.dec.w1[i], hi, lo);
-        const int off = (n >> 3) * 256 + (k >> 2) * 128 + (n & 7) * 16 + (k & 3) * 4;
-        *reinterpret_cast<uint32_t*>(tsm + TcPlan::W1H + off) = hi;
-        *reinterpret_cast<uint32_t*>(tsm + TcPlan::W1L + off) = lo;
-    }
-    for (int i = tid; i < kH * kH; i += 128) {
-        const int n = i / kH, k = i % kH;
-        uint32_t hi, lo; split_tf32(P.dec.w2[i], hi, lo);
-        const int off = (n >> 3) * 1024 + (k >> 2) * 128 + (n & 7) * 16 + (k & 3) * 4;
-        *reinterpret_cast<uint32_t*>(tsm + TcPlan::W2H + off) = hi;
-        *reinterpret_cast<uint32_t*>(tsm + TcPlan::W2L + off) = lo;
-    }
-    if (tid < kH) {
-        vec[tid] = P.dec.b1 ? P.dec.b1[tid] : 0.f;
-        vec[32 + tid] = P.dec.b2 ? P.dec.b2[tid] : 0.f;
-        vec[64 + tid] = P.dec.w3[tid];
-    }
-    if (tid == 0) vec[96] = P.dec.b3 ? P.dec.b3[0] : 0.f;
-    __syncthreads();
-
-    const bool poly = P.oct.poly_interp != 0;
-    const int L = P.oct.num_levels;
-    bool consecutive = true;
-#pragma unroll
-    for (int i = 1; i < LMAX; ++i)
-        if (i < L && P.oct.lv[i].level != P.oct.lv[0].level - i) consecutive = false;
-    const int g = lane >> 2, t = lane & 3;                                // accumulator fragment: rows g, g+8; cols 2t, 2t+1
-    const int num_tiles = (int)((P.n + 127) / 128);
-
-    const int half = tid & 1;                                              // gather: two adjacent lanes per point
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        // ---- hash walk + gather + blend with two lanes per point (levels split for probing, corners split by z bit so
-        //      the pair's row loads of one instruction hit z-neighbour rows = usually one 128-byte line); two passes of
-        //      64 points fill the 128-row A tile ----
-#pragma unroll 1
-        for (int pass = 0; pass < 2; ++pass) {
-            const int row = pass * 64 + (tid >> 1);
-            const int64_t p = (int64_t)tile * 128 + row;
-            const bool valid = p < P.n;
-            float x = 0.f, y = 0.f, z = 0.f;
-            if (valid) { x = __ldg(P.coord + 3 * p); y = __ldg(P.coord + 3 * p + 1); z = __ldg(P.coord + 3 * p + 2); }
-            uint32_t hitmask = 0;
-            float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-            const unsigned long long key0 = valid ? morton_of(x, y, z, P.oct.lv[0].level) : 0ull;
-#pragma unroll
-            for (int g0 = 0; g0 < LMAX; g0 += kGatherGroup) {
-                SlotSector sec[kGatherGroup];
-#pragma unroll
-                for (int j = 0; j < kGatherGroup; ++j) {
-                    const int i = g0 + j;
-                    if (i < L && valid) {
-                        const shine_level& lv = P.oct.lv[i];
-                        const unsigned long long kq = consecutive ? (key0 >> (3 * i)) : morton_of(x, y, z, lv.level);
-                        sec[j] = ldg_sector(reinterpret_cast<const HashSlot*>(lv.hash_slots),
-                                            hash_key(kq) & (lv.hash_capacity - 1), half);
-                    }
-                }
-#pragma unroll
-                for (int j = 0; j < kGatherGroup; ++j) {
-                    const int i = g0 + j;
-                    if (i < L && valid) {
-                        const shine_level& lv = P.oct.lv[i];
-                        const unsigned long long kq = consecutive ? (key0 >> (3 * i)) : morton_of(x, y, z, lv.level);
-                        if (!resolve_sector(reinterpret_cast<const HashSlot*>(lv.hash_slots), lv.hash_capacity - 1, kq, half,
-                                            sec[j]))
-                            continue;
-                        hitmask |= 1u << i;
-                        float q0[8], q1[8], q2[8], q3[8];                            // corners with z bit == half
-                        ldg_row8(lv.features + (int64_t)sec[j].ids[0] * kF, q0);
-                        ldg_row8(lv.features + (int64_t)sec[j].ids[1] * kF, q1);
-                        ldg_row8(lv.features + (int64_t)sec[j].ids[2] * kF, q2);
-                        ldg_row8(lv.features + (int64_t)sec[j].ids[3] * kF, q3);
-                        Blend b; b.init(x, y, z, lv.level, poly);
-                        const float wz = half ? b.tz : b.uz;
-                        const float w0 = __fmul_rn(__fmul_rn(b.ux, b.uy), wz), w1 = __fmul_rn(__fmul_rn(b.ux, b.ty), wz);
-                        const float w2 = __fmul_rn(__fmul_rn(b.tx, b.uy), wz), w3 = __fmul_rn(__fmul_rn(b.tx, b.ty), wz);
-                        blend4(acc, q0, q1, q2, q3, w0, w1, w2, w3);
-                    }
-                }
-            }
-            if (P.mask && valid && half == 0) {
-                bool present = false;
-#pragma unroll
-                for (int i = 0; i < LMAX; ++i) present = (i == P.mask_level) ? (((hitmask >> i) & 1u) != 0) : present;
-                P.mask[p] = (uint8_t)present;
-            }
-            // each lane keeps the 4 channels of its half (= one 16-byte K-chunk of the point's row of the A tile)
-            uint32_t h4[4], l4[4];
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-                const float send = half ? acc[q] : acc[4 + q];
-                const float recv = __shfl_xor_sync(kFull, send, 1);
-                split_fast((half ? acc[4 + q] : acc[q]) + recv, h4[q], l4[q]);
-            }
-            const int off = (row >> 3) * 256 + half * 128 + (row & 7) * 16;
-            *reinterpret_cast<uint4*>(tsm + TcPlan::A1H + off) = make_uint4(h4[0], h4[1], h4[2], h4[3]);
-            *reinterpret_cast<uint4*>(tsm + TcPlan::A1L + off) = make_uint4(l4[0], l4[1], l4[2], l4[3]);
-        }
-        // ---- layer 1 on the tensor core (rows 0..63 and 64..127: SBO 256 B -> 8 groups = 2048 B) -------------------
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        __syncthreads();
-        float d[2][16];
-        wgmma_fence();
-        {
-            const uint64_t bh = wgmma_desc(sbase + TcPlan::W1H, 128, 256), bl = wgmma_desc(sbase + TcPlan::W1L, 128, 256);
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const uint64_t ah = wgmma_desc(sbase + TcPlan::A1H + 2048 * h, 128, 256);
-                const uint64_t al = wgmma_desc(sbase + TcPlan::A1L + 2048 * h, 128, 256);
-                wgmma_n32(d[h], al, bh, 0u);
-                wgmma_n32(d[h], ah, bl, 1u);
-                wgmma_n32(d[h], ah, bh, 1u);
-            }
-        }
-        wgmma_commit();
-        wgmma_wait_all();
-        __syncthreads();                                   // every warp's MMAs are done with X before H1 overwrites it
-
-        // ---- bias + ReLU -> H1 (hi/lo), layer 2 ----------------------------------------------------------------------
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-#pragma unroll
-            for (int rr = 0; rr < 2; ++rr) {
-                const int row = 64 * h + 16 * warp + g + 8 * rr;
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    const int col = 8 * j + 2 * t;
-                    uint32_t h0, h1, l0, l1;
-                    split_fast(fmaxf(d[h][4 * j + 2 * rr] + vec[col], 0.f), h0, l0);
-                    split_fast(fmaxf(d[h][4 * j + 2 * rr + 1] + vec[col + 1], 0.f), h1, l1);
-                    const int off = (row >> 3) * 1024 + (col >> 2) * 128 + (row & 7) * 16 + (col & 3) * 4;
-                    *reinterpret_cast<uint2*>(tsm + TcPlan::A2H + off) = make_uint2(h0, h1);
-                    *reinterpret_cast<uint2*>(tsm + TcPlan::A2L + off) = make_uint2(l0, l1);
-                }
-            }
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        __syncthreads();
-        wgmma_fence();
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk) {
-                const uint64_t ah = wgmma_desc(sbase + TcPlan::A2H + 8192 * h + 256 * kk, 128, 1024);
-                const uint64_t al = wgmma_desc(sbase + TcPlan::A2L + 8192 * h + 256 * kk, 128, 1024);
-                const uint64_t bh = wgmma_desc(sbase + TcPlan::W2H + 256 * kk, 128, 1024);
-                const uint64_t bl = wgmma_desc(sbase + TcPlan::W2L + 256 * kk, 128, 1024);
-                wgmma_n32(d[h], al, bh, kk > 0 ? 1u : 0u);
-                wgmma_n32(d[h], ah, bl, 1u);
-                wgmma_n32(d[h], ah, bh, 1u);
-            }
-        }
-        wgmma_commit();
-        wgmma_wait_all();
-
-        // ---- bias + ReLU + 32 -> 1 output layer: 8 columns per lane, the row's sum over the lane quad -----------------
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-#pragma unroll
-            for (int rr = 0; rr < 2; ++rr) {
-                float pr = 0.f;
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    const int col = 8 * j + 2 * t;
-                    pr = fmaf(fmaxf(d[h][4 * j + 2 * rr] + vec[32 + col], 0.f), vec[64 + col], pr);
-                    pr = fmaf(fmaxf(d[h][4 * j + 2 * rr + 1] + vec[33 + col], 0.f), vec[65 + col], pr);
-                }
-                pr += __shfl_xor_sync(kFull, pr, 1);
-                pr += __shfl_xor_sync(kFull, pr, 2);
-                const int64_t p = (int64_t)tile * 128 + 64 * h + 16 * warp + g + 8 * rr;
-                if (t == 0 && p < P.n) P.pred[p] = pr + vec[96];
-            }
-        }
-        __syncthreads();                                   // H1 has been read by every warp's MMAs before the next gather
-    }
-}
-
 // ------------------------------------------------------------------------------------------------------
 // fold the gradient replicas back: grads[l] += sum_r replicas[l][r]; replicas[l] = 0
 // ------------------------------------------------------------------------------------------------------
@@ -1651,34 +1439,8 @@ int launch_fused(const StepParams& P, uint32_t flags, cudaStream_t st) {
     return small ? launch_fused_t<3, TRAIN, DEC_GRAD, 4>(P, st) : launch_fused_t<3, TRAIN, DEC_GRAD, 8>(P, st);
 }
 
-template <int LMAX>
-int launch_infer_tc_t(const StepParams& P, cudaStream_t st) {
-    auto kern = sdf_infer_tc_kernel<LMAX>;
-    static int per_sm_by_dev[kMaxDevices] = {0};
-    int& per_sm_cached = per_sm_by_dev[current_device()];
-    if (per_sm_cached == 0) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, TcPlan::BYTES);
-        if (e != cudaSuccess) return (int)e;
-        e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-        if (e != cudaSuccess) return (int)e;
-        cudaFuncAttributes fa;
-        e = cudaFuncGetAttributes(&fa, kern);
-        if (e != cudaSuccess) return (int)e;
-        const int by_regs = fa.numRegs > 0 ? 65536 / (fa.numRegs * 128) : 1;
-        const int by_smem = (227 * 1024) / (TcPlan::BYTES + 1024);
-        int q = by_regs < by_smem ? by_regs : by_smem;
-        per_sm_cached = q < 1 ? 1 : q;
-    }
-    const int tiles = (int)((P.n + 127) / 128);
-    int grid = sm_count() * per_sm_cached;
-    if (grid > tiles) grid = tiles;
-    if (grid < 1) grid = 1;
-    kern<<<grid, 128, TcPlan::BYTES, st>>>(P);
-    return (int)cudaGetLastError();
-}
-int launch_infer_tc(const StepParams& P, cudaStream_t st) {
-    return P.oct.num_levels <= 4 ? launch_infer_tc_t<4>(P, st) : launch_infer_tc_t<8>(P, st);
-}
+// the flag bits of the shine_sdf_* calls: any other bit is SHINE_ERR_UNSUPPORTED, never silently ignored
+constexpr uint32_t kSdfFlags = SHINE_FLAG_REDUCTION_SUM | SHINE_FLAG_WEIGHTED | SHINE_FLAG_TF32X1 | SHINE_FLAG_MORTON_ORDERED;
 
 int fill_params(StepParams& P, const shine_octree* oct, const shine_decoder* dec, const float* coord, int64_t n) {
     if (n < 0 || (n > 0 && !coord)) return SHINE_ERR_INVALID_ARG;
@@ -1686,7 +1448,7 @@ int fill_params(StepParams& P, const shine_octree* oct, const shine_decoder* dec
     P.oct = *oct; P.dec = *dec; P.coord = coord; P.n = n;
     P.num_tiles = (int32_t)((n + kTile - 1) / kTile);
     P.label = nullptr; P.weight = nullptr; P.d_loss = nullptr; P.pred = nullptr; P.loss = nullptr; P.mask = nullptr;
-    P.mask_level = 0; P.sigma = 1.f; P.loss_scale = 1.f; P.weighted = 0; P.debug_dx = nullptr;
+    P.mask_level = 0; P.sigma = 1.f; P.loss_scale = 1.f; P.weighted = 0;
     return SHINE_OK;
 }
 
@@ -1834,6 +1596,7 @@ int shine_query_tangent_bwd(const shine_octree* oct, const float* coord, int64_t
 
 int shine_sdf_infer(const shine_octree* oct, const shine_decoder* dec, const float* coord, int64_t n, float* out_pred,
                     uint8_t* out_mask, int32_t mask_level, uint32_t flags, void* stream) {
+    if (flags & ~kSdfFlags) return SHINE_ERR_UNSUPPORTED;
     int rc = check_octree(oct, false);
     if (rc) return rc;
     rc = check_decoder(dec, oct);
@@ -1847,13 +1610,13 @@ int shine_sdf_infer(const shine_octree* oct, const shine_decoder* dec, const flo
     if ((rc = check_same_device(oct, coord))) return rc;
     DeviceGuard guard(oct->lv[0].features);
     P.pred = out_pred; P.mask = out_mask; P.mask_level = mask_level;
-    if (flags & SHINE_FLAG_TCGEN05) return launch_infer_tc(P, (cudaStream_t)stream);
     return launch_fused<false, false>(P, flags, (cudaStream_t)stream);
 }
 
 int shine_sdf_bce_fwd(const shine_octree* oct, const shine_decoder* dec, const float* coord, const float* label,
                       const float* weight, int64_t n, float sigma, float loss_scale, float* out_pred, float* out_loss,
                       uint32_t flags, void* stream) {
+    if (flags & ~kSdfFlags) return SHINE_ERR_UNSUPPORTED;
     int rc = check_octree(oct, false);
     if (rc) return rc;
     rc = check_decoder(dec, oct);
@@ -1875,6 +1638,7 @@ int shine_sdf_bce_fwd(const shine_octree* oct, const shine_decoder* dec, const f
 int shine_sdf_bce_step(const shine_octree* oct, const shine_decoder* dec, const float* coord, const float* label,
                        const float* weight, int64_t n, float sigma, float loss_scale, const float* d_loss,
                        float* out_pred, float* out_loss, uint32_t flags, void* stream) {
+    if (flags & ~kSdfFlags) return SHINE_ERR_UNSUPPORTED;
     int rc = check_octree(oct, true);
     if (rc) return rc;
     rc = check_decoder(dec, oct);
@@ -1892,10 +1656,6 @@ int shine_sdf_bce_step(const shine_octree* oct, const shine_decoder* dec, const 
     DeviceGuard guard(oct->lv[0].features);
     P.label = label; P.weight = weight; P.weighted = (flags & SHINE_FLAG_WEIGHTED) ? 1 : 0;
     P.sigma = sigma; P.loss_scale = loss_scale; P.d_loss = d_loss; P.pred = out_pred; P.loss = out_loss;
-    if ((flags & SHINE_FLAG_TCGEN05) && !(flags & SHINE_FLAG_TF32X1)) {
-        rc = shine_internal::launch_train_tc(P, dec_grad, (cudaStream_t)stream);
-        if (rc != SHINE_ERR_UNSUPPORTED) return rc;      // > 4 levels: the mma.sync kernel below handles it
-    }
     return dec_grad ? launch_fused<true, true>(P, flags, (cudaStream_t)stream)
                     : launch_fused<true, false>(P, flags, (cudaStream_t)stream);
 }

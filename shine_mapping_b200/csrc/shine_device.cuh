@@ -28,11 +28,7 @@ struct StepParams {
     float sigma;
     float loss_scale;
     int32_t weighted;
-    float* debug_dx;         // development aid: dL/dfeature rows [n, 8] of the tcgen05 training kernel (NULL in normal use)
 };
-
-// shine_train_tc.cu: the warp-specialised tcgen05 training kernel (SHINE_FLAG_TCGEN05 on shine_sdf_bce_step)
-int launch_train_tc(const StepParams& P, bool dec_grad, cudaStream_t st);
 
 }  // namespace shine_internal
 
@@ -385,46 +381,6 @@ __device__ __forceinline__ void mma2x4_exact_b(float (&d)[4][4], const AFrag<NTF
     }
 #pragma unroll
     for (int j = 0; j < 4; ++j) mma_tf32(d[j], a.hi, b[j].x, b[j].y);
-}
-
-// ------------------------------------------------------------------------------------------------------
-// wgmma (sm_90a warpgroup MMA, kind tf32, fp32 accumulate) with shared-memory descriptors, mbarrier wait
-// ------------------------------------------------------------------------------------------------------
-// Operand layout: K-major without swizzle, core matrices of 8 rows x 16 bytes; LBO = byte distance of the two core
-// matrices that make up the K = 8 of one instruction, SBO = byte distance of consecutive 8-row groups.
-__device__ __forceinline__ uint64_t wgmma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    return (uint64_t)((smem_addr >> 4) & 0x3FFF) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) |
-           ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32);                     // base offset 0, no swizzle
-}
-__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
-// D[64 x 32] (+)= A[64 x 8] B[32 x 8]^T.  Accumulator fragment of thread (warp w, lane l) of the warpgroup: d[4j + r] is row
-// 16w + l/4 + 8(r >> 1), column 8j + 2(l % 4) + (r & 1) — four m16n8 C fragments side by side.
-__device__ __forceinline__ void wgmma_n32(float (&d)[16], uint64_t a, uint64_t b, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1;\n\t}\n"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-        : "l"(a), "l"(b), "r"(accumulate));
-}
-// D[64 x 8] (+)= A[64 x 8] B[8 x 8]^T (one m16n8 C fragment per warp)
-__device__ __forceinline__ void wgmma_n8(float (&d)[4], uint64_t a, uint64_t b, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %6, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n8k8.f32.tf32.tf32 {%0,%1,%2,%3}, %4, %5, p, 1, 1;\n\t}\n"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-        : "l"(a), "l"(b), "r"(accumulate));
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-    uint32_t done = 0;
-    for (int spin = 0; !done; ++spin) {
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}\n"
-                     : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-        if (spin > (1 << 22)) __trap();   // never hang the GPU on a protocol bug
-    }
 }
 
 // ------------------------------------------------------------------------------------------------------

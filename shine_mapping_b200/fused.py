@@ -139,7 +139,7 @@ def sdf_bce_step(octree: FeatureOctree, decoder: Decoder, coord, sdf_label, sigm
 
 
 @torch.no_grad()
-def sdf_infer(octree: FeatureOctree, decoder: Decoder, coord, mask_level=None, tf32x1=False, tcgen05=False):
+def sdf_infer(octree: FeatureOctree, decoder: Decoder, coord, mask_level=None, tf32x1=False):
     """decoder.sdf(octree.query_feature(coord)) in one kernel, forward only (the mesher's query, reference
     utils/mesher.py:60-72).  With mask_level (index into hierarchical_indices, 0 = leaf) also returns the
     validity mask the mesher derives from hierarchical_indices[level] >= 0 (utils/mesher.py:82-89)."""
@@ -151,7 +151,7 @@ def sdf_infer(octree: FeatureOctree, decoder: Decoder, coord, mask_level=None, t
     dd = decoder.c_descriptor(None)
     _abi.check(_abi.lib().shine_sdf_infer(C.byref(od), C.byref(dd), _abi.ptr(coord), n, _abi.ptr(pred),
                                           _abi.ptr(mask), int(mask_level or 0),
-                                          (_abi.FLAG_TF32X1 if tf32x1 else 0) | (_abi.FLAG_TCGEN05 if tcgen05 else 0),
+                                          _abi.FLAG_TF32X1 if tf32x1 else 0,
                                           _abi.stream_ptr(coord.device)),
                "shine_sdf_infer")
     return (pred, mask.bool()) if mask is not None else pred

@@ -28,7 +28,7 @@ def _align4(n: int) -> int:
 
 class SdfTrainer:
     def __init__(self, config: SHINEConfig, octree: FeatureOctree, decoder: Decoder, process_group=None,
-                 tf32x1: bool = False, shard_mode: str = "replicated", boundary=None, comm=None, tcgen05=None, p2p=None,
+                 tf32x1: bool = False, shard_mode: str = "replicated", boundary=None, comm=None, p2p=None,
                  morton_ordered: bool = False):
         """shard_mode (multi-GPU, see dist.py / partition.py): "replicated" = every rank holds the whole table and a
         slice of the point batch -> all-reduce the whole flat gradient; "spatial" = every rank owns a Morton-prefix
@@ -47,8 +47,6 @@ class SdfTrainer:
         self.group = process_group
         self.morton_ordered = bool(morton_ordered)   # default for every step: batches come from a Morton-sorted SamplePool
         self.tf32x1 = tf32x1
-        # decoder of the fused step on wgmma, warp-specialised (csrc/shine_train_tc.cu); None = the library default
-        self.tcgen05 = (os.environ.get("SHINE_TRAIN_TCGEN05", "0") == "1") if tcgen05 is None else bool(tcgen05)
         self.lr = config.lr
         self.step_count = 0
         self._sig = None
@@ -131,7 +129,6 @@ class SdfTrainer:
             raise ValueError("loss_weight_on needs the per-sample weight tensor")
         flags = (_abi.FLAG_REDUCTION_SUM if cfg.loss_reduction == "sum" else 0) | \
                 (_abi.FLAG_WEIGHTED if weighted else 0) | (_abi.FLAG_TF32X1 if self.tf32x1 else 0) | \
-                (_abi.FLAG_TCGEN05 if self.tcgen05 else 0) | \
                 (_abi.FLAG_MORTON_ORDERED if (self.morton_ordered if morton_ordered is None else morton_ordered) else 0)
         scale = 1.0 if cfg.loss_reduction == "sum" else 1.0 / float(n_norm if n_norm else n)
         # gradient replicas spread same-row atomics of unordered batches; the grouped scatter of ordered batches issues one

@@ -99,8 +99,9 @@ def sort_case_morton(case, level=12):
 def drop_relu_kink_points(case, eps=2e-6):
     """Remove the (very few) batch points that have a decoder pre-activation within `eps` of zero.  At a ReLU kink two
     fp32-grade implementations that sum in a different order can land on different sides; the gradient of that one point
-    then differs by O(1) although both are right.  Found with the tensor-core (SHINE_FLAG_TCGEN05) kernel on point 31 624 of seed 44 (layer-2
-    pre-activation 6.4e-8); the parity bar is for points where the function is differentiable."""
+    then differs by O(1) although both are right.  Found with the wgmma training kernel (removed after commit 7b3d6fd) on
+    point 31 624 of seed 44 (layer-2 pre-activation 6.4e-8); the parity bar is for points where the function is
+    differentiable."""
     o, dec = oracle_from_case(case)
     with torch.no_grad():
         f = o.query_feature(torch.from_numpy(case["coord"])).double()

@@ -193,22 +193,6 @@ def test_infer_and_mask_match_step_pred():
     assert np.array_equal(mask6.cpu().numpy(), (want6["indices"][5] >= 0).all(1))
 
 
-@pytest.mark.parametrize("levels,n_batch", [(4, 3000), (2, 100), (3, 40000), (6, 3000)])
-def test_tcgen05_infer_matches_oracle(levels, n_batch):
-    """wgmma decoder (SHINE_FLAG_TCGEN05) vs the oracle and vs the mma.sync kernel, incl. the mask."""
-    from shine_mapping_b200 import sdf_infer
-    case = make_case(n_points=2500, n_batch=n_batch, feat_levels=levels, seed=90 + levels)
-    cfg, octree, dec = build_cuda_models(case, DEV)
-    coord = torch.from_numpy(case["coord"]).to(DEV)
-    want = run_oracle_step(case)
-    pred, mask = sdf_infer(octree, dec, coord, mask_level=0, tcgen05=True)
-    torch.cuda.synchronize()
-    assert np.abs(pred.cpu().numpy() - want["pred"]).max() < 2e-5
-    assert np.array_equal(mask.cpu().numpy(), (want["indices"][0] >= 0).all(1))
-    ref = sdf_infer(octree, dec, coord)
-    assert (pred - ref).abs().max() < 1e-5
-
-
 # ---- ekional_loss_on: the fused double-backward kernel (csrc/shine_eikonal.cu) and the class surface ------------------
 # Both are checked at the reference's weight_e = 0.1 (totals, the tolerances of the BCE tests) and, because the step is
 # linear in weight_e, the eikonal term on its own: (gradients at weight_e = W - gradients at weight_e = 0) / W against the
@@ -676,55 +660,9 @@ def test_abi_rejects_bad_arguments():
     assert b"invalid" in lib.shine_error_string(-1)
 
 
-# ---- the warp-specialised wgmma training kernel (csrc/shine_train_tc.cu) ---------------------------------------------------------
-
-def _trainer_step(case, tcgen05, freeze=False):
-    from shine_mapping_b200 import SdfTrainer
-    cfg, octree, dec = build_cuda_models(case, DEV, freeze_decoder=freeze)
-    coord = torch.from_numpy(case["coord"]).to(DEV); label = torch.from_numpy(case["label"]).to(DEV)
-    weight = torch.from_numpy(case["weight"]).to(DEV)
-    tr = SdfTrainer(cfg, octree, dec, tcgen05=tcgen05)
-    tr.zero_grad()
-    pred = torch.empty(coord.shape[0], device=DEV)
-    loss = tr.forward_backward(coord, label, weight, pred_out=pred)
-    torch.cuda.synchronize()
-    return {
-        "indices": [t.cpu().numpy() for t in octree.get_indices(coord)],
-        "feature": octree.query_feature(coord).detach().cpu().numpy(),
-        "pred": pred.cpu().numpy(), "loss": float(loss),
-        "table_grads": [g.detach().cpu().numpy().copy() for g in tr.table_grads],
-        "dec_grads": {} if freeze else {k: g.detach().cpu().numpy().copy() for k, g in zip(DEC_KEYS, tr.dec_grads)
-                                        if g is not None},
-    }
-
-
-@pytest.mark.parametrize("levels,poly,weighted,reduction,n_batch", [
-    (4, True, False, "mean", 3000), (2, True, False, "mean", 100), (3, False, True, "sum", 5000),
-    (4, True, True, "mean", 60000),          # > 132 tiles of 128 points: several rounds per CTA, both gather groups busy
-    (1, True, False, "mean", 0),             # 16 stragglers only: one partial tile
-])
-def test_tcgen05_train_step_matches_oracle(levels, poly, weighted, reduction, n_batch):
-    """SHINE_FLAG_TCGEN05 on shine_sdf_bce_step: decoder forward / dgrad as wgmma on 128-point tiles
-    (operands in shared memory), same tolerances as the mma.sync kernel."""
-    from tests.parity_utils import drop_relu_kink_points
-    case = make_case(n_points=2500, n_batch=n_batch, feat_levels=levels, seed=40 + levels, poly=poly, weighted=weighted,
-                     reduction=reduction, n_frames=2 if n_batch > 10000 else 1)
-    case, dropped = drop_relu_kink_points(case)
-    print("points on a ReLU kink dropped:", dropped, compare_step(_trainer_step(case, True), run_oracle_step(case)))
-
-
-def test_tcgen05_train_step_frozen_decoder():
-    case = make_case(n_points=2500, n_batch=4000, feat_levels=4, seed=47)
-    got = _trainer_step(case, True, freeze=True)
-    want = run_oracle_step(case)
-    want["dec_grads"] = {}
-    print(compare_step(got, want))
-
-
-def test_biasless_decoder_matches_oracle():
+def test_biasless_decoder_matches_oracle_in_every_default_kernel():
     """geo_mlp_bias_on: False — every fused kernel reads the biases through null-pointer branches: the general and the
-    grouped (Morton-ordered) kernels of sdf_bce_step, its two-pass mode, the wgmma training kernel, and both inference
-    kernels."""
+    grouped (Morton-ordered) kernels of sdf_bce_step, its two-pass mode, and the inference kernel."""
     from shine_mapping_b200 import sdf_infer
     from tests.parity_utils import drop_relu_kink_points
     case = make_case(n_points=2500, n_batch=3000, feat_levels=3, seed=57, weighted=True, reduction="sum", bias=False)
@@ -737,14 +675,11 @@ def test_biasless_decoder_matches_oracle():
     print("frozen", compare_step(run_cuda_step(case, DEV, freeze_decoder=True), want_f))
     ordered = sort_case_morton(case)
     print("grouped", compare_step(run_cuda_step(ordered, DEV, morton_ordered=True), run_oracle_step(ordered)))
-    print("wgmma train", compare_step(_trainer_step(case, True), want))
     cfg, octree, dec = build_cuda_models(case, DEV)
     assert all(p is None for p in dec.fused_params()[1::2])
-    coord = torch.from_numpy(case["coord"]).to(DEV)
-    for tc in (False, True):
-        pred = sdf_infer(octree, dec, coord, tcgen05=tc)
-        torch.cuda.synchronize()
-        assert np.abs(pred.cpu().numpy() - want["pred"]).max() < 2e-5, tc
+    pred = sdf_infer(octree, dec, torch.from_numpy(case["coord"]).to(DEV))
+    torch.cuda.synchronize()
+    assert np.abs(pred.cpu().numpy() - want["pred"]).max() < 2e-5
 
 
 def test_two_queries_before_one_backward():

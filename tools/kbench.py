@@ -51,8 +51,6 @@ tr3 = SdfTrainer(cfg, octree, decoder)
 tr1 = SdfTrainer(cfg, octree, decoder, tf32x1=True)
 timeit(lambda: tr3.forward_backward(coord, label), "step 3xTF32 dec_grad")
 timeit(lambda: tr3.forward_backward(coord, label, morton_ordered=True), "step 3xTF32 dec_grad grouped")
-trtc = SdfTrainer(cfg, octree, decoder, tcgen05=True)
-timeit(lambda: trtc.forward_backward(coord, label), "step tcgen05 3xTF32 dec_grad")
 if not args.quick: timeit(lambda: tr1.forward_backward(coord, label), "step 1xTF32 dec_grad")
 for p in decoder.parameters(): p.requires_grad = False
 trf3 = SdfTrainer(cfg, octree, decoder); trf1 = SdfTrainer(cfg, octree, decoder, tf32x1=True)
@@ -62,7 +60,6 @@ timeit(lambda: sdf_infer(octree, decoder, coord), "infer 3xTF32")
 if args.quick: sys.exit(0)
 timeit(lambda: trf1.forward_backward(coord, label), "step 1xTF32 frozen decoder")
 timeit(lambda: sdf_infer(octree, decoder, coord, tf32x1=True), "infer 1xTF32")
-timeit(lambda: sdf_infer(octree, decoder, coord, tcgen05=True), "infer tcgen05 3xTF32")
 feat = torch.empty(n, 8, device=dev); od = octree._descriptor(None, tr3.table_grads, n_points=n)
 lib = _abi.lib(); st = _abi.stream_ptr(dev)
 timeit(lambda: lib.shine_query_fwd(C.byref(od), _abi.ptr(coord), n, _abi.ptr(feat), st), "query_fwd (gather only)")
