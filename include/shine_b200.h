@@ -403,6 +403,53 @@ int shine_p2p_exchange(shine_p2p* ctx, float* dec_grads, int64_t dec_floats, con
 int shine_p2p_timeouts(shine_p2p* ctx, int32_t* out_count);
 int shine_p2p_destroy(shine_p2p* ctx);
 
+/* ---- meshing: utils/mesher.py recon_octree_mesh / recon_bbx_mesh -------------------------------------------------
+ * The grid of the marching cubes is block-sparse: bricks of n^3 cubes at integer brick coordinates B; brick B owns the
+ * grid indices G = B n + (i, j, k), 0 <= i, j, k < n, and stores them together with its +1 faces ((n+1)^3 points, the
+ * corners of all its cubes), so that one chunk of bricks can be queried and meshed without the others.  Grid index G
+ * is the point origin + spacing * G (fp32: __fadd_rn(origin, __fmul_rn(spacing, G))) of the [-1,1] cube.  Grid
+ * indices must lie in [0, 2^20). */
+typedef struct shine_brick_grid {
+    const int32_t* bricks;    /* [num_bricks, 3] brick coordinates of this chunk                                        */
+    float* sdf;               /* [num_bricks, (n+1)^3] fp32, point (i,j,k) at (i (n+1) + j) (n+1) + k                   */
+    uint8_t* mask;            /* same layout                                                                             */
+    const int64_t* all_keys;  /* ascending keys (Bx << 42) | (By << 21) | Bz of every brick of the map, or NULL          */
+    int64_t num_all;
+    int64_t num_bricks;
+    float origin[3];
+    float spacing;
+    int32_t n;                /* cubes per brick side, 1 .. 64                                                           */
+    int32_t lo[3];            /* vertices are written relative to grid index lo                                         */
+    int32_t hi[3];            /* the cube at lowest corner G is processed iff mask[G] and G + 1 < hi on every axis        */
+    float missing_sdf;        /* value of a +1 face point whose brick is not in all_keys (its mask is 0)                */
+} shine_brick_grid;
+
+/* Fills sdf = -Decoder.sdf(query_feature(p)) and mask = voxel present at lv[mask_level] (utils/mesher.py:60-89) at every
+ * point of the chunk, with the same kernel as shine_sdf_infer (flags as there).  With all_keys, +1 face points of bricks
+ * missing from all_keys then get missing_sdf and mask 0 (the zero-initialised global grid of utils/mesher.py:323-324). */
+int shine_mesh_grid(const shine_octree* oct, const shine_decoder* dec, const shine_brick_grid* grid, int32_t mask_level,
+                    uint32_t flags, void* stream);
+
+/* Masked marching cubes (skimage.measure.marching_cubes(sdf, 0, mask=mask, allow_degenerate=False), as used by
+ * utils/mesher.py:216-217) over one chunk of a shine_mesh_grid-filled grid, in two calls per chunk:
+ *   count (verts == NULL): every sign-changing edge (one corner < 0, the other >= 0) of a processed cube is entered in the
+ *     edge table (16-byte slots, memset to 0xFF before the first chunk, kept across the chunks of one mesh) and new
+ *     edges are numbered from counters[0]; counters[1] += the chunk's triangles without two coincident vertices;
+ *     counters[3] counts edges that did not fit (the caller must start over with a larger table).
+ *   emit (verts != NULL, after the host read counters[0..1]): verts[id] = position of the edge's vertex, t = v0 / (v0 - v1)
+ *     along the edge, in grid units relative to lo (fp32 [vert_capacity, 3]); the chunk's triangles (int32 vertex ids,
+ *     [tri_capacity, 3]) go to rows counters[2] onwards, counters[2] advancing. */
+int shine_marching_cubes(const shine_brick_grid* grid, void* edge_slots, uint32_t edge_capacity, int32_t* counters,
+                         float* verts, int64_t vert_capacity, int32_t* tris, int64_t tri_capacity, void* stream);
+
+/* Open3D's compute_vertex_normals and cluster_connected_triangles as used by utils/mesher.py:240-249,278-281:
+ * normals [nv, 3] = normalised sum of the unit normals of the adjacent triangles; keep[t] = 1 iff the cluster of
+ * triangles connected through shared edges that holds t has at least min_tris triangles.  edge_slots: 16-byte slots,
+ * capacity a power of two >= 2 * 3 nt, memset to 0xFF; scratch: int32 [2 nt]. */
+int shine_mesh_clusters(const float* verts, int64_t nv, const int32_t* tris, int64_t nt, int32_t min_tris,
+                        void* edge_slots, uint32_t edge_capacity, int32_t* scratch, uint8_t* keep, float* normals,
+                        void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -5,6 +5,7 @@ from .decoder import Decoder
 from .feature_octree import FeatureOctree
 from .fused import sdf_bce_step, sdf_infer
 from .loss import sdf_bce_loss
+from .mesher import Mesher
 from .trainer import SdfTrainer
 
-__all__ = ["SHINEConfig", "Decoder", "FeatureOctree", "sdf_bce_step", "sdf_infer", "sdf_bce_loss", "SdfTrainer"]
+__all__ = ["SHINEConfig", "Decoder", "FeatureOctree", "sdf_bce_step", "sdf_infer", "sdf_bce_loss", "SdfTrainer", "Mesher"]

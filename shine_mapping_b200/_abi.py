@@ -104,6 +104,12 @@ class ShineScanInput(C.Structure):
     _fields_ = [("records", C.c_void_p), ("n", C.c_int64), ("stride_bytes", C.c_int32), ("fp64", C.c_int32)]
 
 
+class ShineBrickGrid(C.Structure):
+    _fields_ = [("bricks", C.c_void_p), ("sdf", C.c_void_p), ("mask", C.c_void_p), ("all_keys", C.c_void_p),
+                ("num_all", C.c_int64), ("num_bricks", C.c_int64), ("origin", C.c_float * 3), ("spacing", C.c_float),
+                ("n", C.c_int32), ("lo", C.c_int32 * 3), ("hi", C.c_int32 * 3), ("missing_sdf", C.c_float)]
+
+
 # name -> (restype, argtypes); every symbol declared in include/shine_b200.h
 _vp, _i64, _i32, _u32, _f32 = C.c_void_p, C.c_int64, C.c_int32, C.c_uint32, C.c_float
 _OCT, _DEC = C.POINTER(ShineOctree), C.POINTER(ShineDecoder)
@@ -161,6 +167,9 @@ SYMBOLS = {
                                                _vp, _vp, _i64, _vp]),
     "shine_scan_sample": (C.c_int, [_vp, _i64, _f32, _f32, _f32, _vp, _i32, _vp, _i32, _f32, _f32, _f32, _vp, _vp, _vp,
                                     _vp]),
+    "shine_mesh_grid": (C.c_int, [_OCT, _DEC, C.POINTER(ShineBrickGrid), _i32, _u32, _vp]),
+    "shine_marching_cubes": (C.c_int, [C.POINTER(ShineBrickGrid), _vp, _u32, _vp, _vp, _i64, _vp, _i64, _vp]),
+    "shine_mesh_clusters": (C.c_int, [_vp, _i64, _vp, _i64, _i32, _vp, _u32, _vp, _vp, _vp, _vp]),
 }
 
 _lib = None

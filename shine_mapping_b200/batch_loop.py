@@ -20,6 +20,7 @@ import os
 import sys
 import time
 
+import numpy as np
 import torch
 
 from .config import SHINEConfig
@@ -123,9 +124,20 @@ class _GraphedIteration:
 
 def run_shine_mapping_batch(config: SHINEConfig, octree: FeatureOctree, decoder: Decoder, pool, iters=None,
                             log_every: int = 0, run_path: str | None = None, process_group=None,
-                            shard_mode: str = "replicated", use_cuda_graph: bool | None = None):
-    """-> dict(loss_first, loss_last, points_per_s, timing).  `octree` must already hold the map of `pool`."""
+                            shard_mode: str = "replicated", use_cuda_graph: bool | None = None, map_bbx=None,
+                            begin_pose_inv=None):
+    """-> dict(loss_first, loss_last, points_per_s, timing, meshes).  `octree` must already hold the map of `pool`.
+    With run_path, every vis_freq_iters iterations the map is meshed to run_path/mesh/mesh_iter_{it+1}.ply
+    (shine_batch.py:236-245): octree or bbx mode (map_bbx, metres) as mc_with_octree selects, transformed by
+    inv(begin_pose_inv).  `meshes` lists the files written."""
     check_supported(config)
+    mesher = None
+    if run_path:
+        from .mesher import Mesher
+        mesher = Mesher(config, octree, decoder)
+        if begin_pose_inv is not None:
+            mesher.global_transform = np.linalg.inv(begin_pose_inv)
+    meshes = []
     dev = octree.hier_features[0].device
     trainer = SdfTrainer(config, octree, decoder, process_group=process_group, shard_mode=shard_mode)
     world = torch.distributed.get_world_size(process_group) if torch.distributed.is_initialized() else 1
@@ -158,12 +170,17 @@ def run_shine_mapping_batch(config: SHINEConfig, octree: FeatureOctree, decoder:
             losses[it] = float(trainer.loss)          # the only host read-back
         if run_path and ((it + 1) % config.save_freq_iters == 0) and it > 0:
             save_checkpoint(octree, decoder, trainer, run_path, f"model/model_iter_{it + 1}", it)
+        if mesher is not None and ((it + 1) % config.vis_freq_iters == 0) and it > 0:     # between graph replays
+            from .mesher import reconstruct
+            meshes.append(os.path.join(run_path, "mesh", f"mesh_iter_{it + 1}.ply"))
+            reconstruct(config, mesher, meshes[-1], map_bbx)
     torch.cuda.synchronize(dev)
     elapsed = time.perf_counter() - t_begin if t_begin is not None else float("nan")
     done = iters - it_begin if t_begin is not None else 0
     return {"loss_first": losses.get(0), "loss_last": losses.get(iters - 1), "losses": losses,
             "iters_per_s": done / elapsed if done else None,
-            "points_per_s": done * config.bs * world / elapsed if done else None, "timing": timing}
+            "points_per_s": done * config.bs * world / elapsed if done else None, "timing": timing,
+            "meshes": meshes}
 
 
 def main(argv=None):
@@ -176,6 +193,8 @@ def main(argv=None):
     ap.add_argument("--iters", type=int, default=None)
     ap.add_argument("--scans", action="store_true",
                     help="map the sequence of the config's pc_path / pose_path / calib_path instead of synthetic scans")
+    ap.add_argument("--run-path", default=None, metavar="DIR",
+                    help="write checkpoints (model/) and meshes (mesh/mesh_iter_*.ply) under DIR")
     args = ap.parse_args(argv)
     config = SHINEConfig()
     config.load(args.config)
@@ -188,15 +207,18 @@ def main(argv=None):
         for frame_id in dataset.used_frames:
             dataset.process_frame(frame_id)
         pool = dataset.pool
+        map_bbx, begin_pose_inv = dataset.map_bbx, dataset.begin_pose_inv
     else:
         print("Load, preprocess and sample data (synthetic scans)")
         # more than pc_count_gpu_limit scans: the pool lives in pinned host memory (dataset/lidar_dataset.py:94-101)
         pool = synth.build_scene_map(config, octree, args.synthetic_azimuth, args.frames, seed=config.seed, pool="auto")
+        map_bbx, begin_pose_inv = pool.map_bbx, None
     where = "pinned host memory" if isinstance(pool, synth.HostSamplePool) else "device memory"
     print(f"Sample pool: {type(pool).__name__} in {where}, {len(pool)} samples")
     octree.print_detail()
     print("Begin mapping")
-    out = run_shine_mapping_batch(config, octree, decoder, pool, iters=args.iters, log_every=1000)
+    out = run_shine_mapping_batch(config, octree, decoder, pool, iters=args.iters, log_every=1000, run_path=args.run_path,
+                                  map_bbx=map_bbx, begin_pose_inv=begin_pose_inv)
     print({k: v for k, v in out.items() if k != "losses"})
 
 

@@ -19,6 +19,8 @@
 #include <math.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 #include "shine_b200.h"
 
 // tuning constants
@@ -512,9 +514,37 @@ __device__ __forceinline__ void grouped_scatter(const StepParams& P, int L, int 
     __syncwarp();
 }
 
-template <int NTF, bool TRAIN, bool DEC_GRAD, int LMAX, bool GROUPED = false>
-__global__ void __launch_bounds__(256, !TRAIN ? SHINE_INFER_MINB : (DEC_GRAD && !GROUPED) ? SHINE_TRAIN_DECGRAD_MINB : SHINE_TRAIN_MINB)
-sdf_fused_kernel(const __grid_constant__ StepParams P) {
+// Where a point's coordinates come from, and the sign its prediction is stored with.
+struct BatchCoords {        // P.coord [n, 3]
+    __device__ __forceinline__ void load(const StepParams& P, int64_t p, float& x, float& y, float& z) const {
+        x = __ldg(P.coord + 3 * p); y = __ldg(P.coord + 3 * p + 1); z = __ldg(P.coord + 3 * p + 2);
+    }
+    __device__ __forceinline__ float out(float v) const { return v; }
+};
+struct GridCoords {         // the points of a shine_internal::BrickGrid, generated from brick id and index
+    shine_internal::BrickGrid g;
+    __device__ __forceinline__ void load(const StepParams&, int64_t p, float& x, float& y, float& z) const {
+        const int n1 = g.n + 1, per = n1 * n1 * n1;
+        const int64_t b = p / per;
+        const int r = (int)(p - b * per);
+        const int i = r / (n1 * n1), j = (r / n1) % n1, k = r % n1;
+        x = __fadd_rn(g.origin[0], __fmul_rn(g.spacing, (float)(__ldg(g.bricks + 3 * b) * g.n + i)));
+        y = __fadd_rn(g.origin[1], __fmul_rn(g.spacing, (float)(__ldg(g.bricks + 3 * b + 1) * g.n + j)));
+        z = __fadd_rn(g.origin[2], __fmul_rn(g.spacing, (float)(__ldg(g.bricks + 3 * b + 2) * g.n + k)));
+    }
+    __device__ __forceinline__ float out(float v) const { return -v; }
+};
+
+// Minimum resident blocks/SM of the inference kernels.  The mesher's grid points are generated in the kernel (brick id and
+// index from a 64-bit division, the brick origin) and that extra live state spills at SHINE_INFER_MINB's 80-register cap:
+// its instantiations take 2 blocks/SM (128 registers) and do not spill.
+template <class Src>
+constexpr int infer_min_blocks() { return std::is_same<Src, BatchCoords>::value ? SHINE_INFER_MINB : 2; }
+
+template <int NTF, bool TRAIN, bool DEC_GRAD, int LMAX, bool GROUPED = false, class Src = BatchCoords>
+__global__ void __launch_bounds__(256, !TRAIN ? infer_min_blocks<Src>() : (DEC_GRAD && !GROUPED) ? SHINE_TRAIN_DECGRAD_MINB : SHINE_TRAIN_MINB)
+sdf_fused_kernel(const __grid_constant__ StepParams P, const __grid_constant__ Src src) {
+    static_assert(std::is_same<Src, BatchCoords>::value || !TRAIN, "generated coordinates are for inference only");
     static_assert(!GROUPED || TRAIN, "the grouped scatter belongs to the training kernels");
     static_assert(!DEC_GRAD || TRAIN, "decoder gradients belong to the training kernels");
     static_assert(SmemPlan::kStagePerWarp >= SmemPlan::kDecGradFloats, "a warp's staging area holds its partial decoder gradient");
@@ -619,7 +649,7 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
         const int64_t p = (int64_t)tl * kTile + g + 8 * odd;
         nvalid = tl < P.num_tiles && p < P.n;
         if (nvalid) {
-            nx = __ldg(P.coord + 3 * p); ny = __ldg(P.coord + 3 * p + 1); nz = __ldg(P.coord + 3 * p + 2);
+            src.load(P, p, nx, ny, nz);
             if (P.label) nlab = __ldg(P.label + p);
             if (P.weighted) nwgt = fabsf(__ldg(P.weight + p));   // shine_batch.py:172 abs()
         }
@@ -840,7 +870,7 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
             // no point of this tile sees a node on any level: features 0, prediction pred0, no table gradient; the decoder
             // gradients follow by linearity from the sum of dL/dpred (virtual backward tile at the end of the block)
             if (!TRAIN && P.mask && half == 0 && valid) P.mask[myp] = 0;
-            if (P.pred && half == 0 && valid) P.pred[myp] = pred0;
+            if (P.pred && half == 0 && valid) P.pred[myp] = src.out(pred0);
             if (P.label != nullptr && valid) {
                 float li, dpz;
                 bce_point(pred0, lab, wgt, li, dpz);
@@ -936,7 +966,7 @@ sdf_fused_kernel(const __grid_constant__ StepParams P) {
         p0 += b3; p8 += b3;
         const float pown = odd ? p8 : p0;
         if (phase == 0) { pred0 = pown; phase = 1; continue; }     // the virtual forward: every row is Decoder.sdf(0)
-        if (P.pred && half == 0 && valid) P.pred[myp] = pown;
+        if (P.pred && half == 0 && valid) P.pred[myp] = src.out(pown);
 
         if (P.label == nullptr) continue;   // pure inference
 
@@ -1390,9 +1420,9 @@ int check_decoder(const shine_decoder* d, const shine_octree* o) {
     return SHINE_OK;
 }
 
-template <int NTF, bool TRAIN, bool DEC_GRAD, int LMAX, bool GROUPED = false>
-int launch_fused_t(const StepParams& P, cudaStream_t st) {
-    auto kern = sdf_fused_kernel<NTF, TRAIN, DEC_GRAD, LMAX, GROUPED>;
+template <int NTF, bool TRAIN, bool DEC_GRAD, int LMAX, bool GROUPED = false, class Src = BatchCoords>
+int launch_fused_t(const StepParams& P, cudaStream_t st, const Src& src = Src()) {
+    auto kern = sdf_fused_kernel<NTF, TRAIN, DEC_GRAD, LMAX, GROUPED, Src>;
     const int smem_floats = SmemPlan::STAGE + (DEC_GRAD ? 8 * SmemPlan::stage_per_warp(GROUPED) : 0) +
                             (GROUPED ? 8 * (LMAX * SmemPlan::kGroupPerLevel + (DEC_GRAD ? SmemPlan::kW2Part : kTile * kF)) : 0);
     const size_t smem_bytes = (size_t)smem_floats * sizeof(float);
@@ -1424,19 +1454,21 @@ int launch_fused_t(const StepParams& P, cudaStream_t st) {
     int grid = sm_count() * per_sm;
     if (grid > blocks_needed) grid = blocks_needed;
     if (grid < 1) grid = 1;
-    kern<<<grid, 256, smem_bytes, st>>>(P);
+    kern<<<grid, 256, smem_bytes, st>>>(P, src);
     return (int)cudaGetLastError();
 }
 
-template <bool TRAIN, bool DEC_GRAD>
-int launch_fused(const StepParams& P, uint32_t flags, cudaStream_t st) {
+template <bool TRAIN, bool DEC_GRAD, class Src = BatchCoords>
+int launch_fused(const StepParams& P, uint32_t flags, cudaStream_t st, const Src& src = Src()) {
     const bool x1 = (flags & SHINE_FLAG_TF32X1) != 0;
     const bool small = P.oct.num_levels <= 4;
     if constexpr (TRAIN) {      // Morton-ordered batches: voxel-grouped scatter (3xTF32, up to 4 levels; else the general kernel)
         if ((flags & SHINE_FLAG_MORTON_ORDERED) && !x1 && small) return launch_fused_t<3, TRAIN, DEC_GRAD, 4, true>(P, st);
     }
-    if (x1) return small ? launch_fused_t<1, TRAIN, DEC_GRAD, 4>(P, st) : launch_fused_t<1, TRAIN, DEC_GRAD, 8>(P, st);
-    return small ? launch_fused_t<3, TRAIN, DEC_GRAD, 4>(P, st) : launch_fused_t<3, TRAIN, DEC_GRAD, 8>(P, st);
+    if (x1) return small ? launch_fused_t<1, TRAIN, DEC_GRAD, 4, false, Src>(P, st, src)
+                         : launch_fused_t<1, TRAIN, DEC_GRAD, 8, false, Src>(P, st, src);
+    return small ? launch_fused_t<3, TRAIN, DEC_GRAD, 4, false, Src>(P, st, src)
+                 : launch_fused_t<3, TRAIN, DEC_GRAD, 8, false, Src>(P, st, src);
 }
 
 // the flag bits of the shine_sdf_* calls: any other bit is SHINE_ERR_UNSUPPORTED, never silently ignored
@@ -1492,6 +1524,13 @@ int dispatch_tangent(const shine_octree* oct, const float* coord, int64_t n, con
 }
 
 }  // namespace
+
+int shine_internal::launch_sdf_grid(const StepParams& P, const BrickGrid& grid, uint32_t flags, cudaStream_t st) {
+    if (flags & ~kSdfFlags) return SHINE_ERR_UNSUPPORTED;
+    const int rc = check_decoder(&P.dec, &P.oct);
+    if (rc) return rc;
+    return launch_fused<false, false, GridCoords>(P, flags, st, GridCoords{grid});
+}
 
 // ------------------------------------------------------------------------------------------------------
 // C ABI

@@ -30,6 +30,19 @@ struct StepParams {
     int32_t weighted;
 };
 
+// The mesher's block-sparse grid (shine_mesh.cu): point p of a query is point r = p % (n+1)^3 of brick b = p / (n+1)^3,
+// r = (i (n+1) + j) (n+1) + k, at grid index G = bricks[b] * n + (i, j, k) and coordinate origin + spacing * G (fp32).
+struct BrickGrid {
+    const int32_t* bricks;   // [bricks, 3]
+    float origin[3];
+    float spacing;
+    int32_t n;
+};
+
+// shine_sdf_infer's kernel over the points of a BrickGrid instead of a coordinate array; out_pred gets -Decoder.sdf
+// (the mesher's sign, utils/mesher.py:72).  Checks the decoder and the flags; P.n / P.num_tiles count the grid's points.
+int launch_sdf_grid(const StepParams& P, const BrickGrid& grid, uint32_t flags, cudaStream_t st);
+
 }  // namespace shine_internal
 
 namespace {

@@ -23,7 +23,9 @@ runs either mode, as the config selects it, on a synthetic drive along +x and pr
 from __future__ import annotations
 
 import ctypes as C
+import os
 
+import numpy as np
 import torch
 
 from . import _abi
@@ -120,7 +122,7 @@ def cal_feature_importance(trainer: SdfTrainer, octree: FeatureOctree, coord_poo
 
 
 def run_shine_mapping_incremental(config: SHINEConfig, octree: FeatureOctree, decoder: Decoder, frames, iters=None,
-                                  log=None, pool=None):
+                                  log=None, pool=None, run_path=None, begin_pose_inv=None, map_bbx=None):
     """frames: iterable of (coord, sdf_label, weight) sample sets, one per scan (what `process_frame` leaves in the
     pools).  Returns per-frame dicts with first/last loss (and first/last eikonal mean with ekional_loss_on).
 
@@ -128,7 +130,12 @@ def run_shine_mapping_incremental(config: SHINEConfig, octree: FeatureOctree, de
     (`continual_learning_reg: False`, dataset/lidar_dataset.py:235-271): frames are then (coord, sdf_label, weight,
     origin_scaled), the pool keeps the earlier frames' samples, dropping with `window_replay_on` those `window_radius`
     metres or more from the new frame's origin, and batches are drawn from the whole pool.  The history also records
-    the pool size."""
+    the pool size.
+
+    run_path: mesh the map to run_path/mesh/mesh_frame_{frame+1}.ply after the first frame and every mesh_freq_frame
+    frames (shine_incre.py:198-211), octree or bbx mode as mc_with_octree selects, transformed by inv(begin_pose_inv).
+    map_bbx: a function returning the map's (min, max) metres so far (`lambda: dataset.map_bbx` for real scans, the box
+    of the frames' points as in the reference); without it, the box of the surface samples so far; the history entry of such a frame records the file under "mesh"."""
     if pool is not None and config.continual_learning_reg:
         raise ValueError("continual_learning_reg keeps the current frame's samples only; a replay pool is the other "
                          "incremental mode (dataset/lidar_dataset.py:223 vs :235): pass pool=None or turn the "
@@ -139,6 +146,12 @@ def run_shine_mapping_incremental(config: SHINEConfig, octree: FeatureOctree, de
     window = config.window_radius * config.scale if config.window_replay_on else None    # lidar_dataset.py:237-239
     dev = None
     history = []
+    mesher, samples_bbx = None, None
+    if run_path:
+        from .mesher import Mesher
+        mesher = Mesher(config, octree, decoder)
+        if begin_pose_inv is not None:
+            mesher.global_transform = np.linalg.inv(begin_pose_inv)
     for fid, frame in enumerate(frames):
         coord, label, weight = frame[:3]
         if fid == config.freeze_after_frame:   # reference shine_incre.py:97-101
@@ -182,6 +195,12 @@ def run_shine_mapping_incremental(config: SHINEConfig, octree: FeatureOctree, de
             history[-1]["pool"] = len(pool)
         if config.ekional_loss_on:
             history[-1].update(eik_first=eik_first, eik_last=eik_last)
+        if mesher is not None:
+            from .mesher import reconstruct, surface_bbx
+            samples_bbx = surface_bbx(coord, weight, config.scale, samples_bbx)
+            if fid == 0 or (fid + 1) % config.mesh_freq_frame == 0:
+                history[-1]["mesh"] = os.path.join(run_path, "mesh", f"mesh_frame_{fid + 1}.ply")
+                reconstruct(config, mesher, history[-1]["mesh"], map_bbx() if map_bbx is not None else samples_bbx)
         if log:
             log(history[-1])
     return history
@@ -200,6 +219,7 @@ def main(argv=None):
     ap.add_argument("--iters", type=int, default=None)
     ap.add_argument("--scans", action="store_true",
                     help="map the sequence of the config's pc_path / pose_path / calib_path instead of the synthetic drive")
+    ap.add_argument("--run-path", default=None, metavar="DIR", help="write meshes (mesh/mesh_frame_*.ply) under DIR")
     args = ap.parse_args(argv)
     config = SHINEConfig()
     config.load(args.config)
@@ -209,9 +229,12 @@ def main(argv=None):
     dev = config.device
     # shine_incre.py:106: the regularisation mode keeps the current frame's samples only, the other mode replays
     pool = None if config.continual_learning_reg else synth.ReplayPool(dev)
+    begin_pose_inv = map_bbx = None
     if args.scans:
         from .scans import LiDARDataset
-        frames = LiDARDataset(config).frames()            # read and sampled one frame at a time, as the loop asks
+        dataset = LiDARDataset(config)
+        frames, begin_pose_inv = dataset.frames(), dataset.begin_pose_inv   # read and sampled one frame at a time
+        map_bbx = lambda: dataset.map_bbx
     else:
         scans = synth.generate_scans(config, args.synthetic_azimuth, args.frames, args.frame_step_m, seed=config.seed,
                                      device=dev)
@@ -219,7 +242,8 @@ def main(argv=None):
                   for f, (coord, label, weight, _) in enumerate(scans)]
     print("Begin mapping:", "replay" + (f" (window {config.window_radius} m)" if config.window_replay_on else "")
           if pool is not None else "regularisation")
-    history = run_shine_mapping_incremental(config, octree, decoder, frames, iters=args.iters, log=print, pool=pool)
+    history = run_shine_mapping_incremental(config, octree, decoder, frames, iters=args.iters, log=print, pool=pool,
+                                            run_path=args.run_path, begin_pose_inv=begin_pose_inv, map_bbx=map_bbx)
     octree.print_detail()
     return history
 

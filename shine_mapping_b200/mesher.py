@@ -1,0 +1,303 @@
+"""Mesh reconstruction from the map, after reference utils/mesher.py (`recon_octree_mesh`, `recon_bbx_mesh`).
+
+The SDF grid is block-sparse: bricks of n^3 marching-cubes cells, each stored with its +1 faces so that a chunk of bricks
+is queried (`shine_mesh_grid`, shine_sdf_infer's kernel over generated coordinates) and meshed (`shine_marching_cubes`)
+without the others.  Peak device memory of the grid is 5 (n+1)^3 bytes per brick of a chunk: CHUNK_POINTS points,
+80 MiB, whatever the size of the map.  Vertices are welded across bricks and chunks through an edge table (16 bytes per
+slot, kept at most half full).  Normals and the cluster filter follow on the GPU (`shine_mesh_clusters`), the compaction and
+`global_transform` are tensor indexing and one 4x4 product.
+
+DESIGN.md §8 states the grid rules and where this differs from the reference.
+"""
+from __future__ import annotations
+
+import ctypes as C
+import os
+
+import numpy as np
+import torch
+
+from . import _abi
+from .config import SHINEConfig
+from .decoder import Decoder
+from .feature_octree import FeatureOctree, morton_to_points
+
+CHUNK_POINTS = 1 << 24      # grid points per chunk (sdf fp32 + mask byte: 80 MiB)
+BBX_TILE = 16               # cubes per brick side in bbx mode
+MAX_EDGE_SLOTS = 1 << 31   # edge-table capacity is a uint32 power of two (32 GiB of 16-byte slots)
+OCTREE_MIN_CLUSTER = 300    # filter_isolated_vertices' default (utils/mesher.py:240), used by recon_octree_mesh
+
+
+def _next_pow2(n: int) -> int:
+    return 1 << max(0, int(n) - 1).bit_length()
+
+
+def _brick_keys(bricks: torch.Tensor) -> torch.Tensor:
+    b = bricks.long()
+    return (b[:, 0] << 42) | (b[:, 1] << 21) | b[:, 2]
+
+
+class Mesher:
+    def __init__(self, config: SHINEConfig, octree: FeatureOctree, decoder: Decoder):
+        if config.mc_local:
+            raise NotImplementedError("mc_local (a mesh of the current frame's bounding box only) is not implemented")
+        if config.semantic_on:
+            raise NotImplementedError("semantic meshing is not implemented")
+        self.config = config
+        self.octree = octree
+        self.decoder = decoder
+        self.world_scale = config.scale
+        self.global_transform = np.eye(4)
+
+    # ---- the reference's surface ---------------------------------------------------------------------------------
+
+    @torch.no_grad()
+    def recon_octree_mesh(self, query_level: int, mc_res_m: float, mesh_path: str | None = None):
+        """utils/mesher.py:296-368: one n^3 block per octree node at `query_level`."""
+        grid = self.octree_grid(query_level, mc_res_m)
+        return self._mesh(grid, OCTREE_MIN_CLUSTER, mesh_path)
+
+    @torch.no_grad()
+    def recon_bbx_mesh(self, bbx_min_m, bbx_max_m, mc_res_m: float, mesh_path: str | None = None):
+        """utils/mesher.py:253-290 with get_query_from_bbx (:110-150): a dense grid over the padded box, of which only
+        the tiles that overlap a node at the coarsest featured level are queried (the others are masked everywhere)."""
+        grid = self.bbx_grid(bbx_min_m, bbx_max_m, mc_res_m)
+        return self._mesh(grid, self.config.min_cluster_vertices, mesh_path)
+
+    # ---- grids -------------------------------------------------------------------------------------------------
+
+    def _mask_level(self) -> int:
+        return min(self.octree.featured_level_num, self.config.mc_vis_level) - 1       # utils/mesher.py:47
+
+    def octree_grid(self, query_level: int, mc_res_m: float) -> dict:
+        dev = self.octree.hier_features[0].device
+        nodes = morton_to_points(self.octree._levels[query_level].node_keys.to(dev)).to(torch.int32)
+        node_res = 2.0 ** (1 - query_level)
+        n = int(np.ceil(node_res / self.world_scale / mc_res_m))
+        h = node_res / n
+        if nodes.shape[0] == 0:
+            lo = hi = [0, 0, 0]
+        else:
+            lo = (nodes.amin(0).long() * n).tolist()
+            hi = ((nodes.amax(0).long() + 1) * n).tolist()
+        origin = np.full(3, -1.0 + 0.5 * h)
+        return dict(bricks=nodes.contiguous(), n=n, origin_scaled=origin, spacing=h, lo=lo, hi=hi,
+                    all_keys=torch.sort(_brick_keys(nodes)).values, voxel_m=h / self.world_scale,
+                    origin_m=(origin + h * np.asarray(lo, dtype=np.float64)) / self.world_scale)
+
+    def bbx_grid(self, bbx_min_m, bbx_max_m, mc_res_m: float) -> dict:
+        cfg = self.config
+        lo_m, hi_m = np.asarray(bbx_min_m, dtype=np.float64), np.asarray(bbx_max_m, dtype=np.float64)
+        dims = (np.ceil((hi_m - lo_m) / mc_res_m) + cfg.pad_voxel * 2).astype(np.int64)    # utils/mesher.py:126-130
+        origin_m = lo_m - cfg.pad_voxel * mc_res_m
+        origin_m[2] -= mc_res_m
+        dims[2] += 1
+        n = BBX_TILE
+        dev = self.octree.hier_features[0].device
+        q = self.octree.free_level_num
+        nodes = morton_to_points(self.octree._levels[q].node_keys.to(dev)).double()
+        node_res = 2.0 ** (1 - q)
+        o = torch.tensor(origin_m * self.world_scale, dtype=torch.float64, device=dev)
+        s = mc_res_m * self.world_scale
+        d = torch.tensor(dims, device=dev)
+        # tiles that a node (closed box, widened by one grid step) overlaps; tiles without a node are masked everywhere
+        gmin = torch.floor((nodes * node_res - 1.0 - o) / s).long() - 1
+        gmax = torch.ceil(((nodes + 1) * node_res - 1.0 - o) / s).long() + 1
+        ok = ((gmax >= 0) & (gmin <= d - 1)).all(1)
+        tmin = (gmin[ok].clamp(min=0) // n)
+        tmax = (torch.minimum(gmax[ok], d - 1) // n)
+        if tmin.shape[0]:
+            span = int((tmax - tmin).max()) + 1
+            r = torch.arange(span, device=dev)
+            off = torch.stack(torch.meshgrid(r, r, r, indexing="ij"), -1).reshape(-1, 3)
+            cand = tmin[:, None, :] + off[None]
+            cand = cand[(cand <= tmax[:, None, :]).all(-1)]
+            bricks = torch.unique(cand, dim=0).to(torch.int32)
+        else:
+            bricks = torch.zeros(0, 3, dtype=torch.int32, device=dev)
+        return dict(bricks=bricks.contiguous(), n=n, origin_scaled=origin_m * self.world_scale, spacing=s, lo=[0, 0, 0],
+                    hi=dims.tolist(), all_keys=None, voxel_m=mc_res_m, origin_m=origin_m)
+
+    # ---- queries -------------------------------------------------------------------------------------------------
+
+    def _desc(self, grid: dict, bricks, sdf, mask) -> _abi.ShineBrickGrid:
+        g = _abi.ShineBrickGrid()
+        g.bricks, g.sdf, g.mask = bricks.data_ptr(), sdf.data_ptr(), mask.data_ptr()
+        keys = grid["all_keys"]
+        g.all_keys, g.num_all = (keys.data_ptr(), keys.numel()) if keys is not None else (None, 0)
+        g.num_bricks = bricks.shape[0]
+        for a in range(3):
+            g.origin[a] = float(np.float32(grid["origin_scaled"][a]))
+            g.lo[a], g.hi[a] = int(grid["lo"][a]), int(grid["hi"][a])
+        g.spacing = float(np.float32(grid["spacing"]))
+        g.n = grid["n"]
+        g.missing_sdf = 0.0
+        return g
+
+    def chunks(self, grid: dict):
+        """-> (bricks, sdf [b, (n+1)^3], mask) per chunk, filled by shine_mesh_grid.  The buffers are reused."""
+        n1 = grid["n"] + 1
+        per = n1 ** 3
+        step = max(1, CHUNK_POINTS // per)
+        bricks = grid["bricks"]
+        dev = bricks.device
+        nb = min(step, bricks.shape[0])
+        sdf = torch.empty(nb * per, dtype=torch.float32, device=dev)
+        mask = torch.empty(nb * per, dtype=torch.uint8, device=dev)
+        od = self.octree._descriptor(None, None)
+        dd = self.decoder.c_descriptor(None)
+        for s in range(0, bricks.shape[0], step):
+            b = bricks[s:s + step]
+            g = self._desc(grid, b, sdf, mask)
+            _abi.check(_abi.lib().shine_mesh_grid(C.byref(od), C.byref(dd), C.byref(g), self._mask_level(), 0,
+                                                  _abi.stream_ptr(dev)), "shine_mesh_grid")
+            yield b, sdf[:b.shape[0] * per].view(b.shape[0], per), mask[:b.shape[0] * per].view(b.shape[0], per), g
+
+    @staticmethod
+    def edge_capacity(grid: dict) -> int:
+        """First size of the edge table: room for about one vertex per cube on two faces of every brick, at load 1/2."""
+        return min(MAX_EDGE_SLOTS, _next_pow2(max(1 << 16, 4 * grid["n"] ** 2 * grid["bricks"].shape[0])))
+
+    def marching_cubes(self, grid: dict):
+        """-> (verts [V,3] fp32 in grid units relative to grid['lo'], faces [T,3] int32), welded, on the device.
+        The edge table is kept at most half full (checked after every chunk); past that, or when an insert finds no free
+        slot, the mesh starts over with a table 4x larger."""
+        dev = grid["bricks"].device
+        cap = self.edge_capacity(grid)
+        lib, st = _abi.lib(), _abi.stream_ptr(dev)
+        while True:
+            slots = torch.full((cap * 16,), 0xFF, dtype=torch.uint8, device=dev)
+            counters = torch.zeros(4, dtype=torch.int32, device=dev)
+            verts = torch.empty(0, 3, dtype=torch.float32, device=dev)
+            faces, full = [], False
+            for _, _, _, g in self.chunks(grid):
+                counters[1:3].zero_()
+                _abi.check(lib.shine_marching_cubes(C.byref(g), _abi.ptr(slots), cap, _abi.ptr(counters), None, 0, None, 0,
+                                                    st), "shine_marching_cubes")
+                nv, nt, _, lost = counters.tolist()                # the chunk's one read-back: output sizes
+                if lost or 2 * nv > cap:
+                    full = True
+                    break
+                if nv > verts.shape[0]:
+                    grown = torch.empty(max(nv, 2 * verts.shape[0]), 3, dtype=torch.float32, device=dev)
+                    grown[:verts.shape[0]] = verts
+                    verts = grown
+                f = torch.empty(nt, 3, dtype=torch.int32, device=dev)
+                _abi.check(lib.shine_marching_cubes(C.byref(g), _abi.ptr(slots), cap, _abi.ptr(counters), _abi.ptr(verts),
+                                                    verts.shape[0], _abi.ptr(f), nt, st), "shine_marching_cubes")
+                faces.append(f)
+            if not full:
+                nv = int(counters[0])
+                return verts[:nv], (torch.cat(faces) if faces else torch.zeros(0, 3, dtype=torch.int32, device=dev))
+            if cap >= MAX_EDGE_SLOTS:
+                raise _abi.ShineB200Error(f"the mesh has more than {MAX_EDGE_SLOTS // 2} vertices (edge table limit)")
+            cap = min(MAX_EDGE_SLOTS, cap * 4)
+
+    def _mesh(self, grid: dict, min_tris: int, mesh_path):
+        verts, faces = self.marching_cubes(grid)
+        verts_m = (torch.tensor(grid["origin_m"], dtype=torch.float64, device=verts.device)
+                   + verts.double() * grid["voxel_m"])
+        normals, keep = normals_and_clusters(verts_m.float(), faces, min_tris)
+        verts_m, faces, normals = compact(verts_m, faces, normals, keep)
+        T = torch.tensor(self.global_transform, dtype=torch.float64, device=verts.device)     # mesh.transform (:284,:362)
+        verts_out = (verts_m @ T[:3, :3].T + T[:3, 3]).float()
+        normals = normals.double() @ T[:3, :3].T
+        normals = (normals / normals.norm(dim=1, keepdim=True).clamp_min(1e-300)).float()
+        if mesh_path:
+            write_ply(mesh_path, verts_out, faces, normals)
+        return verts_out, faces, normals
+
+
+def normals_and_clusters(verts: torch.Tensor, faces: torch.Tensor, min_tris: int):
+    """-> (normals [V,3], keep [T] bool): compute_vertex_normals and the cluster filter's triangle mask."""
+    dev = verts.device
+    nv, nt = verts.shape[0], faces.shape[0]
+    cap = _next_pow2(max(16, 6 * nt))
+    if cap > MAX_EDGE_SLOTS:
+        raise _abi.ShineB200Error(f"{nt} triangles: more than the cluster filter's edge table holds")
+    slots = torch.full((cap * 16,), 0xFF, dtype=torch.uint8, device=dev)
+    scratch = torch.empty(max(1, 2 * nt), dtype=torch.int32, device=dev)
+    keep = torch.empty(max(1, nt), dtype=torch.uint8, device=dev)
+    normals = torch.empty(nv, 3, dtype=torch.float32, device=dev)
+    _abi.check(_abi.lib().shine_mesh_clusters(_abi.ptr(verts.contiguous()), nv, _abi.ptr(faces.contiguous()), nt,
+                                              int(min_tris), _abi.ptr(slots), cap, _abi.ptr(scratch), _abi.ptr(keep),
+                                              _abi.ptr(normals), _abi.stream_ptr(dev)), "shine_mesh_clusters")
+    return normals, keep[:nt].bool()
+
+
+def compact(verts, faces, normals, keep):
+    """Drop the triangles with keep False and then every vertex no triangle uses (Open3D's remove_triangles_by_mask
+    keeps those vertices); vertex ids are renumbered in order."""
+    faces = faces[keep]
+    used = torch.zeros(verts.shape[0], dtype=torch.bool, device=verts.device)
+    used[faces.reshape(-1).long()] = True
+    remap = torch.cumsum(used.int(), 0, dtype=torch.int32) - 1
+    return verts[used], remap[faces.long()], normals[used]
+
+
+def reconstruct(config: SHINEConfig, mesher: Mesher, mesh_path: str, map_bbx=None):
+    """The mesh call of the mapping loops (shine_batch.py:240-245, shine_incre.py:203-211): octree or bbx mode as
+    `mc_with_octree` selects.  map_bbx: (min, max) metres in the map frame, needed by bbx mode."""
+    if config.mc_with_octree:      # mc_query_level = tree_level_world - tree_level_feat + 1 (utils/config.py:366)
+        return mesher.recon_octree_mesh(mesher.octree.free_level_num, config.mc_res_m, mesh_path)
+    if map_bbx is None:
+        raise ValueError("mc_with_octree: False meshes the map's bounding box: pass map_bbx")
+    return mesher.recon_bbx_mesh(map_bbx[0], map_bbx[1], config.mc_res_m, mesh_path)
+
+
+def surface_bbx(coord: torch.Tensor, weight: torch.Tensor, scale: float, bbx=None):
+    """(min, max) metres of the surface samples (weight > 0) of scaled coordinates, merged with `bbx` (None: nothing yet):
+    the synthetic map's map_bbx.  A frame without surface samples leaves `bbx` as it is."""
+    s = coord[weight > 0].double() / scale
+    if s.shape[0] == 0:
+        return bbx
+    lo, hi = s.amin(0).cpu().numpy(), s.amax(0).cpu().numpy()
+    return (lo, hi) if bbx is None else (np.minimum(bbx[0], lo), np.maximum(bbx[1], hi))
+
+
+# ---- PLY -------------------------------------------------------------------------------------------------------------
+
+_VERTEX = np.dtype([("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("nx", "<f4"), ("ny", "<f4"), ("nz", "<f4")])
+_FACE = np.dtype([("n", "u1"), ("v", "<i4", (3,))])
+
+
+def write_ply(path: str, verts, faces, normals) -> None:
+    """Binary little-endian PLY: float32 x y z nx ny nz per vertex, `uchar int` vertex_indices per face."""
+    v = np.asarray(torch.as_tensor(verts).detach().cpu(), dtype=np.float32).reshape(-1, 3)
+    nrm = np.asarray(torch.as_tensor(normals).detach().cpu(), dtype=np.float32).reshape(-1, 3)
+    f = np.asarray(torch.as_tensor(faces).detach().cpu(), dtype=np.int32).reshape(-1, 3)
+    vert = np.empty(v.shape[0], dtype=_VERTEX)
+    for i, k in enumerate("xyz"):
+        vert[k] = v[:, i]
+        vert["n" + k] = nrm[:, i]
+    face = np.empty(f.shape[0], dtype=_FACE)
+    face["n"] = 3
+    face["v"] = f
+    header = ("ply\nformat binary_little_endian 1.0\n"
+              f"element vertex {v.shape[0]}\nproperty float x\nproperty float y\nproperty float z\n"
+              "property float nx\nproperty float ny\nproperty float nz\n"
+              f"element face {f.shape[0]}\nproperty list uchar int vertex_indices\nend_header\n")
+    os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
+    with open(path, "wb") as fh:
+        fh.write(header.encode("ascii"))
+        fh.write(vert.tobytes())
+        fh.write(face.tobytes())
+
+
+def read_ply(path: str):
+    """The files write_ply writes -> (verts [V,3], faces [T,3], normals [V,3]) numpy arrays."""
+    with open(path, "rb") as fh:
+        data = fh.read()
+    end = data.index(b"end_header\n") + len(b"end_header\n")
+    head = data[:end].decode("ascii").splitlines()
+    if head[1] != "format binary_little_endian 1.0":
+        raise ValueError(f"{path}: not a binary little-endian PLY")
+    nv = next(int(l.split()[2]) for l in head if l.startswith("element vertex"))
+    nf = next(int(l.split()[2]) for l in head if l.startswith("element face"))
+    vert = np.frombuffer(data, dtype=_VERTEX, count=nv, offset=end)
+    face = np.frombuffer(data, dtype=_FACE, count=nf, offset=end + nv * _VERTEX.itemsize)
+    if nf and not (face["n"] == 3).all():
+        raise ValueError(f"{path}: faces that are not triangles")
+    v = np.stack([vert[k] for k in "xyz"], 1)
+    nrm = np.stack([vert["n" + k] for k in "xyz"], 1)
+    return v, face["v"].copy(), nrm

@@ -384,6 +384,7 @@ class LiDARDataset:
                 pool = synth.SamplePool(self.device)
         self.pool = pool
         self.processor = ScanProcessor(config, self.device)
+        self._bbx = None
 
     def origin_scaled(self, frame_id: int) -> np.ndarray:
         """dataset/lidar_dataset.py:175: the frame's sensor origin in scaled coordinates, numpy fp64."""
@@ -395,6 +396,9 @@ class LiDARDataset:
         points = self.processor.points(rec, self.poses_ref[frame_id])
         origin = torch.tensor(self.origin_scaled(frame_id), dtype=torch.float32)
         coord, label, weight = self.processor.sample(points, origin.numpy())
+        if points.shape[0]:       # map_bbx of dataset/lidar_dataset.py:196-203, kept on the device (no host read here)
+            lo, hi = points.amin(0), points.amax(0)
+            self._bbx = (lo, hi) if self._bbx is None else (torch.minimum(self._bbx[0], lo), torch.maximum(self._bbx[1], hi))
         return coord, label, weight, origin, points
 
     def surface_samples(self, coord: torch.Tensor) -> torch.Tensor:
@@ -417,6 +421,13 @@ class LiDARDataset:
         else:
             self.pool.append(coord, label, weight)
         return coord, label, weight
+
+    @property
+    def map_bbx(self):
+        """(min, max) metres in the map frame of the points of the frames read so far (None before the first)."""
+        if self._bbx is None:
+            return None
+        return tuple((t.double() / self.config.scale).cpu().numpy() for t in self._bbx)
 
     def frames(self):
         """(coord, sdf_label, weight, origin_scaled) per used frame, for `run_shine_mapping_incremental`."""

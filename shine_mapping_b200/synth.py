@@ -375,9 +375,11 @@ def generate_scans(config: SHINEConfig, n_azimuth: int, n_frames: int = 1, frame
 def build_scene_map(config: SHINEConfig, octree, n_azimuth: int, n_frames: int = 1, frame_step_m: float = 1.0,
                     seed: int = 42, device=None, origin_x0: float = 0.0, pool=None):
     """Scan the analytic scene from `n_frames` poses along +x, sample every scan, grow the octree from the
-    surface samples (weight > 0; dataset/lidar_dataset.py:212-218) and return the pool.
+    surface samples (weight > 0; dataset/lidar_dataset.py:212-218) and return the pool, with `map_bbx` set to the
+    (min, max) metres of the surface samples.
     pool: None = a new SamplePool; "auto" = a new HostSamplePool if `use_host_pool(config, n_frames)`, else a new
     SamplePool; or the (Host)SamplePool to fill."""
+    from . import mesher as _mesher
     device = device or config.device
     if pool is None:
         pool = SamplePool(device)
@@ -391,4 +393,5 @@ def build_scene_map(config: SHINEConfig, octree, n_azimuth: int, n_frames: int =
         else:
             octree.update(hits)
         pool.append(coord, label, weight)
+        pool.map_bbx = _mesher.surface_bbx(coord, weight, config.scale, getattr(pool, "map_bbx", None))   # for bbx meshing
     return pool
