@@ -450,6 +450,36 @@ int shine_mesh_clusters(const float* verts, int64_t nv, const int32_t* tris, int
                         void* edge_slots, uint32_t edge_capacity, int32_t* scratch, uint8_t* keep, float* normals,
                         void* stream);
 
+/* ---- evaluation: eval/eval_utils.py eval_mesh / crop_intersection ----------------------------------------------------
+ * Uniform sampling of a mesh (Open3D SamplePointsUniformly) in two calls, with one host read between them:
+ *   areas: area_t = 0.5 |(p0 - p1) x (p0 - p2)| in fp64 for every triangle, 0 for a triangle with a vertex outside
+ *     crop_box (device [6] fp64: min x y z, max x y z, inclusive; NULL = no crop); their inclusive prefix sums, by a
+ *     deterministic chunked scan, in the scratch; the total area S to the device double *total_area.
+ *   points: sample k lies on the first triangle t with round(cum_t / S * N) > k (N for the last triangle), at
+ *     (a v0 + b v1) + c v2 in fp64 with a = 1 - sqrt(r1), b = sqrt(r1)(1 - r2), c = sqrt(r1) r2; (r1, r2) are two 53-bit
+ *     doubles in [0, 1) from Philox4x32-10 with key seed and counter k.  S must be > 0 when num_samples > 0.
+ *     tri_ids [N] (optional) receives t.
+ * Vertices are fp64 [num_verts, 3]; triangles int32 [num_tris, 3] with indices in [0, num_verts). */
+int64_t shine_mesh_sample_scratch_bytes(int64_t num_tris);
+int shine_mesh_sample_areas(const double* verts, int64_t num_verts, const int32_t* tris, int64_t num_tris,
+                            const double* crop_box, double* total_area, void* scratch, int64_t scratch_bytes,
+                            void* stream);
+int shine_mesh_sample_points(const double* verts, const int32_t* tris, int64_t num_tris, const double* total_area,
+                             int64_t num_samples, uint64_t seed, const void* scratch, int64_t scratch_bytes,
+                             double* points, int32_t* tri_ids, void* stream);
+
+/* Exact nearest neighbour within a radius.  build: a tree over n fp64 reference points [n, 3] in the caller's `tree`
+ * buffer (shine_nn_tree_bytes(n), kept until the last query; 256-byte aligned).  query: for each of m fp64 points,
+ * d2 = (dx*dx + dy*dy) + dz*dz (no contraction) minimised over the reference points; if d2 < radius2, dist = sqrt(d2)
+ * and index = the input index of a nearest point (any one of exact ties), else dist = +inf and index = -1.
+ * scratch: shine_nn_scratch_bytes(n) for a build, shine_nn_scratch_bytes(m) for a query, 256-byte aligned. */
+int64_t shine_nn_tree_bytes(int64_t n);
+int64_t shine_nn_scratch_bytes(int64_t n);
+int shine_nn_build(const double* points, int64_t n, void* tree, int64_t tree_bytes, void* scratch, int64_t scratch_bytes,
+                   void* stream);
+int shine_nn_query(const void* tree, int64_t n, const double* queries, int64_t m, double radius2, double* dist,
+                   int32_t* index, void* scratch, int64_t scratch_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

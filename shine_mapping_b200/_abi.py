@@ -170,6 +170,13 @@ SYMBOLS = {
     "shine_mesh_grid": (C.c_int, [_OCT, _DEC, C.POINTER(ShineBrickGrid), _i32, _u32, _vp]),
     "shine_marching_cubes": (C.c_int, [C.POINTER(ShineBrickGrid), _vp, _u32, _vp, _vp, _i64, _vp, _i64, _vp]),
     "shine_mesh_clusters": (C.c_int, [_vp, _i64, _vp, _i64, _i32, _vp, _u32, _vp, _vp, _vp, _vp]),
+    "shine_mesh_sample_scratch_bytes": (C.c_int64, [_i64]),
+    "shine_mesh_sample_areas": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _vp, _i64, _vp]),
+    "shine_mesh_sample_points": (C.c_int, [_vp, _vp, _i64, _vp, _i64, C.c_uint64, _vp, _i64, _vp, _vp, _vp]),
+    "shine_nn_tree_bytes": (C.c_int64, [_i64]),
+    "shine_nn_scratch_bytes": (C.c_int64, [_i64]),
+    "shine_nn_build": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _i64, _vp]),
+    "shine_nn_query": (C.c_int, [_vp, _i64, _vp, _i64, C.c_double, _vp, _vp, _vp, _i64, _vp]),
 }
 
 _lib = None

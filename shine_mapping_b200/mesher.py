@@ -285,19 +285,68 @@ def write_ply(path: str, verts, faces, normals) -> None:
 
 
 def read_ply(path: str):
-    """The files write_ply writes -> (verts [V,3], faces [T,3], normals [V,3]) numpy arrays."""
+    """A triangle mesh PLY, ascii or binary little-endian -> (verts [V,3], faces [T,3] int32, normals [V,3] or None)
+    numpy arrays.  Vertex x y z (and nx ny nz, when present) are float or double and keep their type; other scalar
+    properties are skipped.  The face element has one list property `vertex_indices` or `vertex_index` of any integer
+    count and index types.  Polygons, big-endian files and a missing face element raise ValueError."""
+    from .scans import _xyz_layout, read_ply_header
     with open(path, "rb") as fh:
-        data = fh.read()
-    end = data.index(b"end_header\n") + len(b"end_header\n")
-    head = data[:end].decode("ascii").splitlines()
-    if head[1] != "format binary_little_endian 1.0":
-        raise ValueError(f"{path}: not a binary little-endian PLY")
-    nv = next(int(l.split()[2]) for l in head if l.startswith("element vertex"))
-    nf = next(int(l.split()[2]) for l in head if l.startswith("element face"))
-    vert = np.frombuffer(data, dtype=_VERTEX, count=nv, offset=end)
-    face = np.frombuffer(data, dtype=_FACE, count=nf, offset=end + nv * _VERTEX.itemsize)
-    if nf and not (face["n"] == 3).all():
-        raise ValueError(f"{path}: faces that are not triangles")
-    v = np.stack([vert[k] for k in "xyz"], 1)
-    nrm = np.stack([vert["n" + k] for k in "xyz"], 1)
-    return v, face["v"].copy(), nrm
+        fmt, elements = read_ply_header(fh, path)
+        body = fh.read()
+    names = [e[0] for e in elements]
+    if "vertex" not in names:
+        raise ValueError(f"{path}: no vertex element")
+    if "face" not in names:
+        raise ValueError(f"{path}: no face element (not a triangle mesh)")
+    vertex, face = elements[names.index("vertex")], elements[names.index("face")]
+    _xyz_layout(path, vertex[2])
+    props = face[2]
+    if len(props) != 1 or props[0][2] != 0 or props[0][0] not in ("vertex_indices", "vertex_index"):
+        raise ValueError(f"{path}: the face element must hold one list property vertex_indices / vertex_index")
+    count_t, index_t = props[0][1] or (None, None)
+    if count_t is None or count_t.kind not in "iu" or index_t.kind not in "iu":
+        raise ValueError(f"{path}: face indices must be a list of integers")
+    # elements before the face element are read; those after it are ignored
+    order = names.index("face")
+    for name, _, fields in elements[:order]:
+        if any(c == 0 for _, _, c in fields):
+            raise ValueError(f"{path}: element {name!r} before the faces has a list property")
+    if fmt == "ascii":
+        tok, pos = body.split(), 0
+        arrays = {}
+        for name, n, fields in elements[:order + 1]:
+            width = len(fields) if name != "face" else 4
+            if pos + n * width > len(tok):
+                raise ValueError(f"{path}: file ends inside element {name!r}")
+            arrays[name] = np.array(tok[pos:pos + n * width], dtype=np.float64).reshape(n, width)
+            pos += n * width
+        vals = arrays["vertex"]
+        col = {nm: i for i, (nm, _, _) in reversed(list(enumerate(vertex[2])))}
+        types = {nm: dt for nm, dt, _ in reversed(vertex[2])}
+        v = np.stack([vals[:, col[a]].astype(types[a]) for a in "xyz"], 1)
+        nrm = (np.stack([vals[:, col[a]].astype(types[a]) for a in ("nx", "ny", "nz")], 1)
+               if all(a in col for a in ("nx", "ny", "nz")) else None)
+        counts, idx = arrays["face"][:, 0], arrays["face"][:, 1:]
+    else:
+        off, recs = 0, {}
+        for name, n, fields in elements[:order + 1]:
+            if name == "face":
+                dt = np.dtype([("n", count_t), ("v", index_t, (3,))])
+            else:
+                dt = np.dtype([(f"p{i}", f[1]) for i, f in enumerate(fields)])
+            if off + n * dt.itemsize > len(body):
+                raise ValueError(f"{path}: file ends inside element {name!r}")
+            recs[name] = (np.frombuffer(body, dtype=dt, count=n, offset=off), fields)
+            off += n * dt.itemsize
+        vert, fields = recs["vertex"]
+        col = {nm: f"p{i}" for i, (nm, _, _) in reversed(list(enumerate(fields)))}
+        v = np.stack([vert[col[a]] for a in "xyz"], 1)
+        nrm = (np.stack([vert[col[a]] for a in ("nx", "ny", "nz")], 1)
+               if all(a in col for a in ("nx", "ny", "nz")) else None)
+        counts, idx = recs["face"][0]["n"], recs["face"][0]["v"]
+    if counts.shape[0] and not (counts == 3).all():
+        raise ValueError(f"{path}: faces that are not triangles (polygons are not supported)")
+    idx = np.asarray(idx)
+    if idx.shape[0] and (idx.min() < 0 or idx.max() >= v.shape[0]):
+        raise ValueError(f"{path}: face indices outside [0, {v.shape[0]})")
+    return v, idx.astype(np.int32).reshape(-1, 3), nrm

@@ -212,37 +212,49 @@ _PLY_TYPES = {"char": "i1", "int8": "i1", "uchar": "u1", "uint8": "u1", "short":
               "float": "<f4", "float32": "<f4", "double": "<f8", "float64": "<f8"}
 
 
+def read_ply_header(fh, filename: str):
+    """Read a PLY header from `fh` (left at the first byte of the body) -> (format, elements): each element is
+    (name, count, [(property, numpy dtype, 1)]); a list property is (property, (count dtype, item dtype), 0), with None
+    for the types when they are not PLY scalar types.
+    Big-endian files and list properties of the vertex element raise."""
+    head = _read_header(fh, filename, b"end_header")
+    if head[0] != "ply":
+        raise ValueError(f"{filename}: malformed header (no 'ply' magic)")
+    fmt, elements = None, []
+    for line in head[1:-1]:
+        tok = line.split()
+        if not tok or tok[0] in ("comment", "obj_info"):
+            continue
+        if tok[0] == "format" and len(tok) >= 2:
+            fmt = tok[1]
+        elif tok[0] == "element" and len(tok) == 3 and tok[2].isdigit():
+            elements.append((tok[1], int(tok[2]), []))
+        elif tok[0] == "property" and elements and len(tok) >= 3:
+            if tok[1] == "list":
+                if elements[-1][0] == "vertex":
+                    raise ValueError(f"{filename}: list property {tok[-1]!r} in the vertex element")
+                types = None
+                if len(tok) == 5 and tok[2] in _PLY_TYPES and tok[3] in _PLY_TYPES:
+                    types = (np.dtype(_PLY_TYPES[tok[2]]), np.dtype(_PLY_TYPES[tok[3]]))
+                elements[-1][2].append((tok[-1], types, 0))
+                continue
+            if tok[1] not in _PLY_TYPES:
+                raise ValueError(f"{filename}: malformed header (property type {tok[1]!r})")
+            elements[-1][2].append((tok[2], np.dtype(_PLY_TYPES[tok[1]]), 1))
+        else:
+            raise ValueError(f"{filename}: malformed header line {line!r}")
+    if fmt == "binary_big_endian":
+        raise ValueError(f"{filename}: big-endian PLY is not supported")
+    if fmt not in ("ascii", "binary_little_endian"):
+        raise ValueError(f"{filename}: malformed header (format {fmt!r})")
+    return fmt, elements
+
+
 def read_ply(filename: str, pinned: bool = True) -> ScanRecords:
     """PLY, ascii or binary_little_endian; x y z are float or double properties of the `vertex` element, which must
     come first; other scalar properties are skipped by size."""
     with open(filename, "rb") as fh:
-        head = _read_header(fh, filename, b"end_header")
-        if head[0] != "ply":
-            raise ValueError(f"{filename}: malformed header (no 'ply' magic)")
-        fmt, elements = None, []
-        for line in head[1:-1]:
-            tok = line.split()
-            if not tok or tok[0] in ("comment", "obj_info"):
-                continue
-            if tok[0] == "format" and len(tok) >= 2:
-                fmt = tok[1]
-            elif tok[0] == "element" and len(tok) == 3 and tok[2].isdigit():
-                elements.append((tok[1], int(tok[2]), []))
-            elif tok[0] == "property" and elements and len(tok) >= 3:
-                if tok[1] == "list":
-                    if elements[-1][0] == "vertex":
-                        raise ValueError(f"{filename}: list property {tok[-1]!r} in the vertex element")
-                    elements[-1][2].append((tok[-1], None, 1))
-                    continue
-                if tok[1] not in _PLY_TYPES:
-                    raise ValueError(f"{filename}: malformed header (property type {tok[1]!r})")
-                elements[-1][2].append((tok[2], np.dtype(_PLY_TYPES[tok[1]]), 1))
-            else:
-                raise ValueError(f"{filename}: malformed header line {line!r}")
-        if fmt == "binary_big_endian":
-            raise ValueError(f"{filename}: big-endian PLY is not supported")
-        if fmt not in ("ascii", "binary_little_endian"):
-            raise ValueError(f"{filename}: malformed header (format {fmt!r})")
+        fmt, elements = read_ply_header(fh, filename)
         if not elements or elements[0][0] != "vertex":
             raise ValueError(f"{filename}: the vertex element must come first")
         _, n, fields = elements[0]

@@ -2,6 +2,7 @@
 
 * `raycast_scene`   — analytic scene (ground plane, two walls, axis-aligned boxes) hit by an HDL-64-like
                       scan pattern from a sensor origin -> hit points in metres.
+* `scene_surface_points` — lattice points on the hittable surfaces of that scene: the ground truth of mesh evaluation.
 * `sample_rays`     — the training-sample contract of the reference's `dataSampler.sample`
                       (utils/data_sampler.py:18-139): per hit, `surface_sample_n` samples uniformly within
                       +-surface_sample_range of the hit and `free_sample_n` samples in free space; label = signed
@@ -20,6 +21,7 @@ from __future__ import annotations
 import ctypes as C
 import math
 
+import numpy as np
 import torch
 
 from .config import SHINEConfig
@@ -42,6 +44,46 @@ def default_boxes(device="cpu") -> torch.Tensor:
         [24.0, -6.5, -1.7, 27.0, -4.0, 1.0], [-20.0, 4.0, -1.7, -16.0, 6.0, -0.2], [35.0, 2.0, -1.7, 38.0, 6.5, 1.5],
         [48.0, -6.0, -1.7, 52.0, -3.8, -0.3], [62.0, 3.0, -1.7, 66.0, 5.0, 0.2], [77.0, -6.8, -1.7, 80.0, -4.4, 0.8],
         [91.0, 3.6, -1.7, 95.0, 5.6, -0.2]], dtype=torch.float32, device=device)
+
+
+def _lattice(lo, hi, spacing: float):
+    """Points lo + spacing * i per axis with i = 0 .. floor((hi - lo) / spacing), fp64, all combinations."""
+    axes = [lo[a] + spacing * np.arange(int(np.floor((hi[a] - lo[a]) / spacing + 1e-9)) + 1) for a in range(len(lo))]
+    return np.stack(np.meshgrid(*axes, indexing="ij"), -1).reshape(-1, len(lo))
+
+
+def scene_surface_points(x_min: float, x_max: float, spacing: float, ground_z: float = -1.7, wall_y: float = 8.0,
+                         wall_top: float = 4.3, boxes: torch.Tensor | None = None) -> torch.Tensor:
+    """Deterministic lattice points (fp64 [M,3], metres) on the surfaces of `raycast_scene` that a ray can hit, over
+    x in [x_min, x_max]: the ground between the walls outside the boxes' footprints, the inner faces of both walls, and
+    the four sides and the top of every box (`default_boxes()` unless given), clipped to the x range."""
+    if not spacing > 0 or not x_max >= x_min:
+        raise ValueError("scene_surface_points needs spacing > 0 and x_max >= x_min")
+    bx = (default_boxes() if boxes is None else boxes).double().cpu().numpy()
+    parts = []
+    g = _lattice((x_min, -wall_y), (x_max, wall_y), spacing)
+    inside = np.zeros(g.shape[0], dtype=bool)
+    for b in bx:
+        inside |= (g[:, 0] > b[0]) & (g[:, 0] < b[3]) & (g[:, 1] > b[1]) & (g[:, 1] < b[4])
+    g = g[~inside]
+    parts.append(np.column_stack((g, np.full(g.shape[0], ground_z))))
+    for y in (-wall_y, wall_y):
+        w = _lattice((x_min, ground_z), (x_max, wall_top), spacing)
+        parts.append(np.column_stack((w[:, 0], np.full(w.shape[0], y), w[:, 1])))
+    for b in bx:
+        lo_x, hi_x = max(b[0], x_min), min(b[3], x_max)
+        if lo_x > hi_x:
+            continue
+        top = _lattice((lo_x, b[1]), (hi_x, b[4]), spacing)
+        parts.append(np.column_stack((top, np.full(top.shape[0], b[5]))))
+        for y in (b[1], b[4]):
+            s = _lattice((lo_x, b[2]), (hi_x, b[5]), spacing)
+            parts.append(np.column_stack((s[:, 0], np.full(s.shape[0], y), s[:, 1])))
+        for x in (b[0], b[3]):
+            if x_min <= x <= x_max:
+                s = _lattice((b[1], b[2]), (b[4], b[5]), spacing)
+                parts.append(np.column_stack((np.full(s.shape[0], x), s)))
+    return torch.from_numpy(np.concatenate(parts))
 
 
 def raycast_scene(origin: torch.Tensor, dirs: torch.Tensor, boxes: torch.Tensor | None = None,
