@@ -12,7 +12,8 @@
  *   - return 0 on success, a positive cudaError_t on a CUDA failure, a negative SHINE_ERR_* on a bad
  *     argument / unsupported configuration.  shine_error_string() decodes either.
  *   - all buffers are caller-owned device memory; nothing is allocated, freed or synchronised inside;
- *     every call is asynchronous on `stream` and re-entrant.  Kernels are launched on the device that owns the
+ *     every call is asynchronous on `stream` and re-entrant (shine_mesh_export_points, which hands back a count, says
+ *     where it waits).  Kernels are launched on the device that owns the
  *     buffers (looked up from the pointers), whatever the calling thread's current device is; a batch on another
  *     device than the tables is SHINE_ERR_INVALID_ARG (pinned host batch pointers are accepted).
  *   - levels are described BOTTOM-UP like `FeatureOctree.hierarchical_indices`
@@ -37,6 +38,7 @@ extern "C" {
 #define SHINE_OK 0
 #define SHINE_ERR_INVALID_ARG (-1)
 #define SHINE_ERR_UNSUPPORTED (-2)
+#define SHINE_ERR_CAPACITY (-3)   /* an output buffer was too small; what fitted was written */
 
 /* flags of shine_sdf_* calls; shine_sdf_infer, shine_sdf_bce_fwd and shine_sdf_bce_step return SHINE_ERR_UNSUPPORTED
  * for any other bit (ABI version 3 also defined bit 8) */
@@ -441,6 +443,25 @@ int shine_mesh_grid(const shine_octree* oct, const shine_decoder* dec, const shi
  *     [tri_capacity, 3]) go to rows counters[2] onwards, counters[2] advancing. */
 int shine_marching_cubes(const shine_brick_grid* grid, void* edge_slots, uint32_t edge_capacity, int32_t* counters,
                          float* verts, int64_t vert_capacity, int32_t* tris, int64_t tri_capacity, void* stream);
+
+/* save_map (utils/mesher.py:152-173 generate_sdf_map): the grid points of one shine_mesh_grid-filled chunk as the body of a
+ * binary little-endian PLY, 20-byte records {float x, y, z, intensities; int32 labels}.  Only the points a brick OWNS are
+ * written (i, j, k < n: its +1 face points belong to a neighbour or are padding, so no point is written twice), and of
+ * those the ones with G < hi on every axis and, with masked_only, mask != 0.
+ *   position    = transform (3x4 fp64, row-major, host) applied to origin_m + voxel_m (G - lo) (fp64, host; origin_m is
+ *                 the position of grid index lo in metres): ((t0 x + t1 y) + t2 z) + t3 per row, every operation rounded
+ *                 on its own, then rounded to fp32;
+ *   intensities = sdf * sdf_factor in fp32 (the buffer holds -Decoder.sdf, the sign of the reference's sdf_pred; with
+ *                 sdf_factor = logistic_gaussian_ratio * sigma_sigmoid_m this is metres, positive in free space);
+ *   labels      = mask != 0.
+ * Record r of the call goes to records[20 (c + r)], c = *counter on entry (device int64, zeroed by the caller before the
+ * first chunk of a buffer); the order of the records is unspecified.  Records at index >= capacity are counted, not
+ * written.  Unlike the other entry points this one WAITS for its kernel: it returns with *count_out (host, optional) =
+ * *counter, and SHINE_ERR_CAPACITY when that exceeds capacity.  records (4-byte aligned), counter and the grid's buffers
+ * must be on one device. */
+int shine_mesh_export_points(const shine_brick_grid* grid, const double* origin_m, double voxel_m, const double* transform,
+                             float sdf_factor, int32_t masked_only, void* records, int64_t capacity, int64_t* counter,
+                             int64_t* count_out, void* stream);
 
 /* Open3D's compute_vertex_normals and cluster_connected_triangles as used by utils/mesher.py:240-249,278-281:
  * normals [nv, 3] = normalised sum of the unit normals of the adjacent triangles; keep[t] = 1 iff the cluster of

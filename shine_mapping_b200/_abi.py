@@ -21,6 +21,7 @@ FLAG_REDUCTION_SUM = 1
 FLAG_WEIGHTED = 2
 FLAG_TF32X1 = 4
 FLAG_MORTON_ORDERED = 16
+ERR_CAPACITY = -3
 
 
 class ShineLevel(C.Structure):
@@ -169,6 +170,8 @@ SYMBOLS = {
                                     _vp]),
     "shine_mesh_grid": (C.c_int, [_OCT, _DEC, C.POINTER(ShineBrickGrid), _i32, _u32, _vp]),
     "shine_marching_cubes": (C.c_int, [C.POINTER(ShineBrickGrid), _vp, _u32, _vp, _vp, _i64, _vp, _i64, _vp]),
+    "shine_mesh_export_points": (C.c_int, [C.POINTER(ShineBrickGrid), C.POINTER(C.c_double), C.c_double,
+                                           C.POINTER(C.c_double), _f32, _i32, _vp, _i64, _vp, C.POINTER(_i64), _vp]),
     "shine_mesh_clusters": (C.c_int, [_vp, _i64, _vp, _i64, _i32, _vp, _u32, _vp, _vp, _vp, _vp]),
     "shine_mesh_sample_scratch_bytes": (C.c_int64, [_i64]),
     "shine_mesh_sample_areas": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _vp, _vp, _i64, _vp]),

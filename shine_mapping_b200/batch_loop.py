@@ -129,7 +129,8 @@ def run_shine_mapping_batch(config: SHINEConfig, octree: FeatureOctree, decoder:
     """-> dict(loss_first, loss_last, points_per_s, timing, meshes).  `octree` must already hold the map of `pool`.
     With run_path, every vis_freq_iters iterations the map is meshed to run_path/mesh/mesh_iter_{it+1}.ply
     (shine_batch.py:236-245): octree or bbx mode (map_bbx, metres) as mc_with_octree selects, transformed by
-    inv(begin_pose_inv).  `meshes` lists the files written."""
+    inv(begin_pose_inv), and with save_map the SDF map to run_path/map/sdf_map_iter_{it+1}.ply.  `meshes` lists the mesh
+    files written."""
     check_supported(config)
     mesher = None
     if run_path:
@@ -171,9 +172,9 @@ def run_shine_mapping_batch(config: SHINEConfig, octree: FeatureOctree, decoder:
         if run_path and ((it + 1) % config.save_freq_iters == 0) and it > 0:
             save_checkpoint(octree, decoder, trainer, run_path, f"model/model_iter_{it + 1}", it)
         if mesher is not None and ((it + 1) % config.vis_freq_iters == 0) and it > 0:     # between graph replays
-            from .mesher import reconstruct
+            from .mesher import reconstruct, sdf_map_path
             meshes.append(os.path.join(run_path, "mesh", f"mesh_iter_{it + 1}.ply"))
-            reconstruct(config, mesher, meshes[-1], map_bbx)
+            reconstruct(config, mesher, meshes[-1], map_bbx, sdf_map_path(config, run_path, f"iter_{it + 1}"))
     torch.cuda.synchronize(dev)
     elapsed = time.perf_counter() - t_begin if t_begin is not None else float("nan")
     done = iters - it_begin if t_begin is not None else 0
@@ -186,6 +187,7 @@ def run_shine_mapping_batch(config: SHINEConfig, octree: FeatureOctree, decoder:
 def main(argv=None):
     import argparse
     from . import synth
+    from .checkpoint import apply_load_model
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
     ap.add_argument("config")
     ap.add_argument("--synthetic-azimuth", type=int, default=2048)
@@ -194,12 +196,14 @@ def main(argv=None):
     ap.add_argument("--scans", action="store_true",
                     help="map the sequence of the config's pc_path / pose_path / calib_path instead of synthetic scans")
     ap.add_argument("--run-path", default=None, metavar="DIR",
-                    help="write checkpoints (model/) and meshes (mesh/mesh_iter_*.ply) under DIR")
+                    help="write checkpoints (model/), meshes (mesh/mesh_iter_*.ply) and, with save_map, SDF maps "
+                         "(map/sdf_map_iter_*.ply) under DIR")
     args = ap.parse_args(argv)
     config = SHINEConfig()
     config.load(args.config)
     torch.manual_seed(config.seed)
     octree, decoder = FeatureOctree(config), Decoder(config)
+    octree = apply_load_model(config, octree, decoder)                             # shine_batch.py:45-55
     if args.scans:
         from .scans import LiDARDataset
         print(f"Load, preprocess and sample data ({config.pc_path})")

@@ -1544,6 +1544,7 @@ const char* shine_error_string(int code) {
     if (code == SHINE_OK) return "ok";
     if (code == SHINE_ERR_INVALID_ARG) return "shine_b200: invalid argument";
     if (code == SHINE_ERR_UNSUPPORTED) return "shine_b200: unsupported configuration for the sm_90a kernels";
+    if (code == SHINE_ERR_CAPACITY) return "shine_b200: output buffer too small";
     if (code > 0) return cudaGetErrorString((cudaError_t)code);
     return "shine_b200: unknown error";
 }

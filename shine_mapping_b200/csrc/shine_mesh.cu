@@ -1,5 +1,5 @@
 // shine_mesh.cu — the mesher (reference utils/mesher.py): block-sparse SDF grid, masked marching cubes, vertex normals
-// and the connected-cluster filter.  The grid query is shine_sdf_infer's kernel (shine_internal::launch_sdf_grid);
+// the connected-cluster filter, and the save_map point records.  The grid query is shine_sdf_infer's kernel (shine_internal::launch_sdf_grid);
 // this file holds what follows it.
 
 #include <cuda_runtime.h>
@@ -273,6 +273,59 @@ __global__ void normalize_kernel(float* normals, int64_t nv) {
     if (len > 0.f) { normals[3 * v] = x / len; normals[3 * v + 1] = y / len; normals[3 * v + 2] = z / len; }
 }
 
+// ---- save_map: the owned grid points of a chunk as PLY records (utils/mesher.py:152-173 generate_sdf_map) ------------
+
+struct ExportParams {
+    double origin[3];   // metres, position of grid index lo
+    double voxel;
+    double t[12];       // 3x4, row-major
+    float factor;
+    int masked_only;
+};
+
+// One thread per owned point (i, j, k < n) of the chunk.  A warp's passing points take consecutive records: one ballot,
+// one atomic by the first passing lane.  Records past `capacity` are counted, not written.
+__global__ void __launch_bounds__(256) export_points_kernel(const __grid_constant__ shine_brick_grid g,
+                                                            const __grid_constant__ ExportParams P,
+                                                            uint8_t* __restrict__ records, int64_t capacity,
+                                                            unsigned long long* __restrict__ counter) {
+    const int n = g.n, n1 = n + 1, per = n * n * n;
+    const int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    bool pass = false;
+    int gi[3] = {0, 0, 0};
+    int64_t p = 0;
+    int m = 0;
+    if (q < g.num_bricks * per) {
+        const int64_t b = q / per;
+        const int r = (int)(q - b * per);
+        const int i = r / (n * n), j = (r / n) % n, k = r % n;
+        gi[0] = g.bricks[3 * b] * n + i; gi[1] = g.bricks[3 * b + 1] * n + j; gi[2] = g.bricks[3 * b + 2] * n + k;
+        p = b * (int64_t)(n1 * n1 * n1) + (i * n1 + j) * n1 + k;
+        m = g.mask[p] != 0;
+        pass = gi[0] < g.hi[0] && gi[1] < g.hi[1] && gi[2] < g.hi[2] && (m || !P.masked_only);
+    }
+    const unsigned ballot = __ballot_sync(kFull, pass);
+    if (!ballot) return;
+    const int lane = threadIdx.x & 31, leader = __ffs(ballot) - 1;
+    unsigned long long base = 0;
+    if (lane == leader) base = atomicAdd(counter, (unsigned long long)__popc(ballot));
+    base = __shfl_sync(kFull, base, leader);
+    if (!pass) return;
+    const int64_t row = (int64_t)base + __popc(ballot & ((1u << lane) - 1u));
+    if (row >= capacity) return;
+    double x[3];
+#pragma unroll
+    for (int a = 0; a < 3; ++a) x[a] = __dadd_rn(P.origin[a], __dmul_rn(P.voxel, (double)(gi[a] - g.lo[a])));
+    float* rec = reinterpret_cast<float*>(records + row * 20);
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {   // ((t0 x + t1 y) + t2 z) + t3, every product and sum rounded on its own
+        const double* t = P.t + 4 * a;
+        rec[a] = (float)__dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(t[0], x[0]), __dmul_rn(t[1], x[1])), __dmul_rn(t[2], x[2])), t[3]);
+    }
+    rec[3] = __fmul_rn(g.sdf[p], P.factor);
+    reinterpret_cast<int32_t*>(rec)[4] = m;
+}
+
 int check_grid(const shine_brick_grid* g) {
     if (!g || g->num_bricks < 0 || g->n < 1 || g->n > 64) return SHINE_ERR_INVALID_ARG;
     if (g->num_bricks > 0 && (!g->bricks || !g->sdf || !g->mask)) return SHINE_ERR_INVALID_ARG;
@@ -331,6 +384,36 @@ int shine_marching_cubes(const shine_brick_grid* grid, void* edge_slots, uint32_
         mc_kernel<false><<<blocks_for(cubes), 256, 0, st>>>(*grid, slots, edge_capacity - 1, counters, nullptr, 0,
                                                              nullptr, 0);
     return (int)cudaGetLastError();
+}
+
+int shine_mesh_export_points(const shine_brick_grid* grid, const double* origin_m, double voxel_m, const double* transform,
+                             float sdf_factor, int32_t masked_only, void* records, int64_t capacity, int64_t* counter,
+                             int64_t* count_out, void* stream) {
+    int rc = check_grid(grid);
+    if (rc) return rc;
+    if (!origin_m || !transform || !counter || capacity < 0 || (capacity > 0 && !records)) return SHINE_ERR_INVALID_ARG;
+    if ((uintptr_t)records & 3u) return SHINE_ERR_INVALID_ARG;
+    const int dev = device_of(counter);
+    if (dev < 0 || (capacity > 0 && device_of(records) != dev)) return SHINE_ERR_INVALID_ARG;
+    if (grid->num_bricks > 0 && device_of(grid->sdf) != dev) return SHINE_ERR_INVALID_ARG;
+    DeviceGuard guard(counter);
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (grid->num_bricks > 0) {
+        ExportParams P;
+        for (int a = 0; a < 3; ++a) P.origin[a] = origin_m[a];
+        for (int a = 0; a < 12; ++a) P.t[a] = transform[a];
+        P.voxel = voxel_m; P.factor = sdf_factor; P.masked_only = masked_only != 0;
+        const int64_t owned = grid->num_bricks * (int64_t)grid->n * grid->n * grid->n;
+        export_points_kernel<<<blocks_for(owned), 256, 0, st>>>(*grid, P, static_cast<uint8_t*>(records), capacity,
+                                                                 reinterpret_cast<unsigned long long*>(counter));
+        if (cudaError_t e = cudaGetLastError()) return (int)e;
+    }
+    int64_t count = 0;
+    cudaError_t e = cudaMemcpyAsync(&count, counter, sizeof(count), cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) return (int)e;
+    if (count_out) *count_out = count;
+    return count > capacity ? SHINE_ERR_CAPACITY : SHINE_OK;
 }
 
 int shine_mesh_clusters(const float* verts, int64_t nv, const int32_t* tris, int64_t nt, int32_t min_tris,

@@ -242,6 +242,81 @@ class FeatureOctree(nn.Module):
             self._dict_cache = (corners, nodes)
         return self._dict_cache
 
+    @classmethod
+    def from_lookup_tables(cls, config: SHINEConfig, corners, nodes, hier_features, importance_weight=(),
+                           features_last_frame=()):
+        """The inverse of `_build_dicts`: an octree on `config.device` from the reference's tables (model/feature_octree.py
+        :46-72) — per world level 0..tree_level_world a dict Morton -> row (`corners`) and a dict Morton -> 8 rows
+        (`nodes`), and the feature tables coarse -> fine with their trailing trash row.  Node order is the dicts'
+        insertion order, so the dict views, `get_indices`, the fused kernels and a later `update()` behave as if the map
+        had been grown here.  The tables come from a file: what the kernels would index with is checked, and a
+        violation is a ValueError naming the table."""
+        self = cls(config)
+        dev = self.device
+        if len(corners) != self.max_level + 1 or len(nodes) != self.max_level + 1:
+            raise ValueError(f"corners_lookup_tables / nodes_lookup_tables: {len(corners)} / {len(nodes)} levels, "
+                             f"tree_level_world {self.max_level} needs {self.max_level + 1}")
+        tables = [torch.as_tensor(t).detach() for t in hier_features]
+        if len(tables) not in (0, self.featured_level_num):
+            raise ValueError(f"hier_features: {len(tables)} tables, tree_level_feat is {self.featured_level_num}")
+        for t in tables:
+            self.hier_features.append(nn.Parameter(t.to(dev).clone().contiguous()))
+        for lvl, st in enumerate(self._levels):
+            what = f"level {lvl}"
+            cm = torch.tensor(list(corners[lvl].keys()), dtype=torch.int64).reshape(-1)
+            cr = torch.tensor(list(corners[lvl].values()), dtype=torch.int64).reshape(-1)
+            if not torch.equal(torch.sort(cr).values, torch.arange(cr.numel())):
+                raise ValueError(f"corners_lookup_tables {what}: the rows are not a numbering 0 .. {cr.numel() - 1}")
+            try:
+                nk = torch.tensor(list(nodes[lvl].keys()), dtype=torch.int64).reshape(-1)
+                ni = torch.tensor(list(nodes[lvl].values()), dtype=torch.int64).reshape(nk.numel(), 8)
+            except (ValueError, RuntimeError, TypeError):
+                raise ValueError(f"nodes_lookup_tables {what}: every node holds 8 corner rows") from None
+            if ni.numel() and (int(ni.min()) < -2 ** 31 or int(ni.max()) >= 2 ** 31):
+                raise ValueError(f"nodes_lookup_tables {what}: corner row outside int32")
+            st.node_keys = nk.to(dev)
+            st.node_ids = ni.to(torch.int32).to(dev)
+            by_row = torch.empty(cr.numel(), dtype=torch.int64)
+            by_row[cr] = cm
+            st.corner_morton_by_row = by_row.to(dev)
+            self._refresh_sorted(st)
+        self.check_tables()
+        for name, given in (("importance_weight", importance_weight), ("features_last_frame", features_last_frame)):
+            given = [torch.as_tensor(t).detach() for t in given]
+            if given and [tuple(t.shape) for t in given] != [tuple(p.shape) for p in self.hier_features]:
+                raise ValueError(f"{name}: shapes {[tuple(t.shape) for t in given]} do not match hier_features")
+            setattr(self, name, [t.to(dev).float().clone() for t in given])
+        return self
+
+    def check_tables(self) -> None:
+        """Consistency of the per-level arrays with the feature tables, for a map that arrives from a file: the kernels
+        index the tables with the stored corner rows.  A violation is a ValueError naming the table, not a fault in a
+        kernel.  A stored row is never -1 (what a miss yields) nor the trash row."""
+        if len(self.hier_features) not in (0, self.featured_level_num):
+            raise ValueError(f"hier_features: {len(self.hier_features)} tables, tree_level_feat is {self.featured_level_num}")
+        for lvl, st in enumerate(self._levels):
+            what = f"level {lvl}"
+            k = lvl - self.free_level_num
+            if k < 0 or not len(self.hier_features):
+                if st.node_keys.numel() or st.corner_morton_by_row.numel():
+                    raise ValueError(f"corners_lookup_tables / nodes_lookup_tables {what}: entries at a level without features")
+                continue
+            t = self.hier_features[k]
+            if t.dim() != 2 or t.shape[0] < 1 or t.shape[1] != self.feature_dim or t.dtype != torch.float32:
+                raise ValueError(f"hier_features[{k}]: {t.dtype} {tuple(t.shape)}, expected float32 [rows + 1, "
+                                 f"{self.feature_dim}]")
+            rows = t.shape[0] - 1
+            if st.corner_morton_by_row.numel() != rows:
+                raise ValueError(f"corners_lookup_tables {what}: {st.corner_morton_by_row.numel()} corners for {rows} "
+                                 "feature rows (+ the trash row)")
+            if st.node_keys.dim() != 1 or tuple(st.node_ids.shape) != (st.node_keys.numel(), 8):
+                raise ValueError(f"nodes_lookup_tables {what}: every node holds 8 corner rows")
+            if st.node_keys.numel():
+                if int(st.node_keys.min()) < 0 or int(st.node_keys.max()) >= 8 ** lvl:
+                    raise ValueError(f"nodes_lookup_tables {what}: Morton code outside the level")
+                if int(st.node_ids.min()) < 0 or int(st.node_ids.max()) >= rows:
+                    raise ValueError(f"nodes_lookup_tables {what}: corner row outside [0, {rows})")
+
     @property
     def corners_lookup_tables(self):
         return self._build_dicts()[0]
@@ -270,6 +345,7 @@ class FeatureOctree(nn.Module):
         state["_grad_scratch"] = {}
         state["_last_coord"] = None
         state["_hier_idx"] = []
+        state.pop("_touched_rows", None)   # incre_loop's device scratch (ctypes descriptors): rebuilt on demand
         levels = []
         for st in self._levels:  # device hash tables are rebuilt on demand after unpickling
             cp = _LevelState.__new__(_LevelState)

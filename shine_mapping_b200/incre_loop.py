@@ -134,6 +134,8 @@ def run_shine_mapping_incremental(config: SHINEConfig, octree: FeatureOctree, de
 
     run_path: mesh the map to run_path/mesh/mesh_frame_{frame+1}.ply after the first frame and every mesh_freq_frame
     frames (shine_incre.py:198-211), octree or bbx mode as mc_with_octree selects, transformed by inv(begin_pose_inv).
+    At those frames the map is also saved to run_path/model/model_frame_{frame+1}.pth (batch_loop.save_checkpoint), from
+    which `load_model` continues a run, and with save_map the SDF map goes to run_path/map/sdf_map_frame_{frame+1}.ply.
     map_bbx: a function returning the map's (min, max) metres so far (`lambda: dataset.map_bbx` for real scans, the box
     of the frames' points as in the reference); without it, the box of the surface samples so far; the history entry of such a frame records the file under "mesh"."""
     if pool is not None and config.continual_learning_reg:
@@ -196,11 +198,14 @@ def run_shine_mapping_incremental(config: SHINEConfig, octree: FeatureOctree, de
         if config.ekional_loss_on:
             history[-1].update(eik_first=eik_first, eik_last=eik_last)
         if mesher is not None:
-            from .mesher import reconstruct, surface_bbx
+            from .batch_loop import save_checkpoint
+            from .mesher import reconstruct, sdf_map_path, surface_bbx
             samples_bbx = surface_bbx(coord, weight, config.scale, samples_bbx)
             if fid == 0 or (fid + 1) % config.mesh_freq_frame == 0:
                 history[-1]["mesh"] = os.path.join(run_path, "mesh", f"mesh_frame_{fid + 1}.ply")
-                reconstruct(config, mesher, history[-1]["mesh"], map_bbx() if map_bbx is not None else samples_bbx)
+                reconstruct(config, mesher, history[-1]["mesh"], map_bbx() if map_bbx is not None else samples_bbx,
+                            sdf_map_path(config, run_path, f"frame_{fid + 1}"))
+                save_checkpoint(octree, decoder, trainer, run_path, f"model/model_frame_{fid + 1}", fid)
         if log:
             log(history[-1])
     return history
@@ -210,6 +215,7 @@ def main(argv=None):
     import argparse
     from . import synth
     from .batch_loop import check_supported
+    from .checkpoint import apply_load_model
     ap = argparse.ArgumentParser(description="Incremental mapping on a synthetic drive along +x (regularisation or replay, "
                                              "as the config selects)")
     ap.add_argument("config")
@@ -219,13 +225,20 @@ def main(argv=None):
     ap.add_argument("--iters", type=int, default=None)
     ap.add_argument("--scans", action="store_true",
                     help="map the sequence of the config's pc_path / pose_path / calib_path instead of the synthetic drive")
-    ap.add_argument("--run-path", default=None, metavar="DIR", help="write meshes (mesh/mesh_frame_*.ply) under DIR")
+    ap.add_argument("--run-path", default=None, metavar="DIR",
+                    help="write meshes (mesh/mesh_frame_*.ply), checkpoints (model/model_frame_*.pth) and, with save_map, "
+                         "SDF maps (map/sdf_map_frame_*.ply) under DIR")
     args = ap.parse_args(argv)
     config = SHINEConfig()
     config.load(args.config)
     check_supported(config)
     torch.manual_seed(config.seed)
     octree, decoder = FeatureOctree(config), Decoder(config)
+    octree = apply_load_model(config, octree, decoder)                          # shine_incre.py:44-54
+    if config.continual_learning_reg and not octree.is_empty() and not octree.importance_weight:
+        # a map saved in batch mode carries no regularisation state: begin it as the map's first frame would
+        octree.importance_weight = [torch.zeros_like(p.data) for p in octree.hier_features]
+        octree.features_last_frame = [p.data.clone() for p in octree.hier_features]
     dev = config.device
     # shine_incre.py:106: the regularisation mode keeps the current frame's samples only, the other mode replays
     pool = None if config.continual_learning_reg else synth.ReplayPool(dev)

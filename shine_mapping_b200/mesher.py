@@ -52,17 +52,30 @@ class Mesher:
     # ---- the reference's surface ---------------------------------------------------------------------------------
 
     @torch.no_grad()
-    def recon_octree_mesh(self, query_level: int, mc_res_m: float, mesh_path: str | None = None):
-        """utils/mesher.py:296-368: one n^3 block per octree node at `query_level`."""
+    def recon_octree_mesh(self, query_level: int, mc_res_m: float, mesh_path: str | None = None,
+                          map_path: str | None = None):
+        """utils/mesher.py:296-368: one n^3 block per octree node at `query_level`.  map_path: also write the SDF map, the
+        masked grid points only (the mode the reference leaves commented out, utils/mesher.py:341)."""
         grid = self.octree_grid(query_level, mc_res_m)
-        return self._mesh(grid, OCTREE_MIN_CLUSTER, mesh_path)
+        return self._mesh(grid, OCTREE_MIN_CLUSTER, mesh_path, map_path, True)
 
     @torch.no_grad()
-    def recon_bbx_mesh(self, bbx_min_m, bbx_max_m, mc_res_m: float, mesh_path: str | None = None):
+    def recon_bbx_mesh(self, bbx_min_m, bbx_max_m, mc_res_m: float, mesh_path: str | None = None,
+                       map_path: str | None = None):
         """utils/mesher.py:253-290 with get_query_from_bbx (:110-150): a dense grid over the padded box, of which only
-        the tiles that overlap a node at the coarsest featured level are queried (the others are masked everywhere)."""
+        the tiles that overlap a node at the coarsest featured level are queried (the others are masked everywhere).
+        map_path: also write the SDF map (utils/mesher.py:263-264), every grid point of the queried tiles."""
         grid = self.bbx_grid(bbx_min_m, bbx_max_m, mc_res_m)
-        return self._mesh(grid, self.config.min_cluster_vertices, mesh_path)
+        return self._mesh(grid, self.config.min_cluster_vertices, mesh_path, map_path, False)
+
+    @torch.no_grad()
+    def save_sdf_map(self, grid: dict, map_path: str, masked_only: bool) -> int:
+        """Write the SDF map of `grid` (`octree_grid` / `bbx_grid`) on its own, without a mesh -> number of points."""
+        with SdfMapWriter(self, grid, map_path, masked_only) as out:
+            out.restart()
+            for *_, g in self.chunks(grid):
+                out.add(g)
+        return out.count
 
     # ---- grids -------------------------------------------------------------------------------------------------
 
@@ -158,10 +171,11 @@ class Mesher:
         """First size of the edge table: room for about one vertex per cube on two faces of every brick, at load 1/2."""
         return min(MAX_EDGE_SLOTS, _next_pow2(max(1 << 16, 4 * grid["n"] ** 2 * grid["bricks"].shape[0])))
 
-    def marching_cubes(self, grid: dict):
+    def marching_cubes(self, grid: dict, sdf_map: "SdfMapWriter | None" = None):
         """-> (verts [V,3] fp32 in grid units relative to grid['lo'], faces [T,3] int32), welded, on the device.
         The edge table is kept at most half full (checked after every chunk); past that, or when an insert finds no free
-        slot, the mesh starts over with a table 4x larger."""
+        slot, the mesh starts over with a table 4x larger.  sdf_map receives every chunk in the same pass (the grid is
+        queried once), and starts over with the mesh."""
         dev = grid["bricks"].device
         cap = self.edge_capacity(grid)
         lib, st = _abi.lib(), _abi.stream_ptr(dev)
@@ -170,7 +184,11 @@ class Mesher:
             counters = torch.zeros(4, dtype=torch.int32, device=dev)
             verts = torch.empty(0, 3, dtype=torch.float32, device=dev)
             faces, full = [], False
+            if sdf_map is not None:
+                sdf_map.restart()
             for _, _, _, g in self.chunks(grid):
+                if sdf_map is not None:
+                    sdf_map.add(g)
                 counters[1:3].zero_()
                 _abi.check(lib.shine_marching_cubes(C.byref(g), _abi.ptr(slots), cap, _abi.ptr(counters), None, 0, None, 0,
                                                     st), "shine_marching_cubes")
@@ -193,8 +211,12 @@ class Mesher:
                 raise _abi.ShineB200Error(f"the mesh has more than {MAX_EDGE_SLOTS // 2} vertices (edge table limit)")
             cap = min(MAX_EDGE_SLOTS, cap * 4)
 
-    def _mesh(self, grid: dict, min_tris: int, mesh_path):
-        verts, faces = self.marching_cubes(grid)
+    def _mesh(self, grid: dict, min_tris: int, mesh_path, map_path=None, masked_only=False):
+        if map_path:
+            with SdfMapWriter(self, grid, map_path, masked_only) as out:
+                verts, faces = self.marching_cubes(grid, out)
+        else:
+            verts, faces = self.marching_cubes(grid)
         verts_m = (torch.tensor(grid["origin_m"], dtype=torch.float64, device=verts.device)
                    + verts.double() * grid["voxel_m"])
         normals, keep = normals_and_clusters(verts_m.float(), faces, min_tris)
@@ -206,6 +228,59 @@ class Mesher:
         if mesh_path:
             write_ply(mesh_path, verts_out, faces, normals)
         return verts_out, faces, normals
+
+
+_SDF_MAP_HEADER = ("ply\nformat binary_little_endian 1.0\nelement vertex {:012d}\nproperty float x\nproperty float y\n"
+                   "property float z\nproperty float intensities\nproperty int labels\nend_header\n")
+SDF_MAP_RECORD = np.dtype([("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("intensities", "<f4"), ("labels", "<i4")])
+
+
+class SdfMapWriter:
+    """`save_map` (utils/mesher.py:152-173 generate_sdf_map): the grid points as a binary little-endian PLY point cloud,
+    `intensities` = the SDF in metres (positive in free space, the sign of the reference's sdf_pred), `labels` = the
+    marching-cubes mask, positions transformed by the mesher's global_transform.  `shine_mesh_export_points` compacts each
+    chunk on the device into the file's records; one device-to-host copy per chunk, appended as it is.  The vertex count is
+    a fixed-width header field, patched when the file is closed.  The order of the points is unspecified."""
+
+    def __init__(self, mesher: Mesher, grid: dict, path: str, masked_only: bool):
+        self.grid, self.path, self.masked_only = grid, path, bool(masked_only)
+        cfg = mesher.config
+        self.factor = float(np.float32(cfg.logistic_gaussian_ratio * cfg.sigma_sigmoid_m))     # utils/mesher.py:161
+        self.origin = (C.c_double * 3)(*np.asarray(grid["origin_m"], dtype=np.float64))
+        self.transform = (C.c_double * 12)(*np.asarray(mesher.global_transform, dtype=np.float64)[:3, :4].reshape(-1))
+        self.count, self.fh, self.records = 0, None, None
+        self.counter = torch.zeros(1, dtype=torch.int64, device=grid["bricks"].device)
+
+    def __enter__(self):
+        os.makedirs(os.path.dirname(os.path.abspath(self.path)), exist_ok=True)
+        self.fh = open(self.path, "wb")
+        return self
+
+    def restart(self):
+        self.fh.seek(0)
+        self.fh.truncate()
+        self.fh.write(_SDF_MAP_HEADER.format(0).encode("ascii"))
+        self.count = 0
+
+    def add(self, g: _abi.ShineBrickGrid):
+        owned = g.num_bricks * g.n ** 3
+        if self.records is None or self.records.numel() < owned * SDF_MAP_RECORD.itemsize:
+            self.records = torch.empty(owned * SDF_MAP_RECORD.itemsize, dtype=torch.uint8, device=self.counter.device)
+        self.counter.zero_()
+        n = C.c_int64(0)
+        _abi.check(_abi.lib().shine_mesh_export_points(
+            C.byref(g), self.origin, float(self.grid["voxel_m"]), self.transform, self.factor, int(self.masked_only),
+            _abi.ptr(self.records), owned, _abi.ptr(self.counter), C.byref(n), _abi.stream_ptr(self.counter.device)),
+            "shine_mesh_export_points")
+        self.fh.write(memoryview(self.records[:n.value * SDF_MAP_RECORD.itemsize].cpu().numpy()))
+        self.count += n.value
+
+    def __exit__(self, exc_type, exc, tb):
+        if exc_type is None:
+            self.fh.seek(0)
+            self.fh.write(_SDF_MAP_HEADER.format(self.count).encode("ascii"))
+        self.fh.close()
+        return False
 
 
 def normals_and_clusters(verts: torch.Tensor, faces: torch.Tensor, min_tris: int):
@@ -235,14 +310,20 @@ def compact(verts, faces, normals, keep):
     return verts[used], remap[faces.long()], normals[used]
 
 
-def reconstruct(config: SHINEConfig, mesher: Mesher, mesh_path: str, map_bbx=None):
+def reconstruct(config: SHINEConfig, mesher: Mesher, mesh_path: str, map_bbx=None, map_path: str | None = None):
     """The mesh call of the mapping loops (shine_batch.py:240-245, shine_incre.py:203-211): octree or bbx mode as
-    `mc_with_octree` selects.  map_bbx: (min, max) metres in the map frame, needed by bbx mode."""
+    `mc_with_octree` selects.  map_bbx: (min, max) metres in the map frame, needed by bbx mode.  map_path: the SDF map file
+    of `save_map`, written in the same pass over the grid."""
     if config.mc_with_octree:      # mc_query_level = tree_level_world - tree_level_feat + 1 (utils/config.py:366)
-        return mesher.recon_octree_mesh(mesher.octree.free_level_num, config.mc_res_m, mesh_path)
+        return mesher.recon_octree_mesh(mesher.octree.free_level_num, config.mc_res_m, mesh_path, map_path)
     if map_bbx is None:
         raise ValueError("mc_with_octree: False meshes the map's bounding box: pass map_bbx")
-    return mesher.recon_bbx_mesh(map_bbx[0], map_bbx[1], config.mc_res_m, mesh_path)
+    return mesher.recon_bbx_mesh(map_bbx[0], map_bbx[1], config.mc_res_m, mesh_path, map_path)
+
+
+def sdf_map_path(config: SHINEConfig, run_path: str, name: str) -> str | None:
+    """RUN/map/sdf_map_{name}.ply (shine_batch.py:240, shine_incre.py:204) when `save_map` is on, else None."""
+    return os.path.join(run_path, "map", f"sdf_map_{name}.ply") if config.save_map else None
 
 
 def surface_bbx(coord: torch.Tensor, weight: torch.Tensor, scale: float, bbx=None):
@@ -282,6 +363,22 @@ def write_ply(path: str, verts, faces, normals) -> None:
         fh.write(header.encode("ascii"))
         fh.write(vert.tobytes())
         fh.write(face.tobytes())
+
+
+def read_point_ply(path: str) -> np.ndarray:
+    """The vertex element of a binary little-endian PLY whose first element it is (an SDF map) -> structured array with
+    one field per scalar property (`x`, `y`, `z`, `intensities`, `labels`, ...)."""
+    from .scans import read_ply_header
+    with open(path, "rb") as fh:
+        fmt, elements = read_ply_header(fh, path)
+        if fmt != "binary_little_endian" or not elements or elements[0][0] != "vertex":
+            raise ValueError(f"{path}: expected a binary little-endian PLY that starts with its vertex element")
+        _, n, fields = elements[0]
+        dt = np.dtype([(name, t) for name, t, _ in fields])
+        body = fh.read(n * dt.itemsize)
+    if len(body) != n * dt.itemsize:
+        raise ValueError(f"{path}: file ends inside the vertex element")
+    return np.frombuffer(body, dtype=dt, count=n)
 
 
 def read_ply(path: str):
@@ -350,3 +447,37 @@ def read_ply(path: str):
     if idx.shape[0] and (idx.min() < 0 or idx.max() >= v.shape[0]):
         raise ValueError(f"{path}: face indices outside [0, {v.shape[0]})")
     return v, idx.astype(np.int32).reshape(-1, 3), nrm
+
+
+def main(argv=None):
+    """python -m shine_mapping_b200.mesher CONFIG CHECKPOINT --out MESH.ply: mesh a saved map without the scans."""
+    import argparse
+    from .checkpoint import load_checkpoint
+    ap = argparse.ArgumentParser(description="Mesh a saved map (a checkpoint of either mapping loop, or of the reference). "
+                                             "The checkpoint is unpickled: load only files you trust.")
+    ap.add_argument("config")
+    ap.add_argument("checkpoint")
+    ap.add_argument("--out", required=True, metavar="MESH.ply")
+    ap.add_argument("--mc-res-m", type=float, default=None, help="marching-cubes resolution (default: the config's mc_res_m)")
+    ap.add_argument("--bbx", type=float, nargs=6, default=None, metavar=("X0", "Y0", "Z0", "X1", "Y1", "Z1"),
+                    help="mesh this box (metres, map frame) in bbx mode instead of the octree's nodes")
+    ap.add_argument("--sdf-map", default=None, metavar="MAP.ply", help="also write the SDF map as a point cloud")
+    args = ap.parse_args(argv)
+    config = SHINEConfig()
+    config.load(args.config)
+    state, octree = load_checkpoint(args.checkpoint, config, config.device)
+    if octree is None or octree.is_empty():
+        raise SystemExit(f"{args.checkpoint}: the checkpoint holds a decoder but no map (feature_octree): nothing to mesh")
+    decoder = Decoder(config)
+    decoder.load_state_dict(state)
+    mesher = Mesher(config, octree, decoder)
+    res = config.mc_res_m if args.mc_res_m is None else args.mc_res_m
+    if args.bbx is not None:
+        verts, faces, _ = mesher.recon_bbx_mesh(args.bbx[:3], args.bbx[3:], res, args.out, args.sdf_map)
+    else:
+        verts, faces, _ = mesher.recon_octree_mesh(octree.free_level_num, res, args.out, args.sdf_map)
+    print(f"{args.out}: {verts.shape[0]} vertices, {faces.shape[0]} triangles")
+
+
+if __name__ == "__main__":
+    main()
