@@ -200,10 +200,11 @@ class Mesher:
                     grown = torch.empty(max(nv, 2 * verts.shape[0]), 3, dtype=torch.float32, device=dev)
                     grown[:verts.shape[0]] = verts
                     verts = grown
-                f = torch.empty(nt, 3, dtype=torch.int32, device=dev)
+                # at least one row: a chunk without triangles still passes a triangle buffer (NULL is refused)
+                f = torch.empty(max(nt, 1), 3, dtype=torch.int32, device=dev)
                 _abi.check(lib.shine_marching_cubes(C.byref(g), _abi.ptr(slots), cap, _abi.ptr(counters), _abi.ptr(verts),
                                                     verts.shape[0], _abi.ptr(f), nt, st), "shine_marching_cubes")
-                faces.append(f)
+                faces.append(f[:nt])
             if not full:
                 nv = int(counters[0])
                 return verts[:nv], (torch.cat(faces) if faces else torch.zeros(0, 3, dtype=torch.int32, device=dev))
@@ -219,7 +220,9 @@ class Mesher:
             verts, faces = self.marching_cubes(grid)
         verts_m = (torch.tensor(grid["origin_m"], dtype=torch.float64, device=verts.device)
                    + verts.double() * grid["voxel_m"])
-        normals, keep = normals_and_clusters(verts_m.float(), faces, min_tris)
+        # normals from the grid-unit positions: unit normals do not change under the shift and positive scale to metres,
+        # and fp32 metres at the map's offset would round away the edges of sliver triangles
+        normals, keep = normals_and_clusters(verts, faces, min_tris)
         verts_m, faces, normals = compact(verts_m, faces, normals, keep)
         T = torch.tensor(self.global_transform, dtype=torch.float64, device=verts.device)     # mesh.transform (:284,:362)
         verts_out = (verts_m @ T[:3, :3].T + T[:3, 3]).float()

@@ -7,7 +7,8 @@ corner is inside when its value is below the iso level.  On every face the cross
 that each inside corner is cut off on its own (the saddle rule of the ambiguous faces); the rule depends only on the
 face's four signs, so the two cubes that share a face draw the same segments and the surface is closed.  The segments
 are oriented with the inside on their left seen from outside the cube, chained into loops and each loop is fanned into
-triangles, wound so that the normal (v1 - v0) x (v2 - v0) points from the inside to the outside.
+triangles, wound so that the normal (v1 - v0) x (v2 - v0) points from the inside to the outside.  The fan starts at a
+vertex none of whose diagonals lies in a cube face, so that every edge of the surface is in exactly two triangles.
 """
 from __future__ import annotations
 
@@ -50,6 +51,24 @@ def _faces():
 FACES = _faces()
 
 
+def _on_one_face(e0: int, e1: int) -> bool:
+    """Whether cube edges e0 and e1 lie on a common face of the cube."""
+    a, b = EDGES[e0], EDGES[e1]
+    return any(CORNERS[a[0]][ax] == CORNERS[a[1]][ax] == CORNERS[b[0]][ax] == CORNERS[b[1]][ax] for ax in range(3))
+
+
+def _fan_start(loop):
+    """The loop rotated to start at a vertex from which no diagonal of the fan lies in a cube face.  Such a diagonal
+    joins two crossings of a face that the loop passes twice (a saddle face); when the cube on the other side does the
+    same, the edge is shared by four triangles and the surface is not a manifold there.  Every loop of the table has
+    such a start."""
+    n = len(loop)
+    for r in range(n):
+        if not any(_on_one_face(loop[r], loop[(r + i) % n]) for i in range(2, n - 1)):
+            return loop[r:] + loop[:r]
+    raise AssertionError(f"no fan start without a diagonal in a face: {loop}")
+
+
 def triangulate(case: int):
     inside = [(case >> c) & 1 for c in range(8)]
     nxt = {}
@@ -77,6 +96,7 @@ def triangulate(case: int):
             seen.add(e)
             loop.append(e)
             e = nxt[e]
+        loop = _fan_start(loop)
         for i in range(1, len(loop) - 1):
             tris.append((loop[0], loop[i], loop[i + 1]))
     return tris
@@ -101,7 +121,12 @@ def tables():
     return edge_mask, tri
 
 
-def main():
+HEADER = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "shine_mapping_b200", "csrc",
+                      "shine_mc_table.cuh")
+
+
+def render() -> str:
+    """The text of shine_mc_table.cuh."""
     edge_mask, tri = tables()
     width = 3 * max(len(t) for t in tri) + 1
     lines = ["// shine_mc_table.cuh — generated by tools/gen_mc_table.py (see there for the rules); do not edit.",
@@ -119,11 +144,13 @@ def main():
         flat += [-1] * (width - len(flat))
         lines.append("    {" + ", ".join(str(v) for v in flat) + "},")
     lines.append("};")
-    path = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "shine_mapping_b200", "csrc",
-                        "shine_mc_table.cuh")
-    with open(path, "w") as f:
-        f.write("\n".join(lines) + "\n")
-    print(path, "max triangles per cube:", (width - 1) // 3)
+    return "\n".join(lines) + "\n"
+
+
+def main():
+    with open(HEADER, "w") as f:
+        f.write(render())
+    print(HEADER, "max triangles per cube:", max(len(t) for t in tables()[1]))
 
 
 if __name__ == "__main__":
