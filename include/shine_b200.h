@@ -331,6 +331,23 @@ int shine_scan_sample(const float* points, int64_t n_rays, float ox, float oy, f
                       int32_t surface_n, const float* u_free, int32_t free_n, float surface_range, float free_end,
                       float free_begin_ratio, float* coord, float* label, float* weight, void* stream);
 
+/* ---- one depth image to camera points (dataset/rgbd_to_kitti_format.py: open3d's create_from_color_and_depth and
+ * create_from_rgbd_image) ------------------------------------------------------------------------------------------
+ * Pixel (i, j), i < height, j < width, is depth[i * row_pitch + j] (device uint16, 2-byte aligned).  d = (float)raw /
+ * (float)depth_scale in fp32, set to 0 when (double)d >= depth_trunc.  A pixel with d > 0 gives, in fp64 with every
+ * operation rounded on its own, z = d, x = ((j - cx) * z) / fx, y = ((i - cy) * z) / fy and
+ * xyz_out[i * width + j] = rows 0..2 of camera_pose · (x, y, z, 1) (row-major 4x4, host memory; each row
+ * ((m0 x + m1 y) + m2 z) + m3 · 1; row 3 is not read); every other pixel gives (NaN, NaN, NaN).  xyz_out: device
+ * [height * width, 3] fp64, 8-byte aligned, row-major pixel order, which shine_scan_* take as 24-byte fp64 records (their
+ * filter drops the NaN records).  rgb_out / rgb_in: both NULL, or device uint8 rgb_out[i * width + j] = rgb_in[i *
+ * row_pitch + j] (3 bytes each) for every pixel.  NULL pointers, height or width < 1, row_pitch < width and depth_scale
+ * <= 0 (or not a positive finite fp32) are SHINE_ERR_INVALID_ARG, height * row_pitch > 2^31 - 1 is
+ * SHINE_ERR_UNSUPPORTED; none of them launches.  One launch, no allocation, no synchronisation. */
+int shine_rgbd_backproject(const uint16_t* depth, int32_t height, int32_t width, int32_t row_pitch, double fx,
+                           double fy, double cx, double cy, double depth_scale, double depth_trunc,
+                           const double* camera_pose, double* xyz_out, uint8_t* rgb_out, const uint8_t* rgb_in,
+                           void* stream);
+
 /* ---- the batch-mode sample pool in pinned host memory (more than `pc_count_gpu_limit` scans) ------------------------
  * Replaces the CPU pools of dataset/lidar_dataset.py:94-101 and the CPU-side gather + copy of get_batch (:431-448).
  * Record i is 32 bytes, 32-byte aligned, {x, y, z, label, weight, 0, 0, 0} fp32, at byte (i & (2^chunk_shift - 1)) * 32 of

@@ -168,6 +168,8 @@ SYMBOLS = {
                                                _vp, _vp, _i64, _vp]),
     "shine_scan_sample": (C.c_int, [_vp, _i64, _f32, _f32, _f32, _vp, _i32, _vp, _i32, _f32, _f32, _f32, _vp, _vp, _vp,
                                     _vp]),
+    "shine_rgbd_backproject": (C.c_int, [_vp, _i32, _i32, _i32, C.c_double, C.c_double, C.c_double, C.c_double,
+                                         C.c_double, C.c_double, C.POINTER(C.c_double), _vp, _vp, _vp, _vp]),
     "shine_mesh_grid": (C.c_int, [_OCT, _DEC, C.POINTER(ShineBrickGrid), _i32, _u32, _vp]),
     "shine_marching_cubes": (C.c_int, [C.POINTER(ShineBrickGrid), _vp, _u32, _vp, _vp, _i64, _vp, _i64, _vp]),
     "shine_mesh_export_points": (C.c_int, [C.POINTER(ShineBrickGrid), C.POINTER(C.c_double), C.c_double,

@@ -186,7 +186,7 @@ def run_shine_mapping_batch(config: SHINEConfig, octree: FeatureOctree, decoder:
 
 def main(argv=None):
     import argparse
-    from . import synth
+    from . import rgbd, synth
     from .checkpoint import apply_load_model
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
     ap.add_argument("config")
@@ -198,16 +198,21 @@ def main(argv=None):
     ap.add_argument("--run-path", default=None, metavar="DIR",
                     help="write checkpoints (model/), meshes (mesh/mesh_iter_*.ply) and, with save_map, SDF maps "
                          "(map/sdf_map_iter_*.ply) under DIR")
+    rgbd.add_loop_arguments(ap)
     args = ap.parse_args(argv)
+    rgbd.check_loop_arguments(ap, args)
     config = SHINEConfig()
     config.load(args.config)
     torch.manual_seed(config.seed)
     octree, decoder = FeatureOctree(config), Decoder(config)
     octree = apply_load_model(config, octree, decoder)                             # shine_batch.py:45-55
-    if args.scans:
+    if args.scans or args.rgbd:
         from .scans import LiDARDataset
-        print(f"Load, preprocess and sample data ({config.pc_path})")
-        dataset = LiDARDataset(config, octree)                                      # shine_batch.py:58-76
+        print(f"Load, preprocess and sample data ({args.rgbd or config.pc_path})")
+        if args.rgbd:
+            dataset = rgbd.dataset_from_args(config, args, octree)
+        else:
+            dataset = LiDARDataset(config, octree)                                  # shine_batch.py:58-76
         for frame_id in dataset.used_frames:
             dataset.process_frame(frame_id)
         pool = dataset.pool

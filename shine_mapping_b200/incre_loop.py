@@ -213,7 +213,7 @@ def run_shine_mapping_incremental(config: SHINEConfig, octree: FeatureOctree, de
 
 def main(argv=None):
     import argparse
-    from . import synth
+    from . import rgbd, synth
     from .batch_loop import check_supported
     from .checkpoint import apply_load_model
     ap = argparse.ArgumentParser(description="Incremental mapping on a synthetic drive along +x (regularisation or replay, "
@@ -228,7 +228,9 @@ def main(argv=None):
     ap.add_argument("--run-path", default=None, metavar="DIR",
                     help="write meshes (mesh/mesh_frame_*.ply), checkpoints (model/model_frame_*.pth) and, with save_map, "
                          "SDF maps (map/sdf_map_frame_*.ply) under DIR")
+    rgbd.add_loop_arguments(ap)
     args = ap.parse_args(argv)
+    rgbd.check_loop_arguments(ap, args)
     config = SHINEConfig()
     config.load(args.config)
     check_supported(config)
@@ -243,9 +245,9 @@ def main(argv=None):
     # shine_incre.py:106: the regularisation mode keeps the current frame's samples only, the other mode replays
     pool = None if config.continual_learning_reg else synth.ReplayPool(dev)
     begin_pose_inv = map_bbx = None
-    if args.scans:
+    if args.scans or args.rgbd:
         from .scans import LiDARDataset
-        dataset = LiDARDataset(config)
+        dataset = rgbd.dataset_from_args(config, args) if args.rgbd else LiDARDataset(config)
         frames, begin_pose_inv = dataset.frames(), dataset.begin_pose_inv   # read and sampled one frame at a time
         map_bbx = lambda: dataset.map_bbx
     else:

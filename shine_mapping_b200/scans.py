@@ -92,13 +92,18 @@ def reference_poses(config: SHINEConfig, poses_w: list, total_pc_count: int):
     return poses_ref, begin_pose_inv, used
 
 
-def check_scan_config(config: SHINEConfig) -> None:
+def check_process_config(config: SHINEConfig) -> None:
     """Settings of process_frame that are not implemented raise, naming their key."""
     for key in ("rand_downsample", "filter_noise", "estimate_normal", "behind_dropoff_on", "semantic_on"):
         if getattr(config, key):
             raise NotImplementedError(f"{key}: True is not implemented for real scans")
     if config.clearance_sample_n > 0:
         raise NotImplementedError("clearance_sample_n > 0 is not implemented for real scans")
+
+
+def check_scan_config(config: SHINEConfig) -> None:
+    """check_process_config, and the config's pose file must be a KITTI *.txt file."""
+    check_process_config(config)
     if config.pose_path.endswith("csv"):
         raise NotImplementedError("pose_path: CSV odometry poses are not implemented; use KITTI poses.txt")
     if not config.pose_path.endswith("txt"):
@@ -376,14 +381,18 @@ class LiDARDataset:
     window; otherwise a device SamplePool.  The map cloud (`map_down_pc`) is not kept: it only feeds meshing."""
 
     def __init__(self, config: SHINEConfig, octree=None, pool=None):
-        from . import synth
         check_scan_config(config)
-        self.config = config
-        self.device = torch.device(config.device)
         calib = read_calib_file(config.calib_path) if config.calib_path != "" else {"Tr": np.eye(4)}
         poses_w = read_poses_file(config.pose_path, calib)
         self.pc_filenames = natural_sorted(os.listdir(config.pc_path))
-        self.total_pc_count = len(self.pc_filenames)
+        self._init_frames(config, poses_w, len(self.pc_filenames), octree, pool)
+
+    def _init_frames(self, config: SHINEConfig, poses_w: list, total_pc_count: int, octree, pool):
+        """Frame selection, reference poses, the pool and the GPU scratch: what every frame source shares."""
+        from . import synth
+        self.config = config
+        self.device = torch.device(config.device)
+        self.total_pc_count = total_pc_count
         self.poses_ref, self.begin_pose_inv, self.used_frames = reference_poses(config, poses_w, self.total_pc_count)
         self.used_pc_count = len(self.used_frames)
         self.octree = octree
@@ -402,9 +411,13 @@ class LiDARDataset:
         """dataset/lidar_dataset.py:175: the frame's sensor origin in scaled coordinates, numpy fp64."""
         return self.poses_ref[frame_id][:3, 3] * self.config.scale
 
+    def read_frame(self, frame_id: int) -> ScanRecords:
+        """The frame's point records, in pinned host or device memory."""
+        return read_scan(os.path.join(self.config.pc_path, self.pc_filenames[frame_id]))
+
     def frame_samples(self, frame_id: int):
         """Read, preprocess and sample one scan -> (coord, sdf_label, weight, origin_scaled fp32 tensor, points)."""
-        rec = read_scan(os.path.join(self.config.pc_path, self.pc_filenames[frame_id]))
+        rec = self.read_frame(frame_id)
         points = self.processor.points(rec, self.poses_ref[frame_id])
         origin = torch.tensor(self.origin_scaled(frame_id), dtype=torch.float32)
         coord, label, weight = self.processor.sample(points, origin.numpy())
