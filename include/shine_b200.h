@@ -50,6 +50,8 @@ extern "C" {
                                          neighbouring points then share nodes, and the step sums the gradients of each run of
                                          equal node on the tensor cores before ONE red per corner row (results equal up to
                                          fp32 summation order); on an unordered batch the flag only costs time           */
+#define SHINE_FLAG_LOSS_L2 32u         /* shine_sdf_diff_*: sdf_diff_loss with l2_loss=True (main_loss_type sdf_l2); without
+                                         it the loss is L1 (sdf_l1).  The other shine_sdf_* calls refuse the bit          */
 
 /* One featured level of the FeatureOctree (model/feature_octree.py:46-63). */
 typedef struct shine_level {
@@ -151,6 +153,21 @@ int shine_sdf_bce_step(const shine_octree* oct, const shine_decoder* dec, const 
                        const float* label, const float* weight, int64_t n, float sigma, float loss_scale,
                        const float* d_loss, float* out_pred, float* out_loss, uint32_t flags, void* stream);
 
+/* The same forward and training step with the reference's other point-wise losses, sdf_diff_loss (utils/loss.py:6-14,
+ * shine_batch.py:171-179; main_loss_type sdf_l1 / sdf_l2):
+ *   diff_m = (pred - label) / scale;   L = sum |weight| |diff_m|   (L1)   or   sum |weight| diff_m^2   (SHINE_FLAG_LOSS_L2)
+ * scale = config.scale (1 / world_size), positive and finite; weight [n] is required (its magnitude is always applied);
+ * loss_scale multiplies every per-point term (1 / the global batch size, the reference's count).  out_loss is ACCUMULATED
+ * (+=).  flags: SHINE_FLAG_TF32X1, SHINE_FLAG_LOSS_L2 and, for the step, SHINE_FLAG_MORTON_ORDERED; any other bit (also
+ * REDUCTION_SUM and WEIGHTED, which sdf_diff_loss does not have) is SHINE_ERR_UNSUPPORTED.  Other arguments as in
+ * shine_sdf_bce_fwd / shine_sdf_bce_step. */
+int shine_sdf_diff_fwd(const shine_octree* oct, const shine_decoder* dec, const float* coord,
+                       const float* label, const float* weight, int64_t n, float scale, float loss_scale,
+                       float* out_pred, float* out_loss, uint32_t flags, void* stream);
+int shine_sdf_diff_step(const shine_octree* oct, const shine_decoder* dec, const float* coord,
+                        const float* label, const float* weight, int64_t n, float scale, float loss_scale,
+                        const float* d_loss, float* out_pred, float* out_loss, uint32_t flags, void* stream);
+
 /* feature_grads[l] += sum of grad_replicas[l][r]; grad_replicas[l] = 0.  No-op for levels without
  * replicas.  Part of the backward (the reference's index_put_ is one pass, shine_batch.py:209). */
 int shine_reduce_grad_replicas(const shine_octree* oct, void* stream);
@@ -232,6 +249,14 @@ int shine_sdf_bce_eikonal_step(const shine_octree* oct, const shine_decoder* dec
                                const float* label, const float* weight, int64_t n, float sigma, float loss_scale,
                                float weight_e, const int32_t* n_surface, float* out_pred, float* out_grad,
                                float* out_loss, float* out_eikonal, uint32_t flags, void* stream);
+/* The same step with sdf_diff_loss in place of the BCE term (see shine_sdf_diff_step): L = sdf_diff_loss(pred, label) +
+ * weight_e * mean_{weight > 0} (1 - |g|)^2, g = sigma * d pred / d coord as above (sigma = sigma_sigmoid, whatever the
+ * loss).  |weight| always multiplies the sdf_diff_loss term; flags: SHINE_FLAG_TF32X1 (accepted, the kernel is fp32
+ * throughout) and SHINE_FLAG_LOSS_L2, any other bit is SHINE_ERR_UNSUPPORTED.  out_loss (+=) the sdf_diff_loss part. */
+int shine_sdf_diff_eikonal_step(const shine_octree* oct, const shine_decoder* dec, const float* coord,
+                                const float* label, const float* weight, int64_t n, float scale, float sigma,
+                                float loss_scale, float weight_e, const int32_t* n_surface, float* out_pred,
+                                float* out_grad, float* out_loss, float* out_eikonal, uint32_t flags, void* stream);
 
 /* ---- continual-learning terms of the incremental loop (BASELINE config 4) ---------------------------------------
  * The reference finds the rows a batch touched with `hierarchical_indices[i].flatten().unique()` (a sort per level

@@ -21,6 +21,7 @@ FLAG_REDUCTION_SUM = 1
 FLAG_WEIGHTED = 2
 FLAG_TF32X1 = 4
 FLAG_MORTON_ORDERED = 16
+FLAG_LOSS_L2 = 32
 ERR_CAPACITY = -3
 
 
@@ -128,6 +129,8 @@ SYMBOLS = {
     "shine_sdf_infer": (C.c_int, [_OCT, _DEC, _vp, _i64, _vp, _vp, _i32, _u32, _vp]),
     "shine_sdf_bce_fwd": (C.c_int, [_OCT, _DEC, _vp, _vp, _vp, _i64, _f32, _f32, _vp, _vp, _u32, _vp]),
     "shine_sdf_bce_step": (C.c_int, [_OCT, _DEC, _vp, _vp, _vp, _i64, _f32, _f32, _vp, _vp, _vp, _u32, _vp]),
+    "shine_sdf_diff_fwd": (C.c_int, [_OCT, _DEC, _vp, _vp, _vp, _i64, _f32, _f32, _vp, _vp, _u32, _vp]),
+    "shine_sdf_diff_step": (C.c_int, [_OCT, _DEC, _vp, _vp, _vp, _i64, _f32, _f32, _vp, _vp, _vp, _u32, _vp]),
     "shine_reduce_grad_replicas": (C.c_int, [_OCT, _vp]),
     "shine_octree_frame_nodes": (C.c_int, [C.POINTER(ShineBuild), _vp, _i64, _vp]),
     "shine_octree_frame_corners": (C.c_int, [C.POINTER(ShineBuild), _i32, _vp]),
@@ -138,6 +141,8 @@ SYMBOLS = {
     "shine_octree_corner_rehash": (C.c_int, [_vp, _u32, _vp, _i64, _vp]),
     "shine_count_positive": (C.c_int, [_vp, _i64, _vp, _vp]),
     "shine_sdf_bce_eikonal_step": (C.c_int, [_OCT, _DEC, _vp, _vp, _vp, _i64, _f32, _f32, _f32, _vp, _vp, _vp, _vp, _vp, _u32, _vp]),
+    "shine_sdf_diff_eikonal_step": (C.c_int, [_OCT, _DEC, _vp, _vp, _vp, _i64, _f32, _f32, _f32, _f32, _vp, _vp, _vp, _vp,
+                                              _vp, _u32, _vp]),
     "shine_mark_touched": (C.c_int, [_OCT, _vp, _i64, C.POINTER(ShineTouched), _vp]),
     "shine_regularization_apply": (C.c_int, [_OCT, C.POINTER(ShineTouched), C.POINTER(ShineRowTables), _f32, _vp, _i32, _vp]),
     "shine_importance_accumulate": (C.c_int, [_OCT, C.POINTER(ShineTouched), C.POINTER(ShineRowTables), _i32, _i32, _vp]),

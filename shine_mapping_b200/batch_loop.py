@@ -7,12 +7,14 @@ from all frames, set up the optimiser, then `iters` x { lr decay -> get_batch ->
 checkpoint in the reference's format.  What differs: the body of an iteration is TWO launches (the fused
 `shine_sdf_bce_step` kernel and the multi-tensor Adam kernel, which also re-zeroes the gradients) instead of
 ~300, and there is no host round trip inside the loop (loss is read back only when logging).
+`main_loss_type` is the reference's point-wise menu (shine_batch.py:171-179): sdf_bce, or sdf_l1 / sdf_l2
+(`sdf_diff_loss`, fused as `shine_sdf_diff_step`), each with or without the eikonal term.
 
 Out of scope here (SURVEY.md §2): dataset I/O (open3d), meshing, visualiser, wandb.  `pool` is anything with the
 `get_batch(bs)` contract of LiDARDataset (dataset/lidar_dataset.py:431-448); `synth.build_scene_map` provides one.
-`ekional_loss_on` is one fused kernel (`shine_sdf_bce_eikonal_step`; the class surface supports the reference's
-autograd recipe too: query_feature is differentiable w.r.t. the coordinates, twice); normal / consistency / semantic /
-ray losses are rejected explicitly.
+`ekional_loss_on` is one fused kernel (`shine_sdf_bce_eikonal_step` / `shine_sdf_diff_eikonal_step`; the class surface
+supports the reference's autograd recipe too: query_feature is differentiable w.r.t. the coordinates, twice); normal /
+consistency / semantic / ray losses are rejected explicitly.
 """
 from __future__ import annotations
 
@@ -29,12 +31,17 @@ from .feature_octree import FeatureOctree
 from .trainer import SdfTrainer
 
 
-def check_supported(config: SHINEConfig) -> None:
+BATCH_LOSSES = ("sdf_bce", "sdf_l1", "sdf_l2")
+
+
+def check_supported(config: SHINEConfig, main_losses=BATCH_LOSSES) -> None:
+    """Raise NotImplementedError for a config this package cannot train.  main_losses: the main_loss_type values the
+    calling loop trains (the batch loop: BATCH_LOSSES; the incremental loop only sdf_bce)."""
     unsupported = [k for k in ("normal_loss_on", "consistency_loss_on", "proj_correction_on",
                                "semantic_on", "time_conditioned", "ray_loss") if getattr(config, k)]
-    if unsupported or config.main_loss_type != "sdf_bce":
-        raise NotImplementedError(
-            f"implemented: main_loss_type=sdf_bce (+ ekional_loss_on); not {unsupported or config.main_loss_type}")
+    if unsupported or config.main_loss_type not in main_losses:
+        raise NotImplementedError(f"implemented: main_loss_type={'/'.join(main_losses)} (+ ekional_loss_on); "
+                                  f"not {unsupported or config.main_loss_type}")
     if not config.opt_adam:
         raise NotImplementedError("only Adam (reference utils/tools.py:78-79) is implemented")
 
@@ -68,14 +75,17 @@ def eikonal_iteration(config: SHINEConfig, octree: FeatureOctree, decoder: Decod
     `query_feature` is differentiable w.r.t. the coordinates (shine_query_coord_grad) and that gradient is itself
     differentiable (tangent kernels), so the reference's get_gradient(create_graph=True) recipe works as is.  Gradients
     accumulate into the trainer's flat buffer (param.grad are views of it)."""
-    from .loss import sdf_bce_loss
+    from .loss import sdf_bce_loss, sdf_diff_loss
     sigma = config.sigma_sigmoid
     coord = coord.detach().requires_grad_(True)
     feature = octree.query_feature(coord)
     pred = decoder.sdf(feature)
     g = torch.autograd.grad(pred, coord, torch.ones_like(pred), create_graph=True, retain_graph=True)[0] * sigma
     surface_mask = weight > 0
-    loss = sdf_bce_loss(pred, sdf_label, sigma, torch.abs(weight), config.loss_weight_on, config.loss_reduction)
+    if config.main_loss_type == "sdf_bce":
+        loss = sdf_bce_loss(pred, sdf_label, sigma, torch.abs(weight), config.loss_weight_on, config.loss_reduction)
+    else:                                                                         # shine_batch.py:176-179
+        loss = sdf_diff_loss(pred, sdf_label, torch.abs(weight), config.scale, l2_loss=config.main_loss_type == "sdf_l2")
     eikonal = ((1.0 - g[surface_mask].norm(2, dim=-1)) ** 2).mean()
     total = loss + config.weight_e * eikonal
     total.backward()

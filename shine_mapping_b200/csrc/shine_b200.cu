@@ -541,12 +541,13 @@ struct GridCoords {         // the points of a shine_internal::BrickGrid, genera
 template <class Src>
 constexpr int infer_min_blocks() { return std::is_same<Src, BatchCoords>::value ? SHINE_INFER_MINB : 2; }
 
-template <int NTF, bool TRAIN, bool DEC_GRAD, int LMAX, bool GROUPED = false, class Src = BatchCoords>
+template <int NTF, bool TRAIN, bool DEC_GRAD, int LMAX, bool GROUPED = false, class Src = BatchCoords, int LOSS = kLossBce>
 __global__ void __launch_bounds__(256, !TRAIN ? infer_min_blocks<Src>() : (DEC_GRAD && !GROUPED) ? SHINE_TRAIN_DECGRAD_MINB : SHINE_TRAIN_MINB)
 sdf_fused_kernel(const __grid_constant__ StepParams P, const __grid_constant__ Src src) {
     static_assert(std::is_same<Src, BatchCoords>::value || !TRAIN, "generated coordinates are for inference only");
     static_assert(!GROUPED || TRAIN, "the grouped scatter belongs to the training kernels");
     static_assert(!DEC_GRAD || TRAIN, "decoder gradients belong to the training kernels");
+    static_assert(LOSS == kLossBce || std::is_same<Src, BatchCoords>::value, "the loss belongs to labelled batches");
     static_assert(SmemPlan::kStagePerWarp >= SmemPlan::kDecGradFloats, "a warp's staging area holds its partial decoder gradient");
     static_assert(SmemPlan::kStageGrouped >= kH * kF + 3 * kH + 1, "a grouped warp's staging area holds its partial bias / dW1 gradients");
     static_assert(!(GROUPED && DEC_GRAD) ||
@@ -665,16 +666,23 @@ sdf_fused_kernel(const __grid_constant__ StepParams P, const __grid_constant__ S
     int phase = 0;                          // 0: virtual forward, 1: this warp's tiles, 2: virtual backward (warp 0)
     bool advance = false, last_pass = false;
     float pred0 = 0.f, zsum = 0.f;
-    auto bce_point = [&](float pv, float lb, float wg, float& li, float& dp) {
-        // MUFU-based exp / log / reciprocal (~2 ulp): |d loss| <~ 1e-7, far inside the 2e-5 parity tolerance
-        const float zt = __fdividef(1.0f, 1.0f + __expf(-__fdividef(lb, P.sigma)));   // sigmoid(label / sigma)
-        const float e = __expf(-fabsf(pv));
-        li = fmaxf(pv, 0.f) - pv * zt + __logf(1.0f + e);                               // log1p(e), e in (0, 1]
-        dp = 0.f;
-        if (TRAIN) {
-            const float rs = __fdividef(1.0f, 1.0f + e);
-            const float sg = pv >= 0.f ? rs : e * rs;                                   // sigmoid(pred)
-            dp = (sg - zt) * wg * smem[SmemPlan::GSCALE];
+    // one sample's loss term li (the caller weights it) and dL/dpred dp (weighted and scaled)
+    auto loss_point = [&](float pv, float lb, float wg, float& li, float& dp) {
+        if constexpr (LOSS == kLossBce) {
+            // MUFU-based exp / log / reciprocal (~2 ulp): |d loss| <~ 1e-7, far inside the 2e-5 parity tolerance
+            const float zt = __fdividef(1.0f, 1.0f + __expf(-__fdividef(lb, P.sigma)));   // sigmoid(label / sigma)
+            const float e = __expf(-fabsf(pv));
+            li = fmaxf(pv, 0.f) - pv * zt + __logf(1.0f + e);                               // log1p(e), e in (0, 1]
+            dp = 0.f;
+            if (TRAIN) {
+                const float rs = __fdividef(1.0f, 1.0f + e);
+                const float sg = pv >= 0.f ? rs : e * rs;                                   // sigmoid(pred)
+                dp = (sg - zt) * wg * smem[SmemPlan::GSCALE];
+            }
+        } else {
+            float dli;
+            diff_point<LOSS>(pv, lb, P.scale, li, dli);
+            dp = TRAIN ? dli * wg * smem[SmemPlan::GSCALE] : 0.f;
         }
     };
     for (int seq = warp_global;; seq = advance ? seq + warp_stride : seq) {
@@ -873,7 +881,7 @@ sdf_fused_kernel(const __grid_constant__ StepParams P, const __grid_constant__ S
             if (P.pred && half == 0 && valid) P.pred[myp] = src.out(pred0);
             if (P.label != nullptr && valid) {
                 float li, dpz;
-                bce_point(pred0, lab, wgt, li, dpz);
+                loss_point(pred0, lab, wgt, li, dpz);
                 if (half == 0) { loss_acc += wgt * li; zsum += dpz; }
             }
             continue;
@@ -970,11 +978,11 @@ sdf_fused_kernel(const __grid_constant__ StepParams P, const __grid_constant__ S
 
         if (P.label == nullptr) continue;   // pure inference
 
-        // ---- sdf_bce_loss (utils/loss.py:17-24) + dL/dpred ---------------------------------------------
+        // ---- sdf_bce_loss (utils/loss.py:17-24) or sdf_diff_loss (:6-14) + dL/dpred -------------------------
         float dpo = 0.f;
         if (valid) {
             float li;
-            bce_point(pown, lab, wgt, li, dpo);
+            loss_point(pown, lab, wgt, li, dpo);
             if (half == 0) loss_acc += wgt * li;
         }
         if (!TRAIN) continue;
@@ -1420,9 +1428,9 @@ int check_decoder(const shine_decoder* d, const shine_octree* o) {
     return SHINE_OK;
 }
 
-template <int NTF, bool TRAIN, bool DEC_GRAD, int LMAX, bool GROUPED = false, class Src = BatchCoords>
+template <int NTF, bool TRAIN, bool DEC_GRAD, int LMAX, bool GROUPED = false, class Src = BatchCoords, int LOSS = kLossBce>
 int launch_fused_t(const StepParams& P, cudaStream_t st, const Src& src = Src()) {
-    auto kern = sdf_fused_kernel<NTF, TRAIN, DEC_GRAD, LMAX, GROUPED, Src>;
+    auto kern = sdf_fused_kernel<NTF, TRAIN, DEC_GRAD, LMAX, GROUPED, Src, LOSS>;
     const int smem_floats = SmemPlan::STAGE + (DEC_GRAD ? 8 * SmemPlan::stage_per_warp(GROUPED) : 0) +
                             (GROUPED ? 8 * (LMAX * SmemPlan::kGroupPerLevel + (DEC_GRAD ? SmemPlan::kW2Part : kTile * kF)) : 0);
     const size_t smem_bytes = (size_t)smem_floats * sizeof(float);
@@ -1458,21 +1466,31 @@ int launch_fused_t(const StepParams& P, cudaStream_t st, const Src& src = Src())
     return (int)cudaGetLastError();
 }
 
-template <bool TRAIN, bool DEC_GRAD, class Src = BatchCoords>
+template <bool TRAIN, bool DEC_GRAD, class Src = BatchCoords, int LOSS = kLossBce>
 int launch_fused(const StepParams& P, uint32_t flags, cudaStream_t st, const Src& src = Src()) {
     const bool x1 = (flags & SHINE_FLAG_TF32X1) != 0;
     const bool small = P.oct.num_levels <= 4;
     if constexpr (TRAIN) {      // Morton-ordered batches: voxel-grouped scatter (3xTF32, up to 4 levels; else the general kernel)
-        if ((flags & SHINE_FLAG_MORTON_ORDERED) && !x1 && small) return launch_fused_t<3, TRAIN, DEC_GRAD, 4, true>(P, st);
+        if ((flags & SHINE_FLAG_MORTON_ORDERED) && !x1 && small)
+            return launch_fused_t<3, TRAIN, DEC_GRAD, 4, true, Src, LOSS>(P, st);
     }
-    if (x1) return small ? launch_fused_t<1, TRAIN, DEC_GRAD, 4, false, Src>(P, st, src)
-                         : launch_fused_t<1, TRAIN, DEC_GRAD, 8, false, Src>(P, st, src);
-    return small ? launch_fused_t<3, TRAIN, DEC_GRAD, 4, false, Src>(P, st, src)
-                 : launch_fused_t<3, TRAIN, DEC_GRAD, 8, false, Src>(P, st, src);
+    if (x1) return small ? launch_fused_t<1, TRAIN, DEC_GRAD, 4, false, Src, LOSS>(P, st, src)
+                         : launch_fused_t<1, TRAIN, DEC_GRAD, 8, false, Src, LOSS>(P, st, src);
+    return small ? launch_fused_t<3, TRAIN, DEC_GRAD, 4, false, Src, LOSS>(P, st, src)
+                 : launch_fused_t<3, TRAIN, DEC_GRAD, 8, false, Src, LOSS>(P, st, src);
+}
+
+// the sdf_diff_loss step and forward: the per-sample loss (L1 / L2) picks the kernels
+template <bool TRAIN, bool DEC_GRAD>
+int launch_diff(const StepParams& P, uint32_t flags, cudaStream_t st) {
+    return (flags & SHINE_FLAG_LOSS_L2) ? launch_fused<TRAIN, DEC_GRAD, BatchCoords, kLossL2>(P, flags, st)
+                                        : launch_fused<TRAIN, DEC_GRAD, BatchCoords, kLossL1>(P, flags, st);
 }
 
 // the flag bits of the shine_sdf_* calls: any other bit is SHINE_ERR_UNSUPPORTED, never silently ignored
 constexpr uint32_t kSdfFlags = SHINE_FLAG_REDUCTION_SUM | SHINE_FLAG_WEIGHTED | SHINE_FLAG_TF32X1 | SHINE_FLAG_MORTON_ORDERED;
+// the flag bits of the shine_sdf_diff_* calls: reduction and weighting are fixed by sdf_diff_loss (weighted sum / count)
+constexpr uint32_t kDiffFlags = SHINE_FLAG_TF32X1 | SHINE_FLAG_MORTON_ORDERED | SHINE_FLAG_LOSS_L2;
 
 int fill_params(StepParams& P, const shine_octree* oct, const shine_decoder* dec, const float* coord, int64_t n) {
     if (n < 0 || (n > 0 && !coord)) return SHINE_ERR_INVALID_ARG;
@@ -1480,7 +1498,7 @@ int fill_params(StepParams& P, const shine_octree* oct, const shine_decoder* dec
     P.oct = *oct; P.dec = *dec; P.coord = coord; P.n = n;
     P.num_tiles = (int32_t)((n + kTile - 1) / kTile);
     P.label = nullptr; P.weight = nullptr; P.d_loss = nullptr; P.pred = nullptr; P.loss = nullptr; P.mask = nullptr;
-    P.mask_level = 0; P.sigma = 1.f; P.loss_scale = 1.f; P.weighted = 0;
+    P.mask_level = 0; P.sigma = 1.f; P.loss_scale = 1.f; P.weighted = 0; P.scale = 1.f;
     return SHINE_OK;
 }
 
@@ -1698,6 +1716,49 @@ int shine_sdf_bce_step(const shine_octree* oct, const shine_decoder* dec, const 
     P.sigma = sigma; P.loss_scale = loss_scale; P.d_loss = d_loss; P.pred = out_pred; P.loss = out_loss;
     return dec_grad ? launch_fused<true, true>(P, flags, (cudaStream_t)stream)
                     : launch_fused<true, false>(P, flags, (cudaStream_t)stream);
+}
+
+int shine_sdf_diff_fwd(const shine_octree* oct, const shine_decoder* dec, const float* coord, const float* label,
+                       const float* weight, int64_t n, float scale, float loss_scale, float* out_pred, float* out_loss,
+                       uint32_t flags, void* stream) {
+    if (flags & ~(kDiffFlags & ~SHINE_FLAG_MORTON_ORDERED)) return SHINE_ERR_UNSUPPORTED;
+    int rc = check_octree(oct, false);
+    if (rc) return rc;
+    rc = check_decoder(dec, oct);
+    if (rc) return rc;
+    if (!weight || (n > 0 && !label) || !valid_scale(scale)) return SHINE_ERR_INVALID_ARG;
+    StepParams P;
+    rc = fill_params(P, oct, dec, coord, n);
+    if (rc) return rc;
+    if (n == 0) return SHINE_OK;
+    if ((rc = check_same_device(oct, coord))) return rc;
+    DeviceGuard guard(oct->lv[0].features);
+    P.label = label; P.weight = weight; P.weighted = 1;          // shine_batch.py:172 |weight|, always applied
+    P.scale = scale; P.loss_scale = loss_scale; P.pred = out_pred; P.loss = out_loss;
+    return launch_diff<false, false>(P, flags, (cudaStream_t)stream);
+}
+
+int shine_sdf_diff_step(const shine_octree* oct, const shine_decoder* dec, const float* coord, const float* label,
+                        const float* weight, int64_t n, float scale, float loss_scale, const float* d_loss,
+                        float* out_pred, float* out_loss, uint32_t flags, void* stream) {
+    if (flags & ~kDiffFlags) return SHINE_ERR_UNSUPPORTED;
+    int rc = check_octree(oct, true);
+    if (rc) return rc;
+    rc = check_decoder(dec, oct);
+    if (rc) return rc;
+    if (!weight || (n > 0 && !label) || !valid_scale(scale)) return SHINE_ERR_INVALID_ARG;
+    const bool dec_grad = dec->gw1 || dec->gw2 || dec->gw3;
+    if (dec_grad && !(dec->gw1 && dec->gw2 && dec->gw3)) return SHINE_ERR_INVALID_ARG;
+    StepParams P;
+    rc = fill_params(P, oct, dec, coord, n);
+    if (rc) return rc;
+    if (n == 0) return SHINE_OK;
+    if ((rc = check_same_device(oct, coord))) return rc;
+    DeviceGuard guard(oct->lv[0].features);
+    P.label = label; P.weight = weight; P.weighted = 1;
+    P.scale = scale; P.loss_scale = loss_scale; P.d_loss = d_loss; P.pred = out_pred; P.loss = out_loss;
+    return dec_grad ? launch_diff<true, true>(P, flags, (cudaStream_t)stream)
+                    : launch_diff<true, false>(P, flags, (cudaStream_t)stream);
 }
 
 int shine_reduce_grad_replicas(const shine_octree* oct, void* stream) {

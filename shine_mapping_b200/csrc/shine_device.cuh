@@ -28,6 +28,7 @@ struct StepParams {
     float sigma;
     float loss_scale;
     int32_t weighted;
+    float scale;             // sdf_diff_loss (L1 / L2 steps): config.scale, map units per metre
 };
 
 // The mesher's block-sparse grid (shine_mesh.cu): point p of a query is point r = p % (n+1)^3 of brick b = p / (n+1)^3,
@@ -471,5 +472,29 @@ inline int check_same_device(const shine_octree* o, const void* batch_ptr) {
     const int d = device_of(batch_ptr);
     return (d >= 0 && d != device_of(o->lv[0].features)) ? SHINE_ERR_INVALID_ARG : SHINE_OK;
 }
+
+// The per-sample loss of the training kernels, a template parameter: sdf_bce_loss (utils/loss.py:17-24), or sdf_diff_loss
+// (utils/loss.py:6-14) with l2_loss False (L1) or True (L2).
+enum SdfLoss : int { kLossBce = 0, kLossL1 = 1, kLossL2 = 2 };
+
+// One sample of sdf_diff_loss with diff_m = (pred - label) / scale (back to metres): the unweighted term li (|diff_m| or
+// diff_m^2) and its derivative with respect to pred (sign(diff_m) / scale, torch's sign(0) = 0, or 2 diff_m / scale).
+// IEEE divisions as torch rounds them.  (A product with a rounded 1 / scale was tried: the Morton-ordered training kernel
+// then spills 12 bytes instead of the BCE kernel's 4.)
+template <int LOSS>
+__device__ __forceinline__ void diff_point(float pv, float lb, float scale, float& li, float& dli) {
+    static_assert(LOSS == kLossL1 || LOSS == kLossL2, "sdf_diff_loss is L1 or L2");
+    const float dm = __fdiv_rn(__fsub_rn(pv, lb), scale);
+    if (LOSS == kLossL2) {
+        li = __fmul_rn(dm, dm);
+        dli = __fdiv_rn(__fmul_rn(2.0f, dm), scale);
+    } else {
+        li = fabsf(dm);
+        dli = __fdiv_rn(dm > 0.f ? 1.0f : (dm < 0.f ? -1.0f : 0.0f), scale);
+    }
+}
+
+// the sdf_diff_loss entries: the scale a caller passes must be a positive finite number
+inline bool valid_scale(float scale) { return scale > 0.f && scale <= 3.402823466e38f; }
 
 }  // namespace

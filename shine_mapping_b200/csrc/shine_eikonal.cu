@@ -31,11 +31,12 @@ struct EikParams {
     const int32_t* n_surface;  // device scalar: number of samples with weight > 0
     float* pred;               // nullable
     float* grad_out;           // nullable [n,3]: g
-    float* loss;               // += BCE part
+    float* loss;               // += BCE (or sdf_diff_loss) part
     float* eikonal;            // += sum_surface (1-|g|)^2 / N_surf
     int64_t n;
     float sigma, loss_scale, weight_e;
     int32_t weighted;
+    float scale;               // sdf_diff_loss: config.scale
 };
 
 constexpr int kTS = 36;     // row stride (floats) of the per-warp [component][point] tiles: conflict-free for the
@@ -55,7 +56,7 @@ struct EikSmem {
     static constexpr int FLOATS = TILES + kEW * kPerWarp;
 };
 
-template <bool DEC_GRAD>
+template <bool DEC_GRAD, int LOSS = kLossBce>
 __global__ void __launch_bounds__(kET, 2) sdf_eikonal_kernel(const __grid_constant__ EikParams P) {
     extern __shared__ __align__(16) float sm[];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -178,14 +179,21 @@ __global__ void __launch_bounds__(kET, 2) sdf_eikonal_kernel(const __grid_consta
         }
         if (P.pred && valid) P.pred[p] = pr;
 
-        // ---- sdf_bce_loss (utils/loss.py:17-24) and dL_bce/dpred ----------------------------------------------------------
+        // ---- sdf_bce_loss (utils/loss.py:17-24) or sdf_diff_loss (:6-14) and its dL/dpred --------------------------------
         float dp = 0.f;
         if (valid) {
-            const float zt = __fdividef(1.0f, 1.0f + __expf(-__fdividef(lab, P.sigma)));
-            const float e = __expf(-fabsf(pr));
-            loss_acc += wgt * (fmaxf(pr, 0.f) - pr * zt + __logf(1.0f + e));
-            const float rs = __fdividef(1.0f, 1.0f + e);
-            dp = ((pr >= 0.f ? rs : e * rs) - zt) * wgt * P.loss_scale;
+            if constexpr (LOSS == kLossBce) {
+                const float zt = __fdividef(1.0f, 1.0f + __expf(-__fdividef(lab, P.sigma)));
+                const float e = __expf(-fabsf(pr));
+                loss_acc += wgt * (fmaxf(pr, 0.f) - pr * zt + __logf(1.0f + e));
+                const float rs = __fdividef(1.0f, 1.0f + e);
+                dp = ((pr >= 0.f ? rs : e * rs) - zt) * wgt * P.loss_scale;
+            } else {
+                float li, dli;
+                diff_point<LOSS>(pr, lab, P.scale, li, dli);
+                loss_acc += wgt * li;
+                dp = dli * wgt * P.loss_scale;
+            }
         }
 
         // ---- a1 = D1 W2^T a2,  q = W1^T a1 = dpred/dfeature -----------------------------------------------------------------
@@ -378,9 +386,9 @@ __global__ void count_positive_kernel(const float* __restrict__ w, int64_t n, in
     if ((threadIdx.x & 31) == 0 && local) atomicAdd(out, local);
 }
 
-template <bool DEC_GRAD>
+template <bool DEC_GRAD, int LOSS = kLossBce>
 int launch_eikonal(const EikParams& P, cudaStream_t st) {
-    auto kern = sdf_eikonal_kernel<DEC_GRAD>;
+    auto kern = sdf_eikonal_kernel<DEC_GRAD, LOSS>;
     const size_t bytes = (size_t)EikSmem::FLOATS * sizeof(float);
     static int ready[kMaxDevices] = {0};
     int& done = ready[current_device()];
@@ -433,6 +441,35 @@ int shine_sdf_bce_eikonal_step(const shine_octree* oct, const shine_decoder* dec
     P.sigma = sigma; P.loss_scale = loss_scale; P.weight_e = weight_e;
     P.weighted = (flags & SHINE_FLAG_WEIGHTED) ? 1 : 0;
     return dec_grad ? launch_eikonal<true>(P, (cudaStream_t)stream) : launch_eikonal<false>(P, (cudaStream_t)stream);
+}
+
+int shine_sdf_diff_eikonal_step(const shine_octree* oct, const shine_decoder* dec, const float* coord, const float* label,
+                                const float* weight, int64_t n, float scale, float sigma, float loss_scale, float weight_e,
+                                const int32_t* n_surface, float* out_pred, float* out_grad, float* out_loss,
+                                float* out_eikonal, uint32_t flags, void* stream) {
+    if (flags & ~(SHINE_FLAG_TF32X1 | SHINE_FLAG_LOSS_L2)) return SHINE_ERR_UNSUPPORTED;
+    int rc = check_octree(oct, true);
+    if (rc) return rc;
+    if (!dec) return SHINE_ERR_INVALID_ARG;
+    if (dec->in_dim != kF || dec->hidden != kH || dec->mlp_level != 2 || oct->feature_dim != kF) return SHINE_ERR_UNSUPPORTED;
+    if (!dec->w1 || !dec->w2 || !dec->w3) return SHINE_ERR_INVALID_ARG;
+    if (!weight || n < 0 || (n > 0 && (!coord || !label || !n_surface))) return SHINE_ERR_INVALID_ARG;
+    if (!(sigma > 0.f) || !valid_scale(scale)) return SHINE_ERR_INVALID_ARG;
+    const bool dec_grad = dec->gw1 || dec->gw2 || dec->gw3;
+    if (dec_grad && !(dec->gw1 && dec->gw2 && dec->gw3)) return SHINE_ERR_INVALID_ARG;
+    if (n == 0) return SHINE_OK;
+    if ((rc = check_same_device(oct, coord))) return rc;
+    DeviceGuard guard(oct->lv[0].features);
+    EikParams P;
+    P.oct = *oct; P.dec = *dec; P.coord = coord; P.label = label; P.weight = weight; P.n_surface = n_surface;
+    P.pred = out_pred; P.grad_out = out_grad; P.loss = out_loss; P.eikonal = out_eikonal; P.n = n;
+    P.sigma = sigma; P.loss_scale = loss_scale; P.weight_e = weight_e;
+    P.weighted = 1;                                       // shine_batch.py:172 |weight|, always applied
+    P.scale = scale;
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (flags & SHINE_FLAG_LOSS_L2)
+        return dec_grad ? launch_eikonal<true, kLossL2>(P, st) : launch_eikonal<false, kLossL2>(P, st);
+    return dec_grad ? launch_eikonal<true, kLossL1>(P, st) : launch_eikonal<false, kLossL1>(P, st);
 }
 
 }  // extern "C"

@@ -1,5 +1,6 @@
 """The fused hot path: reference shine_batch.py:123 (`query_feature`) + :128 (`Decoder.sdf`) + :174
-(`sdf_bce_loss`) + :209 (`backward`) as ONE sm_90a kernel launch (`shine_sdf_bce_step`).
+(`sdf_bce_loss`) + :209 (`backward`) as ONE sm_90a kernel launch (`shine_sdf_bce_step`); `sdf_diff_step` is the same
+with the reference's other point-wise losses (:176-179, `sdf_diff_loss`, main_loss_type sdf_l1 / sdf_l2).
 
 `sdf_bce_step(...)` returns the loss with autograd attached.  Because the loss gradient of a sample depends only
 on that sample, the kernel computes forward, loss AND the full backward (table scatter-add + decoder grads) in one
@@ -135,6 +136,94 @@ def sdf_bce_step(octree: FeatureOctree, decoder: Decoder, coord, sdf_label, sigm
     loss, pred = _SdfBce.apply(octree, decoder, coord, sdf_label, weight, float(sigma), bool(weighted),
                                bce_reduction, n_norm, single_pass,
                                (_abi.FLAG_TF32X1 if tf32x1 else 0) | (_abi.FLAG_MORTON_ORDERED if morton_ordered else 0), *params)
+    return (loss, pred) if return_pred else loss
+
+
+class _SdfDiff(torch.autograd.Function):
+    """`_SdfBce` with sdf_diff_loss (`shine_sdf_diff_fwd` / `shine_sdf_diff_step`)."""
+
+    @staticmethod
+    def forward(ctx, octree, decoder, coord, label, weight, scale, flags, n_norm, single_pass, *params):
+        L = octree.featured_level_num
+        tables, dparams = params[:L], params[L:]
+        n = coord.shape[0]
+        dev = coord.device
+        lib = _abi.lib()
+        stream = _abi.stream_ptr(dev)
+        loss_scale = 1.0 / float(n_norm if n_norm else n)         # utils/loss.py:7,12-14: sum / count
+        pred = torch.empty(n, dtype=torch.float32, device=dev)
+        loss = torch.zeros((), dtype=torch.float32, device=dev)
+        need_t = [bool(x) for x in ctx.needs_input_grad[9:9 + L]]
+        need_d = [bool(x) for x in ctx.needs_input_grad[9 + L:]]
+        want_grad = any(need_t) or any(need_d)
+        ctx.octree, ctx.decoder = octree, decoder
+        ctx.cfg = (scale, loss_scale, flags, n, need_t, need_d)
+        if want_grad and single_pass:
+            tgrads = [torch.zeros_like(p) for p in tables]
+            dgrads = [torch.zeros_like(p) if (p is not None and any(need_d)) else None for p in dparams]
+            od = octree._descriptor(tables, tgrads)
+            dd = decoder.c_descriptor(dgrads if any(need_d) else None)
+            _abi.check(lib.shine_sdf_diff_step(C.byref(od), C.byref(dd), _abi.ptr(coord), _abi.ptr(label), _abi.ptr(weight),
+                                               n, scale, loss_scale, None, _abi.ptr(pred), _abi.ptr(loss), flags, stream),
+                       "shine_sdf_diff_step")
+            ctx.stash = (tgrads, dgrads)
+        else:
+            od = octree._descriptor(tables, None)
+            dd = decoder.c_descriptor(None)
+            _abi.check(lib.shine_sdf_diff_fwd(C.byref(od), C.byref(dd), _abi.ptr(coord), _abi.ptr(label), _abi.ptr(weight),
+                                              n, scale, loss_scale, _abi.ptr(pred), _abi.ptr(loss),
+                                              flags & ~_abi.FLAG_MORTON_ORDERED, stream), "shine_sdf_diff_fwd")
+            ctx.stash = None
+            if want_grad:
+                ctx.save_for_backward(coord, label, weight, *params)
+        ctx.mark_non_differentiable(pred)
+        return loss, pred
+
+    @staticmethod
+    def backward(ctx, dloss, _dpred):
+        scale, loss_scale, flags, n, need_t, need_d = ctx.cfg
+        octree, decoder = ctx.octree, ctx.decoder
+        L = octree.featured_level_num
+        if ctx.stash is not None:
+            tgrads, dgrads = ctx.stash
+            ctx.stash = None
+            for g in list(tgrads) + [g for g in dgrads if g is not None]:
+                g.mul_(dloss)
+        else:
+            coord, label, weight, *params = ctx.saved_tensors
+            tables, dparams = params[:L], params[L:]
+            tgrads = [torch.zeros_like(p) for p in tables]
+            dgrads = [torch.zeros_like(p) if (p is not None and any(need_d)) else None for p in dparams]
+            od = octree._descriptor(tables, tgrads)
+            dd = decoder.c_descriptor(dgrads if any(need_d) else None)
+            dl = dloss.detach().float().contiguous()
+            _abi.check(_abi.lib().shine_sdf_diff_step(
+                C.byref(od), C.byref(dd), _abi.ptr(coord), _abi.ptr(label), _abi.ptr(weight), n, scale, loss_scale,
+                _abi.ptr(dl), None, None, flags, _abi.stream_ptr(coord.device)), "shine_sdf_diff_step")
+        out_t = [g if need else None for g, need in zip(tgrads, need_t)]
+        out_d = [g if need else None for g, need in zip(dgrads, need_d)]
+        return (None,) * 9 + tuple(out_t) + tuple(out_d)
+
+
+def sdf_diff_step(octree: FeatureOctree, decoder: Decoder, coord, sdf_label, weight, scale, l2_loss=True, n_norm=None,
+                  single_pass=True, tf32x1=False, return_pred=False, morton_ordered=False):
+    """loss (= sdf_diff_loss(decoder.sdf(octree.query_feature(coord)), sdf_label, |weight|, scale, l2_loss), the
+    reference's main_loss_type sdf_l2 / sdf_l1) with autograd to `octree.hier_features` and the decoder parameters.
+
+    weight: the per-sample weights (required; their magnitude always multiplies the loss).  scale: config.scale.
+    n_norm: the loss's count (defaults to len(coord); pass the GLOBAL batch when sharding points).  The other arguments
+    as in `sdf_bce_step`."""
+    if coord.requires_grad:
+        raise NotImplementedError("gradients w.r.t. coordinates are not part of the fused sm_90a path")
+    if weight is None:
+        raise ValueError("sdf_diff_step needs the per-sample weight tensor")
+    coord, sdf_label, weight = _prep(coord, "coord"), _prep(sdf_label, "sdf_label"), _prep(weight, "weight")
+    flags = (_abi.FLAG_LOSS_L2 if l2_loss else 0) | (_abi.FLAG_TF32X1 if tf32x1 else 0) | \
+            (_abi.FLAG_MORTON_ORDERED if morton_ordered else 0)
+    params = list(octree.hier_features) + list(decoder.fused_params())
+    octree._last_coord, octree._hier_idx = coord, []
+    loss, pred = _SdfDiff.apply(octree, decoder, coord, sdf_label, weight, float(scale), flags, n_norm, single_pass,
+                                *params)
     return (loss, pred) if return_pred else loss
 
 

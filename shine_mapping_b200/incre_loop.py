@@ -164,7 +164,8 @@ def run_shine_mapping_incremental(config: SHINEConfig, octree: FeatureOctree, de
         octree.update(surface, incremental_on=config.continual_learning_reg)        # lidar_dataset.py:212-218
         if pool is not None:
             pool.add_frame(coord, label, weight, frame[3], window)                  # lidar_dataset.py:235-271
-        trainer = SdfTrainer(config, octree, decoder)                               # fresh Adam state per frame
+        # fresh Adam state per frame; sdf_bce whatever main_loss_type says, as the reference's shine_incre.py:150
+        trainer = SdfTrainer(config, octree, decoder, main_loss_type="sdf_bce")
         dev = trainer.flat_grad.device
         trainer.zero_grad()
         first = last = None
@@ -233,7 +234,7 @@ def main(argv=None):
     rgbd.check_loop_arguments(ap, args)
     config = SHINEConfig()
     config.load(args.config)
-    check_supported(config)
+    check_supported(config, main_losses=("sdf_bce",))   # shine_incre.py:150 trains sdf_bce whatever main_loss_type says
     torch.manual_seed(config.seed)
     octree, decoder = FeatureOctree(config), Decoder(config)
     octree = apply_load_model(config, octree, decoder)                          # shine_incre.py:44-54

@@ -5,7 +5,8 @@ One flat fp32 gradient buffer holds every table level and the decoder (each segm
   * zeroing the gradients is ONE memset (or free: fused into the Adam kernel),
   * the data-parallel exchange is ONE NCCL all-reduce over NVLink (decoder 1 377 floats + table rows),
   * `param.grad` of every parameter is a view into it, so stock torch optimizers still work.
-`forward_backward()` = one `shine_sdf_bce_step` launch; `optimizer_step()` = one `shine_adam_step` launch with the
+`forward_backward()` = one `shine_sdf_bce_step` launch (`shine_sdf_diff_step` with main_loss_type sdf_l1 / sdf_l2);
+`optimizer_step()` = one `shine_adam_step` launch with the
 reference's grouping (utils/tools.py:57-83: Adam betas (0.9, 0.99), eps 1e-15, weight decay on the decoder only,
 per-level lr scaled leaf -> coarse by lr_level_reduce_ratio).
 """
@@ -26,11 +27,22 @@ def _align4(n: int) -> int:
     return (n + 3) & ~3
 
 
+def diff_loss_flags(main_loss_type: str):
+    """main_loss_type -> None for sdf_bce, else the loss bit of the shine_sdf_diff_* calls (sdf_l1: 0, sdf_l2:
+    FLAG_LOSS_L2; shine_batch.py:176-179)."""
+    kinds = {"sdf_bce": None, "sdf_l1": 0, "sdf_l2": _abi.FLAG_LOSS_L2}
+    if main_loss_type not in kinds:
+        raise NotImplementedError(f"main_loss_type {main_loss_type!r}: the trainer has {sorted(kinds)}")
+    return kinds[main_loss_type]
+
+
 class SdfTrainer:
     def __init__(self, config: SHINEConfig, octree: FeatureOctree, decoder: Decoder, process_group=None,
                  tf32x1: bool = False, shard_mode: str = "replicated", boundary=None, comm=None, p2p=None,
-                 morton_ordered: bool = False):
-        """shard_mode (multi-GPU, see dist.py / partition.py): "replicated" = every rank holds the whole table and a
+                 morton_ordered: bool = False, main_loss_type: str | None = None):
+        """main_loss_type: the loss every step trains, None = config.main_loss_type (the incremental loop passes
+        "sdf_bce": the reference's shine_incre.py:150 trains it whatever the config says).
+        shard_mode (multi-GPU, see dist.py / partition.py): "replicated" = every rank holds the whole table and a
         slice of the point batch -> all-reduce the whole flat gradient; "spatial" = every rank owns a Morton-prefix
         range of ONE map and the samples inside it (BASELINE config 5) -> ONE all-reduce over
         [decoder gradients | gradients of the corner rows shared with other ranks] (`boundary`: partition.BoundaryPlan).
@@ -51,6 +63,8 @@ class SdfTrainer:
         self.step_count = 0
         self._sig = None
         self.sigma = config.sigma_sigmoid
+        self.main_loss_type = config.main_loss_type if main_loss_type is None else main_loss_type
+        self._diff = diff_loss_flags(self.main_loss_type)   # None: sdf_bce
         self._sync()
 
     # ---- flat buffers --------------------------------------------------------------------------------------
@@ -124,6 +138,9 @@ class SdfTrainer:
         self._sync()
         cfg = self.config
         n = coord.shape[0]
+        diff = self._diff
+        if diff is not None and weight is None:
+            raise ValueError(f"main_loss_type {self.main_loss_type} needs the per-sample weight tensor")
         weighted = bool(cfg.loss_weight_on) if weighted is None else bool(weighted)
         if weighted and weight is None:
             raise ValueError("loss_weight_on needs the per-sample weight tensor")
@@ -139,10 +156,17 @@ class SdfTrainer:
         if not accumulate_loss and not self._loss_clean:
             self.loss.zero_()
         self._loss_clean = False
-        _abi.check(_abi.lib().shine_sdf_bce_step(
-            C.byref(od), C.byref(dd), _abi.ptr(coord), _abi.ptr(sdf_label),
-            _abi.ptr(weight) if weighted else None, n, float(self.sigma), scale, None,
-            _abi.ptr(pred_out), _abi.ptr(self.loss), flags, _abi.stream_ptr(coord.device)), "shine_sdf_bce_step")
+        if diff is None:
+            _abi.check(_abi.lib().shine_sdf_bce_step(
+                C.byref(od), C.byref(dd), _abi.ptr(coord), _abi.ptr(sdf_label),
+                _abi.ptr(weight) if weighted else None, n, float(self.sigma), scale, None,
+                _abi.ptr(pred_out), _abi.ptr(self.loss), flags, _abi.stream_ptr(coord.device)), "shine_sdf_bce_step")
+        else:   # sdf_diff_loss: always weighted, divided by the batch size whatever loss_reduction says
+            flags = diff | (flags & (_abi.FLAG_TF32X1 | _abi.FLAG_MORTON_ORDERED))
+            _abi.check(_abi.lib().shine_sdf_diff_step(
+                C.byref(od), C.byref(dd), _abi.ptr(coord), _abi.ptr(sdf_label), _abi.ptr(weight), n, float(cfg.scale),
+                1.0 / float(n_norm if n_norm else n), None, _abi.ptr(pred_out), _abi.ptr(self.loss), flags,
+                _abi.stream_ptr(coord.device)), "shine_sdf_diff_step")
         if mid_event is not None:          # lets a profiler time the fused kernel and the replica fold separately
             mid_event.record()
         if replicas:
@@ -154,7 +178,8 @@ class SdfTrainer:
         """The step with `ekional_loss_on` (reference shine_batch.py:119-142,172-185,208-209) as ONE launch
         (`shine_sdf_bce_eikonal_step`): BCE + weight_e * mean over surface samples of (1 - |sigma d pred/d coord|)^2,
         gradients of both terms accumulated into the flat buffer.  -> (bce loss, eikonal mean) device scalars;
-        the loop's total loss is bce + config.weight_e * eikonal.
+        the loop's total loss is bce + config.weight_e * eikonal.  With main_loss_type sdf_l1 / sdf_l2 the first term is
+        sdf_diff_loss (`shine_sdf_diff_eikonal_step`) and the first scalar its value.
         n_surface: denominator of the eikonal mean, the analogue of n_norm: the number of surface samples (weight > 0) in
         the GLOBAL batch when this call sees one part of it.  None = counted on the device from this batch and, when the
         trainer runs on several ranks, summed over them, so that the per-rank eikonal values and gradients add up to those
@@ -187,10 +212,18 @@ class SdfTrainer:
                 total = count.float()                 # exact below 2^24 samples; the collectives here sum fp32
                 self._all_reduce(total)
                 count.copy_(total.round())
-        _abi.check(lib.shine_sdf_bce_eikonal_step(
-            C.byref(od), C.byref(dd), _abi.ptr(coord), _abi.ptr(sdf_label), _abi.ptr(weight), n, float(self.sigma), scale,
-            float(cfg.weight_e), _abi.ptr(count), _abi.ptr(pred_out), _abi.ptr(grad_out), _abi.ptr(self.loss),
-            _abi.ptr(eik), flags, st), "shine_sdf_bce_eikonal_step")
+        diff = self._diff
+        if diff is None:
+            _abi.check(lib.shine_sdf_bce_eikonal_step(
+                C.byref(od), C.byref(dd), _abi.ptr(coord), _abi.ptr(sdf_label), _abi.ptr(weight), n, float(self.sigma), scale,
+                float(cfg.weight_e), _abi.ptr(count), _abi.ptr(pred_out), _abi.ptr(grad_out), _abi.ptr(self.loss),
+                _abi.ptr(eik), flags, st), "shine_sdf_bce_eikonal_step")
+        else:
+            _abi.check(lib.shine_sdf_diff_eikonal_step(
+                C.byref(od), C.byref(dd), _abi.ptr(coord), _abi.ptr(sdf_label), _abi.ptr(weight), n, float(cfg.scale),
+                float(self.sigma), 1.0 / float(n_norm if n_norm else n), float(cfg.weight_e), _abi.ptr(count),
+                _abi.ptr(pred_out), _abi.ptr(grad_out), _abi.ptr(self.loss), _abi.ptr(eik), diff, st),
+                "shine_sdf_diff_eikonal_step")
         return self.loss, eik.view(())
 
     def _all_reduce(self, buf):
@@ -317,6 +350,10 @@ class SdfTrainer:
             self.all_reduce_grads()
             self.optimizer_step(zero_grad=False, device_step=True)
 
+    def _uses_weight(self) -> bool:
+        """Whether the steps read the per-sample weights: sdf_bce with loss_weight_on, sdf_l1 / sdf_l2 always."""
+        return bool(self.config.loss_weight_on) or self._diff is not None
+
     # ---- pipelined host-buffer entry ------------------------------------------------------------------------
 
     class StepGraph:
@@ -383,7 +420,7 @@ class SdfTrainer:
         own inputs and reads its own result; only the waiting is overlapped."""
         dev = self.flat_grad.device
         n = coord_h.shape[0]
-        weighted = bool(self.config.loss_weight_on) and weight_h is not None
+        weighted = self._uses_weight() and weight_h is not None
         self._sync()
         pl = getattr(self, "_pipe", None)
         if pl is None or pl["cap"] < n or pl["sig"] != self._sig:
@@ -437,7 +474,7 @@ class SdfTrainer:
         pays a fixed ~20 us of kernel prologue/epilogue per slice)."""
         dev = self.flat_grad.device
         n = coord_h.shape[0]
-        weighted = bool(self.config.loss_weight_on) and weight_h is not None
+        weighted = self._uses_weight() and weight_h is not None
         self._sync()
         if getattr(self, "_h2d", None) is None or self._h2d[0].shape[0] < n:
             self._h2d = (torch.empty(n, 3, device=dev), torch.empty(n, device=dev), torch.empty(n, device=dev))
