@@ -34,6 +34,17 @@ def diff_dpred(pred, label, weight, scale, l2_loss, count, sign=None):
     return weight * s / scale / count
 
 
+def l1_sign(pred, label, got_pred, atol, rtol):
+    """The L1 sign per sample for grading an fp32 kernel: sign(pred - label) of the oracle's pred, and the sign of the
+    kernel's own difference (0 where its pred equals the label) where |pred - label| <= atol + rtol |pred|: there either
+    side of the label is right."""
+    pred, label = np.asarray(pred, np.float64), np.asarray(label)
+    near = np.abs(pred - label) <= atol + rtol * np.abs(pred)
+    sign = np.sign(pred - label)
+    sign[near] = np.sign(np.asarray(got_pred, np.float32)[near] - label[near])
+    return sign
+
+
 def _promote(octree, dec, coord, label, weight):
     octree.hier_features = [f.detach().double().requires_grad_(True) for f in octree.hier_features]
     dec = {k: v.detach().double().requires_grad_(True) for k, v in dec.items()}

@@ -215,17 +215,36 @@ def _eikonal_case(levels, poly, seed, weighted=False, reduction="mean", scale=1.
     return sort_case_morton(case) if ordered else case
 
 
-def _eik_weight(case):
-    return 100.0 * (case["coord"].shape[0] if case["cfg"]["reduction"] == "sum" else 1)
+def _eik_weight(case, want=None):
+    """sdf_bce: 100 (x N with the sum).  sdf_l1 / sdf_l2 (want: the oracle's outputs at weight_e = 0.1) put every sample's
+    full-size dL/dpred into the first term, whose gradients reach 10^5 x the eikonal ones on x300 tables with L2: there
+    W = 100 x the largest ratio of the two maxima (at least 100), so that the floor of the eikonal-only grading,
+    1e-5 max|first| / W, stays at about 1e-4 of its 1e-3 bar."""
+    if want is None:
+        return 100.0 * (case["coord"].shape[0] if case["cfg"]["reduction"] == "sum" else 1)
+    ratio = 1.0
+    for tot, eik in _grad_pairs(want):
+        if np.abs(eik).max() > 0:
+            ratio = max(ratio, float(np.abs(tot - 0.1 * eik).max() / np.abs(eik).max()))
+    return 100.0 * ratio
 
 
-def _oracle_eikonal(case, weight_e=0.1, n_surface=None):
-    from oracle import shine_oracle as orc
+def _grad_pairs(want):
+    """(total, eikonal-only) gradient pairs of an oracle result: table levels without the trash row, then the decoder."""
+    pairs = [(t[:-1], e[:-1]) for t, e in zip(want["table_grads"], want["eik_table_grads"])]
+    return pairs + [(want["dec_grads"][k], want["eik_dec_grads"][k]) for k in want["eik_dec_grads"]]
+
+
+def _oracle_eikonal(case, weight_e=0.1, n_surface=None, loss_type="sdf_bce", l1_sign=None):
+    """loss_type sdf_l1 / sdf_l2: the first term is sdf_diff_loss (tests/sdf_diff_oracle.py); l1_sign as there."""
+    from tests import sdf_diff_oracle as sdo
     from tests.parity_utils import oracle_from_case
+    from tests.test_gpu_sdf_diff import _scale
     o, odec = oracle_from_case(case)
     c = case["cfg"]
-    r = orc.train_step_eikonal(o, odec, torch.from_numpy(case["coord"]), torch.from_numpy(case["label"]),
-                               torch.from_numpy(case["weight"]), c["sigma"], weight_e, c["weighted"], c["reduction"], n_surface)
+    r = sdo.train_step_eikonal(o, odec, torch.from_numpy(case["coord"]), torch.from_numpy(case["label"]),
+                               torch.from_numpy(case["weight"]), c["sigma"], weight_e, c["weighted"], c["reduction"],
+                               n_surface, loss_type=loss_type, scale=_scale(case), l1_sign=l1_sign)
     out = {k: float(r[k]) for k in ("loss", "bce", "eikonal")}
     out.update(g=r["g"].numpy(), pred=r["pred"].numpy(), table_grads=[t.numpy() for t in r["table_grads"]],
                eik_table_grads=[t.numpy() for t in r["eik_table_grads"]],
@@ -239,14 +258,14 @@ def _grads(tr, frozen):
             {} if frozen else {k: g.cpu().numpy().copy() for k, g in zip(DEC_KEYS, tr.dec_grads) if g is not None})
 
 
-def _fused_eikonal_runs(case, weights=None, frozen=False, outs=True):
+def _fused_eikonal_runs(case, weights=None, frozen=False, outs=True, loss_type="sdf_bce"):
     """The fused step (SdfTrainer.forward_backward_eikonal, one launch) at each weight_e, on one trainer."""
     from shine_mapping_b200 import SdfTrainer
     cfg, octree, dec = build_cuda_models(case, DEV, freeze_decoder=frozen)
     coord = torch.from_numpy(case["coord"]).to(DEV); label = torch.from_numpy(case["label"]).to(DEV)
     weight = torch.from_numpy(case["weight"]).to(DEV)
     n = coord.shape[0]
-    tr = SdfTrainer(cfg, octree, dec)
+    tr = SdfTrainer(cfg, octree, dec, main_loss_type=loss_type)
     runs = {}
     for w in weights or (0.1, 0.0, _eik_weight(case)):
         cfg.weight_e = w
@@ -285,10 +304,11 @@ def _class_surface_eikonal_runs(case):
     return runs
 
 
-def _check_eikonal(runs, want, weight_e=0.1):
+def _check_eikonal(runs, want, weight_e=0.1, floor_share=None):
     """runs: {weight_e: outputs} at weight_e, 0 and W.  want: the oracle's (or a golden's) outputs at weight_e with the
     eikonal mean's own gradients.  Asserts parity; returns a line with the worst deviations, each relative to the
-    maximum it is graded against (bars: 1e-4 for g / eikonal / loss, 1e-3 for the gradients)."""
+    maximum it is graded against (bars: 1e-4 for g / eikonal / loss, 1e-3 for the gradients).  floor_share: the largest
+    share of its bar the floor of an eikonal-only gradient may take (a first term that swamps the eikonal one fails)."""
     big = max(runs)
     tot, r0, r1 = runs[weight_e], runs[0.0], runs[big]
     worst = {}
@@ -300,6 +320,10 @@ def _check_eikonal(runs, want, weight_e=0.1):
         assert d <= bound * scale + floor, f"{name}: max|d| {d:.3e} > {bound:g} x {scale:.3e} + {floor:.1e}"
         if scale > 0:        # lout.bias has no eikonal part: graded by the floor alone
             worst[name.split(" ")[0]] = max(worst.get(name.split(" ")[0], 0.0), d / scale)
+            if floor_share is not None and name.startswith("eik_"):
+                share = floor / (bound * scale)
+                assert share <= floor_share, f"{name}: the floor is {share:.2e} of the bar (W = {big:g} is too small)"
+                worst["floor/bar"] = max(worst.get("floor/bar", 0.0), share)
 
     if tot["g"] is not None:
         rel("g", tot["g"], want["g"], 1e-4, 1e-7)
@@ -416,40 +440,102 @@ def test_fused_eikonal_step_matches_oracle(levels, poly, weighted, reduction, sc
           _check_eikonal(_fused_eikonal_runs(case, frozen=frozen, outs=outs), want))
 
 
+DIFF_LOSSES = ("sdf_l1", "sdf_l2")
+
+
+def _diff_eikonal_runs(case, loss_type, frozen=False, outs=True):
+    """The fused sdf_l1 / sdf_l2 + eikonal step (shine_sdf_diff_eikonal_step) at weight_e = 0.1, 0 and W = _eik_weight(case,
+    oracle), graded by _check_eikonal with the floor at most 0.1 of its bar.  The L1 oracle takes the kernel's sign near
+    the label from a run with pred_out (the kernel's pred does not depend on the outputs asked for, so runs without
+    them are graded against the same oracle).  -> (runs, oracle, report line with N, surface count and eikonal share)."""
+    from tests import sdf_diff_oracle as sdo
+    want = _oracle_eikonal(case, loss_type=loss_type)
+    big = _eik_weight(case, want)
+    runs = _fused_eikonal_runs(case, (0.1, 0.0, big), frozen, outs, loss_type)
+    if loss_type == "sdf_l1":
+        pred = runs[0.1]["pred"] if outs else _fused_eikonal_runs(case, (0.1,), frozen, True, loss_type)[0.1]["pred"]
+        want = _oracle_eikonal(case, loss_type=loss_type, l1_sign=sdo.l1_sign(want["pred"], case["label"], pred, 2e-5, 1e-5))
+    if frozen:
+        want["dec_grads"], want["eik_dec_grads"] = {}, {}
+    share = [0.1 * np.abs(e).max() / np.abs(t).max() for t, e in _grad_pairs(want) if np.abs(e).max() > 0] or [0.0]
+    line = (f"{loss_type} N={case['coord'].shape[0]} surface={int((case['weight'] > 0).sum())} W={big:.3g} "
+            f"eikonal share {min(share):.1e}..{max(share):.1e} " + _check_eikonal(runs, want, floor_share=0.1))
+    return runs, want, line
+
+
+DIFF_EIKONAL_CASES = [   # levels, poly, scale, n, ordered, frozen, bias, outs, seed
+    pytest.param(1, True, 1.0, None, False, False, True, True, 201, id="L1"),
+    pytest.param(2, True, 300.0, None, False, False, True, True, 202, id="L2-x300"),
+    pytest.param(3, False, 1.0, None, False, False, True, True, 203, id="L3-linear"),
+    pytest.param(4, True, 300.0, None, False, False, True, True, 204, id="L4-x300"),
+    pytest.param(6, False, 300.0, None, False, False, True, True, 206, id="L6-linear-x300"),
+    pytest.param(8, True, 300.0, None, False, False, True, True, 208, id="L8-x300"),
+    pytest.param(4, True, 300.0, None, False, True, True, True, 214, id="L4-frozen-x300"),
+    pytest.param(3, True, 300.0, None, False, False, False, True, 223, id="L3-nobias-x300"),
+    pytest.param(4, True, 300.0, None, True, False, True, True, 234, id="L4-morton-x300"),
+    pytest.param(2, False, 1.0, None, False, False, True, False, 242, id="L2-linear-no-outs"),
+    pytest.param(2, True, 300.0, 1, False, False, True, True, 252, id="n1"),
+    pytest.param(3, False, 300.0, 31, False, False, True, True, 253, id="n31"),
+    pytest.param(2, True, 300.0, 33, False, False, True, False, 252, id="n33"),
+    pytest.param(4, True, 300.0, 129, False, False, True, True, 254, id="n129"),
+    pytest.param(4, True, 300.0, 60016, False, False, True, True, 264, id="n60016-x300"),
+]
+
+
+@pytest.mark.parametrize("loss_type", DIFF_LOSSES)
+@pytest.mark.parametrize("levels,poly,scale,n,ordered,frozen,bias,outs,seed", DIFF_EIKONAL_CASES)
+def test_fused_sdf_diff_eikonal_step_matches_oracle(loss_type, levels, poly, scale, n, ordered, frozen, bias, outs, seed):
+    """ONE launch of shine_sdf_diff_eikonal_step against the oracle's double backward, on the configurations of
+    test_fused_eikonal_step_matches_oracle that apply to sdf_diff_loss (always |w|, always the mean): 1..8 levels, poly /
+    linear interpolation, the frozen-decoder instantiation, a decoder without biases, a Morton-ordered batch, tables
+    x1 and x300, tile tails, the grid-stride loop, pred_out / grad_out passed or not."""
+    case = _eikonal_case(levels, poly, seed, True, "mean", scale, n=n, ordered=ordered, bias=bias,
+                         n_batch=60000 if (n or 0) > 10000 else 1500)
+    print(_diff_eikonal_runs(case, loss_type, frozen, outs)[2])
+
+
 def test_fused_eikonal_step_without_surface_sample():
     """No sample with weight > 0: the eikonal value is exactly 0 (as include/shine_b200.h documents; the reference's
-    torch mean over an empty selection would be NaN) and the gradients are those of the BCE-only step."""
+    torch mean over an empty selection would be NaN) and the gradients are those of the first term's step alone, for
+    sdf_bce and sdf_l1 / sdf_l2."""
+    from tests import test_gpu_sdf_diff as sdd
     case = _eikonal_case(3, True, 171, True, "mean", 300.0)
     case["weight"] = -np.abs(case["weight"])
-    runs = _fused_eikonal_runs(case)
-    want = run_oracle_step(case)
-    for w, r in runs.items():
-        assert r["eikonal"] == 0.0, w
-        assert abs(r["bce"] - want["loss"]) <= 1e-4 * abs(want["loss"]), w
-        assert np.all(np.abs(r["pred"] - want["pred"]) <= 2e-5 + 1e-5 * np.abs(want["pred"])), w
-        for k, gt in enumerate(want["table_grads"]):
-            assert np.abs(r["table_grads"][k] - gt)[:-1].max() <= 2e-4 * np.abs(gt).max() + 1e-10, (w, k)
-        for k, gt in want["dec_grads"].items():
-            assert np.abs(r["dec_grads"][k] - gt).max() <= 2e-4 * np.abs(gt).max() + 1e-10, (w, k)
-        for k in range(len(want["table_grads"])):       # weight_e does not enter: the same kernel arithmetic every time
-            assert np.abs(r["table_grads"][k] - runs[0.0]["table_grads"][k]).max() <= 1e-6 * np.abs(want["table_grads"][k]).max()
+    for loss_type in ("sdf_bce",) + DIFF_LOSSES:
+        runs = _fused_eikonal_runs(case, loss_type=loss_type)
+        want = run_oracle_step(case) if loss_type == "sdf_bce" else sdd._oracle(case, loss_type, runs[0.1]["pred"])
+        for w, r in runs.items():
+            assert r["eikonal"] == 0.0, (loss_type, w)
+            assert abs(r["bce"] - want["loss"]) <= 1e-4 * abs(want["loss"]), (loss_type, w)
+            assert np.all(np.abs(r["pred"] - want["pred"]) <= 2e-5 + 1e-5 * np.abs(want["pred"])), (loss_type, w)
+            for k, gt in enumerate(want["table_grads"]):
+                assert np.abs(r["table_grads"][k] - gt)[:-1].max() <= 2e-4 * np.abs(gt).max() + 1e-10, (loss_type, w, k)
+            for k, gt in want["dec_grads"].items():
+                assert np.abs(r["dec_grads"][k] - gt).max() <= 2e-4 * np.abs(gt).max() + 1e-10, (loss_type, w, k)
+            for k in range(len(want["table_grads"])):   # weight_e does not enter: the same kernel arithmetic every time
+                assert (np.abs(r["table_grads"][k] - runs[0.0]["table_grads"][k]).max() <=
+                        1e-6 * np.abs(want["table_grads"][k]).max()), (loss_type, w, k)
 
 
 def test_fused_eikonal_step_surface_samples_that_miss_every_level():
     """Surface samples outside the map: g = 0, so each adds (1 - 0)^2 = 1 to the mean and nothing to the gradients
-    (torch's d|g|/dg is 0 at g = 0)."""
+    (torch's d|g|/dg is 0 at g = 0); with sdf_bce and with sdf_l1 / sdf_l2 as the first term."""
     case = _eikonal_case(3, False, 172, scale=300.0)
     rng = np.random.default_rng(11)
     far = rng.uniform(0.6, 0.9, size=(77, 3)).astype(np.float32)
     case["coord"] = np.concatenate([case["coord"], far])
     case["label"] = np.concatenate([case["label"], np.zeros(77, np.float32)])
     case["weight"] = np.concatenate([case["weight"], np.ones(77, np.float32)])
-    want = _oracle_eikonal(case)
-    runs = _fused_eikonal_runs(case)
-    assert np.all(want["g"][-77:] == 0.0) and np.all(runs[0.1]["g"][-77:] == 0.0)
     n_surf = int((case["weight"] > 0).sum())
-    assert want["eikonal"] >= 77.0 / n_surf
-    print(_check_eikonal(runs, want))
+    for loss_type in ("sdf_bce",) + DIFF_LOSSES:
+        if loss_type == "sdf_bce":
+            want, runs = _oracle_eikonal(case), _fused_eikonal_runs(case)
+            line = _check_eikonal(runs, want)
+        else:
+            runs, want, line = _diff_eikonal_runs(case, loss_type)
+        assert np.all(want["g"][-77:] == 0.0) and np.all(runs[0.1]["g"][-77:] == 0.0), loss_type
+        assert want["eikonal"] >= 77.0 / n_surf, loss_type
+        print(loss_type, line)
 
 
 def test_fused_eikonal_shards_add_up_to_the_global_batch():

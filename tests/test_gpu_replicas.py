@@ -28,7 +28,15 @@ its error E_j:
   * forward, on absolute values with the fp64 pass's ReLU masks (A0 = sum w |row|, A1 = |W1| A0 + |b1|, A2 = |W2| A1 + |b2|,
     Ap = |w3| A2 + |b3|): the blend is off by (8L + 2) u A0, layer k adds EPS_MM(K) and the bias add u, so
     |pred - pred64| <= P = EPS_FWD Ap (checked against the kernel's own pred);
-  * dL/dpred = s (sigmoid(pred) - sigmoid(label / sigma)), s = loss scale x |weight|: off by s (P / 4 + 16 u) + 4 u |g|;
+  * dL/dpred = s (sigmoid(pred) - sigmoid(label / sigma)), s = loss scale x |weight|: off by dg = s (P / 4 + 16 u) + 4 u |g|;
+  * sdf_l2 / sdf_l1 (`diff_point`): d = (pred - label) / scale, then dL/dpred = 2 d / scale or sign(d) / scale, times |w|,
+    times the step's 1/n, every operation one fp32 rounding; scale and 1/n reach the kernel rounded to fp32.  s = |w| / n:
+      L2: the subtraction, two divisions, the products by |w| and 1/n, 1/n itself and scale (twice) are 8 roundings, and
+          pred is off by P: dg = 2 s P / scale^2 + 8 u |g|;
+      L1: the sign is exact (pred - label rounds to 0 only when they are equal); one division, two products, 1/n and
+          scale are 5 roundings: dg = 6 u |g|.  Where |pred64 - label| <= P the kernel's pred may lie on either side of the
+          label, or on it (sign 0: dL/dpred exactly 0); there the reference takes sign(kernel pred - label), elsewhere
+          sign(pred64 - label).  So the L1 reference is built after the step, from the pred it returned;
   * dfeat = W1^T (m1 . W2^T (m2 . w3 g)), two 32-term contractions: E = D ((2 EPS_MM(32) + 2 u) |g| + dg), D = |W1|^T (m1 .
     |W2|^T (m2 . |w3|)).
 Points within twice the forward error of a ReLU kink are dropped from the fused cases: there a correct fp32 kernel may take
@@ -42,7 +50,9 @@ import pytest
 import torch
 
 from oracle import shine_oracle as orc
+from tests import sdf_diff_oracle as sdo
 from tests.parity_utils import build_cuda_models, compare_step, make_case, oracle_from_case, sort_case_morton
+from tests.test_gpu_sdf_diff import _scale
 
 DEV = "cuda:0"
 U = 2.0 ** -24
@@ -50,6 +60,7 @@ C_SLACK = 4
 H = 32
 INVALID = -1                            # SHINE_ERR_INVALID_ARG
 gpu = pytest.mark.gpu
+DIFF_LOSSES = ("sdf_l1", "sdf_l2")
 
 
 def eps_mm(k, tf32x1=False):
@@ -99,6 +110,7 @@ class FoldSpy:
         assert self.calls, f"{what}: the step never called the replica fold"
         assert self.calls[-1] == want, f"{what}: the step ran with R = {self.calls[-1]} per level, expected {want}"
         assert max(want) > 1, f"{what}: the case does not switch replicas on"
+        print(f"[replicas] {what}: R per level {want}")
         self.calls.clear()
 
 
@@ -176,9 +188,10 @@ def _abs_feature(o, coord):
 
 
 class Ref:
-    """fp64 oracle step of a case (or the fp64 query backward of a given dfeat), with S, k and T per row."""
+    """fp64 oracle step of a case (or the fp64 query backward of a given dfeat), with S, k and T per row.
+    loss_type: the step's loss; sdf_l1 needs `pred`, the kernel's pred of the step being graded (module docstring)."""
 
-    def __init__(self, case, dfeat=None, tf32x1=False, grouped=False):
+    def __init__(self, case, dfeat=None, tf32x1=False, grouped=False, loss_type="sdf_bce", pred=None):
         c = case["cfg"]
         o, dec = _oracle64(case)
         coord = torch.from_numpy(case["coord"])
@@ -187,20 +200,37 @@ class Ref:
         if dfeat is None:
             label = torch.from_numpy(case["label"]).double()
             weight = torch.from_numpy(case["weight"]).double()
-            res = orc.train_step(o, dec, coord, label, weight, c["sigma"], c["weighted"], c["reduction"])
+            dd = {k: v.detach() for k, v in dec.items()}
+            with torch.no_grad():
+                feat = o.query_feature(coord)
+                dp = _decoder_passes(feat, _abs_feature(o, coord), dd, tf32x1, L)
+            scale, sign = _scale(case), None
+            if loss_type == "sdf_l1":
+                assert pred is not None, "the sdf_l1 reference needs the kernel's pred"
+                sign = sdo.l1_sign(orc.decoder_sdf(feat, dd).numpy(), case["label"], pred, dp["P"].numpy(), 0.0)
+            res = sdo.train_step(o, dec, coord, label, weight, c["sigma"], c["weighted"], c["reduction"], loss_type=loss_type,
+                                 scale=scale, double=True, l1_sign=sign)
             self.want = [g.detach().numpy() for g in res["table_grads"]]
             self.pred = res["pred"].numpy()
             self.step = {"loss": float(res["loss"]), "dec_grads": {k: g.numpy() for k, g in res["dec_grads"].items()}}
             feat = res["feature"].clone().requires_grad_(True)
-            dd = {k: v.detach() for k, v in dec.items()}
-            pred = orc.decoder_sdf(feat, dd)
-            loss = orc.sdf_bce_loss(pred, label, c["sigma"], weight.abs(), c["weighted"], c["reduction"])
-            dfeat64, g = torch.autograd.grad(loss, [feat, pred])
+            pred64 = orc.decoder_sdf(feat, dd)
+            if loss_type == "sdf_bce":
+                loss = orc.sdf_bce_loss(pred64, label, c["sigma"], weight.abs(), c["weighted"], c["reduction"])
+                dfeat64, g = torch.autograd.grad(loss, [feat, pred64])
+            else:
+                g = sdo.diff_dpred(pred64.detach(), label, weight.abs(), scale, loss_type == "sdf_l2", n,
+                                   None if sign is None else torch.from_numpy(sign))
+                dfeat64 = torch.autograd.grad(pred64, feat, g)[0]
             with torch.no_grad():
-                dp = _decoder_passes(feat.detach(), _abs_feature(o, coord), dd, tf32x1, L)
-                s = (weight.abs() if c["weighted"] else torch.ones(n, dtype=torch.float64))
-                s = s / n if c["reduction"] == "mean" else s
-                dg = s * (dp["P"] / 4 + 16 * U) + 4 * U * g.abs()
+                if loss_type == "sdf_bce":
+                    s = (weight.abs() if c["weighted"] else torch.ones(n, dtype=torch.float64))
+                    s = s / n if c["reduction"] == "mean" else s
+                    dg = s * (dp["P"] / 4 + 16 * U) + 4 * U * g.abs()
+                elif loss_type == "sdf_l2":
+                    dg = 2 * (weight.abs() / n) * dp["P"] / scale ** 2 + 8 * U * g.abs()
+                else:
+                    dg = 6 * U * g.abs()
                 E = dp["D"] * (dp["ebwd"] * g.abs() + dg)[:, None]
             self.P = dp["P"].numpy()
             self.kinks = int(dp["kink"].sum())
@@ -211,6 +241,7 @@ class Ref:
             self.want = [t.grad.numpy() for t in o.hier_features]
             E = torch.zeros(n, F, dtype=torch.float64)
             self.P, self.kinks = None, 0
+        self.dfeat = dfeat64.detach().numpy()
         pts = torch.arange(n).repeat_interleave(8)
         self.S, self.k, self.T = [None] * L, [None] * L, [None] * L
         for i, (ix, w) in enumerate(_blend(o, coord)):
@@ -261,10 +292,10 @@ def _dev(case):
     return tuple(torch.from_numpy(case[k]).to(DEV) for k in ("coord", "label", "weight"))
 
 
-def trainer(case, freeze=False, **kw):
+def trainer(case, freeze=False, main_loss_type="sdf_bce", **kw):
     from shine_mapping_b200 import SdfTrainer
     cfg, octree, dec = build_cuda_models(case, DEV, freeze_decoder=freeze)
-    tr = SdfTrainer(cfg, octree, dec, **kw)
+    tr = SdfTrainer(cfg, octree, dec, main_loss_type=main_loss_type, **kw)
     tr.use_replicas = True
     return tr, FoldSpy(octree)
 
@@ -282,9 +313,13 @@ def train_step(tr, case, morton_ordered=None):
     return tables, pred.cpu().numpy(), loss, dec
 
 
-def check_step(tr, spy, case, ref, what, tf32x1=False, morton_ordered=None):
-    """One trainer step: R per level as expected, every element within its bound, compare_step, scratch all zero."""
+def check_step(tr, spy, case, ref, what, tf32x1=False, morton_ordered=None, grouped=False):
+    """One trainer step: R per level as expected, every element within its bound, compare_step, scratch all zero.
+    ref None: the Ref of the trainer's loss, built after the step from the pred it returned."""
     tables, pred, loss, dec = train_step(tr, case, morton_ordered)
+    if ref is None:
+        ref = Ref(case, tf32x1=tf32x1, grouped=grouped, loss_type=tr.main_loss_type, pred=pred)
+    what = f"{what} {tr.main_loss_type}"
     spy.expect(expected_replicas(case["tables"], ref.n), what)
     worst = ref.grade(tables, what, pred)
     print(what, ref.compare(tables, pred, loss, dec, tf32x1))
@@ -317,48 +352,75 @@ def check_query_bwd(octree, spy, case, ref, dfeat, what):
 
 # ---- fused kernels at forced R ------------------------------------------------------------------------------------------
 
+def with_weights(case, loss_type, seed):
+    """sdf_l1 / sdf_l2 always weight by |w|: give the case weights other than +-1 (same points and labels)."""
+    if loss_type == "sdf_bce":
+        return case
+    w = case["weight"] * np.random.default_rng(seed).uniform(0.5, 1.5, case["weight"].shape[0]).astype(np.float32)
+    return dict(case, weight=w)
+
+
+def with_own_pred_labels(tr, case, every=97):
+    """sdf_l1: every `every`-th sample gets the kernel's own pred as label, an exact zero difference (dL/dpred = 0)."""
+    if tr.main_loss_type != "sdf_l1":
+        return case
+    out = dict(case, label=case["label"].copy())
+    out["label"][::every] = train_step(tr, case)[1][::every]
+    return out
+
+
 @gpu
-@pytest.mark.parametrize("rmax", [2, 4, 8, 16, 32, 64])
-def test_general_kernel_at_every_replica_count(rmax, force):
+@pytest.mark.parametrize("rmax,loss_type", [pytest.param(r, "sdf_bce", id=str(r)) for r in (2, 4, 8, 16, 32, 64)] +
+                         [pytest.param(64, lt, id=f"64-{lt}") for lt in DIFF_LOSSES])
+def test_general_kernel_at_every_replica_count(rmax, loss_type, force):
     """The LMAX = 8 general kernel (6 levels) with the coarsest level at R = rmax and the finer ones at smaller R: every tail
-    split of the fold's 8-wide loop (nrep = 1, 3, 7, 15, 31, 63)."""
+    split of the fold's 8-wide loop (nrep = 1, 3, 7, 15, 31, 63; R <= 64 takes them all at once)."""
     force(1, rmax)
-    case, dropped = drop_kinks(make_case(n_points=2500, n_batch=3000, feat_levels=6, seed=60 + rmax))
+    case, dropped = drop_kinks(with_weights(make_case(n_points=2500, n_batch=3000, feat_levels=6, seed=60 + rmax),
+                                            loss_type, rmax))
     assert expected_replicas(case["tables"], case["coord"].shape[0])[0] == rmax
-    tr, spy = trainer(case)
-    check_step(tr, spy, case, Ref(case), f"general L=6 R<={rmax} (kinks dropped: {dropped})")
+    tr, spy = trainer(case, main_loss_type=loss_type)
+    case = with_own_pred_labels(tr, case)
+    check_step(tr, spy, case, None, f"general L=6 R<={rmax} (kinks dropped: {dropped})")
+
+
+VARIANTS = [("tf32x1", False, "mean"), ("frozen", True, "sum"), ("biasless", True, "mean"), ("plain", False, "sum")]
 
 
 @gpu
-@pytest.mark.parametrize("levels", [3, 8])
-@pytest.mark.parametrize("variant,weighted,reduction", [("tf32x1", False, "mean"), ("frozen", True, "sum"),
-                                                        ("biasless", True, "mean"), ("plain", False, "sum")])
-def test_general_kernel_variants(levels, variant, weighted, reduction, force):
+@pytest.mark.parametrize("levels,variant,weighted,reduction,loss_type",
+                         [pytest.param(lv, v, w, r, "sdf_bce", id=f"{v}-{w}-{r}-{lv}") for v, w, r in VARIANTS
+                          for lv in (3, 8)] +
+                         [pytest.param(lv, v, True, "mean", lt, id=f"{v}-{lv}-{lt}") for lt in DIFF_LOSSES
+                          for lv, v in ((3, "tf32x1"), (8, "frozen"), (3, "biasless"), (8, "plain"))])
+def test_general_kernel_variants(levels, variant, weighted, reduction, loss_type, force):
     """L <= 4 and L > 4 instantiations with plain TF32, a frozen decoder (no decoder gradients) and a bias-less decoder.
-    Plain TF32 puts many points within its forward error of a ReLU kink, hence the larger batch."""
+    Plain TF32 puts many points within its forward error of a ReLU kink, hence the larger batch.  sdf_l1 / sdf_l2 always
+    weight by |w| with the mean: weighted / reduction do not apply to them."""
     force(1, 64)
     tf32x1 = variant == "tf32x1"
     case = make_case(n_points=2500, n_batch=12000 if tf32x1 else 3000, feat_levels=levels, seed=70 + levels,
                      weighted=weighted, reduction=reduction, bias=variant != "biasless", n_frames=2 if levels == 8 else 1)
     case, dropped = drop_kinks(case, tf32x1)
-    tr, spy = trainer(case, freeze=variant == "frozen", tf32x1=tf32x1)
-    check_step(tr, spy, case, Ref(case, tf32x1=tf32x1), f"general L={levels} {variant} (kinks dropped: {dropped})", tf32x1)
+    tr, spy = trainer(case, freeze=variant == "frozen", tf32x1=tf32x1, main_loss_type=loss_type)
+    check_step(tr, spy, case, None, f"general L={levels} {variant} (kinks dropped: {dropped})", tf32x1)
 
 
 @gpu
-@pytest.mark.parametrize("ordered", [True, False])
-def test_grouped_kernel_with_replicas(ordered, force):
+@pytest.mark.parametrize("ordered,loss_type", [pytest.param(o, "sdf_bce", id=str(o)) for o in (True, False)] +
+                         [pytest.param(o, lt, id=f"{o}-{lt}") for lt in DIFF_LOSSES for o in (True, False)])
+def test_grouped_kernel_with_replicas(ordered, loss_type, force):
     """The voxel-grouped kernel with `grouped_replicas`: replica by tile, per-node 3xTF32 sums (Morton-ordered batch) and
     its per-point fall-back (batch in the order drawn)."""
     force(1, 64)
-    case = make_case(n_points=2500, n_batch=6000, feat_levels=4, seed=81)
+    case = with_weights(make_case(n_points=2500, n_batch=6000, feat_levels=4, seed=81), loss_type, 81)
     if ordered:
         case = sort_case_morton(case)
     case, dropped = drop_kinks(case)
-    tr, spy = trainer(case, morton_ordered=True)
+    tr, spy = trainer(case, morton_ordered=True, main_loss_type=loss_type)
     tr.grouped_replicas = True
-    check_step(tr, spy, case, Ref(case, grouped=True), f"grouped ordered={ordered} (kinks dropped: {dropped})",
-               morton_ordered=True)
+    check_step(tr, spy, case, None, f"grouped ordered={ordered} (kinks dropped: {dropped})", morton_ordered=True,
+               grouped=True)
 
 
 @gpu
@@ -382,11 +444,14 @@ def natural_case():
 
 @gpu
 def test_natural_size_general_kernel(natural_case):
-    """50 000 points at L = 8 switch replicas on by themselves: R = 16 / 8 / 4 / 2 on the four coarsest levels."""
+    """50 000 points at L = 8 switch replicas on by themselves: R = 16 / 8 / 4 / 2 on the four coarsest levels; each loss
+    on a trainer of its own."""
     case, dropped = drop_kinks(natural_case)
     assert expected_replicas(case["tables"], case["coord"].shape[0])[:4] == [16, 8, 4, 2]
-    tr, spy = trainer(case)
-    check_step(tr, spy, case, Ref(case), f"natural L=8 general (kinks dropped: {dropped})")
+    for loss_type in ("sdf_bce",) + DIFF_LOSSES:
+        c = with_weights(case, loss_type, 58)
+        tr, spy = trainer(c, main_loss_type=loss_type)
+        check_step(tr, spy, c, None, f"natural L=8 general (kinks dropped: {dropped})")
 
 
 @gpu
@@ -505,14 +570,21 @@ def test_step_from_host_chunks_with_different_replica_counts(force):
     chunks = [(n * k // 3, n * (k + 1) // 3) for k in range(3)]
     want = [expected_replicas(case["tables"], e - b) for b, e in chunks]
     assert [r[0] for r in want] == [32, 64, 64], want
-    tr, spy = trainer(case)
-    coord_h = torch.from_numpy(case["coord"]).pin_memory(); label_h = torch.from_numpy(case["label"]).pin_memory()
-    tr.step_from_host(coord_h, label_h, chunks=3)
-    torch.cuda.synchronize()
-    assert spy.calls[:3] == want, f"chunks ran with R = {spy.calls[:3]}, expected {want}"
-    ref = Ref(case)
-    ref.grade([g.detach().cpu().numpy() for g in tr.table_grads], "step_from_host chunks=3")
-    assert_scratch_zero(tr.octree, "step_from_host")
+    for loss_type in ("sdf_bce",) + DIFF_LOSSES:
+        # sdf_l1 / sdf_l2 read the weights: each chunk copies its own slice of them (weights other than +-1 show a wrong one)
+        c = with_weights(case, loss_type, 116)
+        tr, spy = trainer(c, main_loss_type=loss_type)
+        what = f"step_from_host chunks=3 {loss_type}"
+        pred = train_step(tr, c)[1] if loss_type == "sdf_l1" else None     # the kernel's pred for the L1 reference
+        spy.calls.clear()
+        coord_h, label_h, weight_h = (torch.from_numpy(c[k]).pin_memory() for k in ("coord", "label", "weight"))
+        tr.step_from_host(coord_h, label_h, weight_h if loss_type != "sdf_bce" else None, chunks=3)
+        torch.cuda.synchronize()
+        assert spy.calls[:3] == want, f"{what}: chunks ran with R = {spy.calls[:3]}, expected {want}"
+        print(f"[replicas] {what}: R per level of the chunks {want}")
+        ref = Ref(c, loss_type=loss_type, pred=pred)
+        ref.grade([g.detach().cpu().numpy() for g in tr.table_grads], what)
+        assert_scratch_zero(tr.octree, what)
 
 
 @gpu
@@ -520,21 +592,25 @@ def test_capture_step_replays_on_changed_data(force):
     force(1, 64)
     case, _ = drop_kinks(make_case(n_points=2500, n_batch=6000, feat_levels=6, seed=117))
     n = case["coord"].shape[0] // 2
-    a, b = subset(case, np.arange(n)), subset(case, np.arange(n, 2 * n))
-    refs = {"A": Ref(a), "B": Ref(b)}
-    tr, spy = trainer(a)
-    coord, label, weight = _dev(a)
-    graph = tr.capture_step(coord, label, weight, exchange=False)
-    spy.expect(expected_replicas(a["tables"], n), "capture")
-    refs["A"].grade([g.detach().cpu().numpy() for g in tr.table_grads], "capture warm-up on A")
-    for name in ("B", "A", "B"):
-        src = _dev(b if name == "B" else a)
-        for dst, s in zip((coord, label, weight), src):
-            dst.copy_(s)
-        graph.replay()
-        torch.cuda.synchronize()
-        refs[name].grade([g.detach().cpu().numpy() for g in tr.table_grads], f"replay on {name}")
-        assert_scratch_zero(tr.octree, f"replay on {name}")
+    for loss_type in ("sdf_bce",) + DIFF_LOSSES:
+        c = with_weights(case, loss_type, 117)
+        a, b = subset(c, np.arange(n)), subset(c, np.arange(n, 2 * n))
+        tr, spy = trainer(a, main_loss_type=loss_type)
+        # the kernel's pred of each half for the L1 reference (the replays write no pred)
+        preds = {k: train_step(tr, v)[1] if loss_type == "sdf_l1" else None for k, v in (("A", a), ("B", b))}
+        refs = {k: Ref(v, loss_type=loss_type, pred=preds[k]) for k, v in (("A", a), ("B", b))}
+        coord, label, weight = _dev(a)
+        graph = tr.capture_step(coord, label, weight, exchange=False)
+        spy.expect(expected_replicas(a["tables"], n), f"capture {loss_type}")
+        refs["A"].grade([g.detach().cpu().numpy() for g in tr.table_grads], f"capture warm-up on A {loss_type}")
+        for name in ("B", "A", "B"):
+            src = _dev(b if name == "B" else a)
+            for dst, s in zip((coord, label, weight), src):
+                dst.copy_(s)
+            graph.replay()
+            torch.cuda.synchronize()
+            refs[name].grade([g.detach().cpu().numpy() for g in tr.table_grads], f"replay on {name} {loss_type}")
+            assert_scratch_zero(tr.octree, f"replay on {name} {loss_type}")
 
 
 # ---- the fold kernel on its own, bit-exact ---------------------------------------------------------------------------------
@@ -634,13 +710,19 @@ def _abi_call(lib, name, desc):
     if name == "shine_sdf_bce_eikonal_step":
         return lib.shine_sdf_bce_eikonal_step(o, C.byref(dec), None, None, None, 0, 1.0, 1.0, 0.1, None, None, None, None,
                                               None, 0, None)
+    # the sdf_diff_loss entries need their weights and a valid scale even for an empty batch
+    if name == "shine_sdf_diff_step":
+        return lib.shine_sdf_diff_step(o, C.byref(dec), None, None, 0x3000, 0, 0.01, 1.0, None, None, None, 0, None)
+    if name == "shine_sdf_diff_eikonal_step":
+        return lib.shine_sdf_diff_eikonal_step(o, C.byref(dec), None, None, 0x3000, 0, 0.01, 1.0, 1.0, 0.1, None, None,
+                                               None, None, None, 0, None)
     if name == "shine_query_bwd":
         return lib.shine_query_bwd(o, None, 0, None, None)
     return lib.shine_reduce_grad_replicas(o, None)
 
 
 @pytest.mark.parametrize("name", ["shine_sdf_bce_step", "shine_query_bwd", "shine_reduce_grad_replicas",
-                                  "shine_sdf_bce_eikonal_step"])
+                                  "shine_sdf_bce_eikonal_step", "shine_sdf_diff_step", "shine_sdf_diff_eikonal_step"])
 def test_abi_replica_checks(name, built_lib):
     """R must be a power of two up to 64 with a scratch pointer; R = 0 and 1 need no scratch.  Placeholder pointers and an
     empty batch: an accepted descriptor returns OK without touching the device."""
@@ -666,32 +748,30 @@ def test_abi_replica_checks(name, built_lib):
 # ---- the bound itself -------------------------------------------------------------------------------------------------------
 
 def test_bound_passes_the_fp32_oracle_and_sees_one_lost_term():
-    """The fp32 oracle (a correct fp32 implementation in another summation order) is inside the bound; the same gradients
-    with one (point, corner) term taken out of a row that several points touch, or added twice, are not."""
-    from tests.parity_utils import run_oracle_step
-    case, _ = drop_kinks(make_case(n_points=1500, n_batch=1500, feat_levels=3, seed=5))
-    ref = Ref(case)
-    got = run_oracle_step(case)["table_grads"]
-    ref.grade(got, "fp32 oracle")
-    o, dec = _oracle64(case)
-    coord = torch.from_numpy(case["coord"])
-    ix, w = _blend(o, coord)[0]                    # leaf level = table L - 1
-    kk = len(got) - 1
-    feat = o.query_feature(coord).detach().requires_grad_(True)
-    c = case["cfg"]
-    pred = orc.decoder_sdf(feat, {k: v.detach() for k, v in dec.items()})
-    loss = orc.sdf_bce_loss(pred, torch.from_numpy(case["label"]).double(), c["sigma"],
-                            torch.from_numpy(case["weight"]).double().abs(), c["weighted"], c["reduction"])
-    dfeat = torch.autograd.grad(loss, feat)[0]
-    terms = (w[:, None] * dfeat.repeat_interleave(8, 0)).numpy()          # w_{j,c} dfeat_j of every (point, corner)
-    rows = ix.numpy()
-    # a median-sized term in a row that three or more terms touch
-    cand = [j for j in range(len(rows)) if rows[j] >= 0 and ref.k[kk][rows[j]] >= 3 and np.abs(terms[j]).max() > 0]
-    cand.sort(key=lambda j: np.abs(terms[j]).max())
-    j = cand[len(cand) // 2]
-    term = terms[j]
-    for sign, name in ((-1.0, "lost"), (1.0, "duplicated")):
-        bad = [t.copy() for t in got]
-        bad[kk][rows[j]] += sign * term.astype(np.float32)
-        with pytest.raises(AssertionError, match="outside the bound"):
-            ref.grade(bad, f"one {name} term")
+    """For each loss, the fp32 oracle (a correct fp32 implementation in another summation order) is inside the bound; the
+    same gradients with one (point, corner) term taken out of a row that several points touch, or added twice, are not.
+    sdf_l1 takes the fp32 oracle's pred as the kernel's for its signs near the label."""
+    for loss_type in ("sdf_bce",) + DIFF_LOSSES:
+        case, _ = drop_kinks(with_weights(make_case(n_points=1500, n_batch=1500, feat_levels=3, seed=5), loss_type, 5))
+        o, dec = oracle_from_case(case)
+        res = sdo.train_step(o, dec, *(torch.from_numpy(case[k]) for k in ("coord", "label", "weight")),
+                             case["cfg"]["sigma"], case["cfg"]["weighted"], case["cfg"]["reduction"], loss_type=loss_type,
+                             scale=_scale(case))
+        got, pred = [g.detach().numpy() for g in res["table_grads"]], res["pred"].numpy()
+        ref = Ref(case, loss_type=loss_type, pred=pred)
+        ref.grade(got, f"fp32 oracle {loss_type}", pred)
+        o, dec = _oracle64(case)
+        ix, w = _blend(o, torch.from_numpy(case["coord"]))[0]            # leaf level = table L - 1
+        kk = len(got) - 1
+        terms = w[:, None].numpy() * np.repeat(ref.dfeat, 8, 0)          # w_{j,c} dfeat_j of every (point, corner)
+        rows = ix.numpy()
+        # a median-sized term in a row that three or more terms touch
+        cand = [j for j in range(len(rows)) if rows[j] >= 0 and ref.k[kk][rows[j]] >= 3 and np.abs(terms[j]).max() > 0]
+        cand.sort(key=lambda j: np.abs(terms[j]).max())
+        j = cand[len(cand) // 2]
+        term = terms[j]
+        for sign, name in ((-1.0, "lost"), (1.0, "duplicated")):
+            bad = [t.copy() for t in got]
+            bad[kk][rows[j]] += sign * term.astype(np.float32)
+            with pytest.raises(AssertionError, match="outside the bound"):
+                ref.grade(bad, f"one {name} term {loss_type}")

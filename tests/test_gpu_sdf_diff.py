@@ -58,10 +58,7 @@ def _oracle(case, loss_type, got_pred=None, atol=PRED_ATOL, rtol=PRED_RTOL):
         o2, dec2 = oracle_from_case(case)
         ref = sdo.train_step(o2, dec2, torch.from_numpy(case["coord"]), torch.from_numpy(label),
                              torch.from_numpy(case["weight"]), 1.0, loss_type=loss_type, scale=_scale(case), double=True)
-        p = ref["pred"].numpy()
-        near = np.abs(p - label) <= atol + rtol * np.abs(p)
-        sign = np.sign(p - label)
-        sign[near] = np.sign(got_pred[near].astype(np.float32) - label[near])
+        sign = sdo.l1_sign(ref["pred"].numpy(), label, got_pred, atol, rtol)
     res = sdo.train_step(o, dec, torch.from_numpy(case["coord"]), torch.from_numpy(label), torch.from_numpy(case["weight"]),
                          1.0, loss_type=loss_type, scale=_scale(case), double=True, l1_sign=sign)
     return sdo.as_numpy(res, o)
