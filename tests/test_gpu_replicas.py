@@ -42,6 +42,9 @@ its error E_j:
 Points within twice the forward error of a ReLU kink are dropped from the fused cases: there a correct fp32 kernel may take
 the other branch.  `compare_step` (2e-4 of the level maximum) runs as a second check, and each case prints its worst
 error / bound.
+The eikonal paths extend this model (blend-weight derivatives, g, gamma and the eikonal scatter): tests/eikonal_bound.py.
+The pieces both use (eps_mm, the fp32 blend, the decoder passes, the kink filter, the grading loop) live in
+tests/error_bound.py.
 """
 import ctypes as C
 
@@ -51,20 +54,18 @@ import torch
 
 from oracle import shine_oracle as orc
 from tests import sdf_diff_oracle as sdo
+from tests.error_bound import C_SLACK, U, drop_kinks, eps_mm, grade_tables, subset
+from tests.error_bound import abs_feature as _abs_feature
+from tests.error_bound import blend as _blend
+from tests.error_bound import decoder_passes as _decoder_passes
+from tests.error_bound import oracle64 as _oracle64
 from tests.parity_utils import build_cuda_models, compare_step, make_case, oracle_from_case, sort_case_morton
 from tests.test_gpu_sdf_diff import _scale
 
 DEV = "cuda:0"
-U = 2.0 ** -24
-C_SLACK = 4
-H = 32
 INVALID = -1                            # SHINE_ERR_INVALID_ARG
 gpu = pytest.mark.gpu
 DIFF_LOSSES = ("sdf_l1", "sdf_l2")
-
-
-def eps_mm(k, tf32x1=False):
-    return (2.0 ** -9 if tf32x1 else 64 * U) + 8 * k * U
 
 
 # ---- forcing replicas and proving they were on ----------------------------------------------------------------------------
@@ -123,69 +124,6 @@ def assert_scratch_zero(octree, what=""):
 
 
 # ---- fp64 reference and the per-element bound -----------------------------------------------------------------------------
-
-def subset(case, keep):
-    out = dict(case)
-    for k in ("coord", "label", "weight"):
-        out[k] = np.ascontiguousarray(case[k][keep])
-    return out
-
-
-def _oracle64(case):
-    o, dec = oracle_from_case(case)
-    o.hier_features = [t.detach().double().requires_grad_(True) for t in o.hier_features]
-    return o, {k: v.detach().double().requires_grad_(True) for k, v in dec.items()}
-
-
-def _blend(o, coord):
-    """Per level (bottom-up): the oracle's corner rows [N*8] and fp32 blend weights [N*8] as fp64."""
-    idx = o.get_indices(coord)
-    out = []
-    for i in range(o.featured_level_num):
-        w = o.interpolat(coord, o.max_level - i, o.polynomial_interpolation).reshape(-1).double()
-        out.append((idx[i].reshape(-1), w))
-    return out
-
-
-def _decoder_passes(feat, absfeat, dec, tf32x1, n_levels):
-    """fp64 forward with the absolute-value passes of the module docstring -> dict of per-point quantities."""
-    z = torch.zeros((), dtype=torch.float64)
-    W1, W2, w3 = (dec[k].detach() for k in ("layers.0.weight", "layers.1.weight", "lout.weight"))
-    b1, b2, b3 = (dec.get(k, z).detach() for k in ("layers.0.bias", "layers.1.bias", "lout.bias"))
-    F = W1.shape[1]
-    a1 = feat @ W1.T + b1
-    m1 = (a1 > 0).double()
-    a2 = (a1 * m1) @ W2.T + b2
-    m2 = (a2 > 0).double()
-    A1 = absfeat @ W1.abs().T + b1.abs()
-    A2 = (A1 * m1) @ W2.abs().T + b2.abs()
-    Ap = ((A2 * m2) @ w3.abs().T + b3.abs()).squeeze(1)
-    e1 = (8 * n_levels + 2) * U + eps_mm(F, tf32x1) + U
-    e2 = e1 + eps_mm(H, tf32x1) + U
-    efwd = e2 + eps_mm(H, tf32x1) + U
-    D = ((m2 * w3.abs()) @ W2.abs() * m1) @ W1.abs()
-    kink = ((a1.abs() <= 2 * e1 * A1).any(1) | (a2.abs() <= 2 * e2 * A2).any(1))
-    return {"A0": absfeat, "P": efwd * Ap, "D": D, "kink": kink, "ebwd": 2 * eps_mm(H, tf32x1) + 2 * U}
-
-
-def drop_kinks(case, tf32x1=False):
-    """The case without the points whose pre-activations lie within twice the forward error of a ReLU kink."""
-    o, dec = _oracle64(case)
-    coord = torch.from_numpy(case["coord"])
-    with torch.no_grad():
-        feat = o.query_feature(coord)
-        absfeat = _abs_feature(o, coord)
-        kink = _decoder_passes(feat, absfeat, dec, tf32x1, o.featured_level_num)["kink"].numpy()
-    return subset(case, ~kink), int(kink.sum())
-
-
-def _abs_feature(o, coord):
-    total = torch.zeros(coord.shape[0], o.feature_dim, dtype=torch.float64)
-    for i, (ix, w) in enumerate(_blend(o, coord)):
-        t = o.hier_features[o.featured_level_num - 1 - i].detach().abs()
-        total += (t[ix] * w[:, None]).reshape(coord.shape[0], 8, -1).sum(1)
-    return total
-
 
 class Ref:
     """fp64 oracle step of a case (or the fp64 query backward of a given dfeat), with S, k and T per row.
@@ -255,25 +193,12 @@ class Ref:
 
     def grade(self, got_tables, what, pred=None):
         """Every element of every level (trash row excluded) against its bound -> worst error / bound."""
-        worst = 0.0
-        for kk, got in enumerate(got_tables):
-            got = np.asarray(got, dtype=np.float64)[:-1]
-            want, S, k, T = self.want[kk][:-1], self.S[kk][:-1], self.k[kk][:-1], self.T[kk][:-1]
-            bound = (k[:, None] + self.slack) * U * S + T
-            err = np.abs(got - want)
-            bad = np.argwhere(err > bound)
-            if bad.size:
-                r, f = bad[0]
-                raise AssertionError(
-                    f"{what}: level {kk} has {len(bad)} elements outside the bound; first: row {r} channel {f} got "
-                    f"{got[r, f]:.9g} want {want[r, f]:.9g} bound {bound[r, f]:.3g} (k_u = {k[r]}, S = {S[r, f]:.3g})")
-            if err.size:
-                worst = max(worst, float((err / np.where(bound > 0, bound, 1.0)).max()))
+        bounds = [(k[:, None] + self.slack) * U * S + T for S, k, T in zip(self.S, self.k, self.T)]
+        worst = grade_tables(got_tables, self.want, bounds, self.k, self.S, what, "replica bounds")
         if pred is not None:
             e = np.abs(np.asarray(pred, dtype=np.float64) - self.pred)
             assert (e <= self.P).all(), f"{what}: pred outside its bound at {int((e > self.P).sum())} points"
             print(f"[replica bounds] {what}: pred worst {float((e / self.P).max()):.3f} of the bound")
-        print(f"[replica bounds] {what}: table grads worst {worst:.3f} of the bound")
         return worst
 
     def compare(self, got_tables, pred, loss, dec_grads, tf32x1=False):
