@@ -11,6 +11,7 @@ With SHINE_FLAG_TF32X1 (plain TF32) pred is only good to ~2e-3 and is tested sep
 """
 from __future__ import annotations
 
+import copy
 import os
 import sys
 
@@ -116,11 +117,15 @@ def drop_relu_kink_points(case, eps=2e-6):
 
 
 def oracle_from_case(case):
-    """Rebuild the oracle octree by replaying the frames, then overwrite its tables with the case's."""
+    """Rebuild the oracle octree by replaying the frames, then overwrite its tables with the case's.  A case that carries
+    "oracle", an OracleOctree already grown by its frames, reuses that octree's lookup tables instead of replaying."""
     c = case["cfg"]
-    o = orc.OracleOctree(c["tree_level_world"], c["tree_level_feat"], c["feature_dim"], 0.05, c["poly_int_on"])
-    for fr in case["frames"]:
-        o.update(torch.from_numpy(np.asarray(fr)))
+    if case.get("oracle") is not None:
+        o = copy.copy(case["oracle"])
+    else:
+        o = orc.OracleOctree(c["tree_level_world"], c["tree_level_feat"], c["feature_dim"], 0.05, c["poly_int_on"])
+        for fr in case["frames"]:
+            o.update(torch.from_numpy(np.asarray(fr)))
     assert [tuple(t.shape) for t in o.hier_features] == [tuple(t.shape) for t in case["tables"]], \
         "oracle row counts differ from the case's tables"
     o.hier_features = [torch.from_numpy(np.asarray(t).copy()).requires_grad_(True) for t in case["tables"]]

@@ -171,6 +171,7 @@ class Ref:
                     dg = 6 * U * g.abs()
                 E = dp["D"] * (dp["ebwd"] * g.abs() + dg)[:, None]
             self.P = dp["P"].numpy()
+            self.kink = dp["kink"].numpy()
             self.kinks = int(dp["kink"].sum())
         else:
             dfeat64 = torch.from_numpy(dfeat).double()
@@ -178,7 +179,7 @@ class Ref:
             feat.backward(dfeat64)
             self.want = [t.grad.numpy() for t in o.hier_features]
             E = torch.zeros(n, F, dtype=torch.float64)
-            self.P, self.kinks = None, 0
+            self.P, self.kink, self.kinks = None, np.zeros(n, dtype=bool), 0
         self.dfeat = dfeat64.detach().numpy()
         pts = torch.arange(n).repeat_interleave(8)
         self.S, self.k, self.T = [None] * L, [None] * L, [None] * L
