@@ -66,8 +66,20 @@ def decoder_passes(feat, absfeat, dec, tf32x1, n_levels):
     e2 = e1 + eps_mm(H, tf32x1) + U
     efwd = e2 + eps_mm(H, tf32x1) + U
     D = ((m2 * w3.abs()) @ W2.abs() * m1) @ W1.abs()
-    kink = ((a1.abs() <= 2 * e1 * A1).any(1) | (a2.abs() <= 2 * e2 * A2).any(1))
-    return {"A0": absfeat, "P": efwd * Ap, "D": D, "kink": kink, "ebwd": 2 * eps_mm(H, tf32x1) + 2 * U}
+    # a unit whose absolute-value pass is 0 is an exact 0 in every precision (a point that misses every level, a decoder
+    # without biases): its mask is exact, not a kink
+    u1 = (a1.abs() <= 2 * e1 * A1) & (A1 > 0)
+    m1_hi = ((m1 > 0) | u1).double()
+    A2_hi = (A1 * m1_hi) @ W2.abs().T + b2.abs()
+    u2 = (a2.abs() <= 2 * e2 * A2_hi) & (A2_hi > 0)
+    kink = u1.any(1) | u2.any(1)
+    # pred of a kink point, whichever branch the kernel takes: an uncertain unit is off by at most |a| + e A <= 3 e A of
+    # its fp64 value (2 e A + e A), and the pass runs with the uncertain units live (A2_hi, m2_hi)
+    Ap_hi = ((A2_hi * ((m2 > 0) | u2).double()) @ w3.abs().T + b3.abs()).squeeze(1)
+    P = torch.where(kink, 3 * efwd * Ap_hi, efwd * Ap)
+    return {"A0": absfeat, "P": P, "D": D, "kink": kink, "ebwd": 2 * eps_mm(H, tf32x1) + 2 * U,
+            "A1": A1, "A2": A2, "A2_hi": A2_hi, "e1": e1, "e2": e2, "ef": (8 * n_levels + 2) * U * absfeat,
+            "m1_hi": m1_hi, "m2_hi": ((m2 > 0) | u2).double()}
 
 
 def drop_kinks(case, tf32x1=False):
@@ -150,3 +162,25 @@ def grade_values(got, want, bound, what, name, tag="bounds"):
     worst = float((err / np.where(bound > 0, bound, 1.0)).max()) if err.size else 0.0
     print(f"[{tag}] {what}: {name} worst {worst:.3f} of the bound")
     return worst
+
+
+def grouped_counts(ix, rows, max_runs=6, tile=16):
+    """k_u of the voxel-grouped scatter (`grouped_scatter`): the fp32 adds that land on each row of one level.  ix [n, 8]
+    corner rows of the level per point (-1: a miss).  Tiles are 16 consecutive points; a tile whose hitting points fall into
+    at most `max_runs` (kMaxGroupedRuns) distinct nodes adds one term per (node, corner) row, its per-node sums formed by a
+    tensor-core contraction; a scattered tile (more nodes) adds one term per (point, corner)."""
+    ix = np.asarray(ix)
+    n = ix.shape[0]
+    pad = -n % tile
+    node = np.concatenate((ix[:, 0], np.full(pad, -1, dtype=ix.dtype))).reshape(-1, tile)   # corner 0 names the node
+    srt = np.sort(node, axis=1)
+    nruns = ((srt >= 0) & np.concatenate((np.ones((srt.shape[0], 1), bool), srt[:, 1:] != srt[:, :-1]), 1)).sum(1)
+    tile_of = np.arange(n) // tile
+    hit = ix[:, 0] >= 0
+    scattered = (nruns > max_runs)[tile_of] & hit
+    k = np.bincount(ix[scattered].reshape(-1), minlength=rows)
+    grouped = hit & ~scattered
+    key = tile_of[grouped].astype(np.int64) * (int(node.max()) + 2) + ix[grouped, 0]
+    _, first = np.unique(key, return_index=True)                       # one point per (tile, node)
+    k += np.bincount(ix[grouped][first].reshape(-1), minlength=rows)
+    return k

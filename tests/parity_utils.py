@@ -175,10 +175,28 @@ def build_cuda_models(case, device="cuda:0", freeze_decoder=False):
     return cfg, octree, dec
 
 
+FROZEN_SENTINEL = 1.5 ** 60
+
+
+def fill_frozen_grads(dec):
+    """Give a frozen decoder's parameters sentinel gradients -> their copies (check_frozen_grads after the step)."""
+    for p in dec.parameters():
+        p.grad = torch.full_like(p, FROZEN_SENTINEL)
+    return [p.grad.clone() for p in dec.parameters()]
+
+
+def check_frozen_grads(dec, before):
+    """A frozen decoder's gradients come back bit for bit."""
+    for (name, p), b in zip(dec.named_parameters(), before):
+        assert p.grad is not None and torch.equal(p.grad.view(torch.int32), b.view(torch.int32)), \
+            f"the step wrote the gradient of frozen decoder parameter {name}"
+
+
 def run_cuda_step(case, device="cuda:0", single_pass=True, tf32x1=False, unfused=False, morton_ordered=False,
                   freeze_decoder=False):
     from shine_mapping_b200 import sdf_bce_loss, sdf_bce_step
     cfg, octree, dec = build_cuda_models(case, device, freeze_decoder=freeze_decoder)
+    frozen = fill_frozen_grads(dec) if freeze_decoder else None
     c = case["cfg"]
     coord = torch.from_numpy(case["coord"]).to(device); label = torch.from_numpy(case["label"]).to(device)
     weight = torch.from_numpy(case["weight"]).to(device)
@@ -192,6 +210,8 @@ def run_cuda_step(case, device="cuda:0", single_pass=True, tf32x1=False, unfused
                                   single_pass=single_pass, tf32x1=tf32x1, return_pred=True, morton_ordered=morton_ordered)
     loss.backward()
     torch.cuda.synchronize()
+    if frozen is not None:
+        check_frozen_grads(dec, frozen)
     return {
         "indices": indices, "feature": feature.detach().cpu().numpy(), "pred": pred.detach().cpu().numpy(),
         "loss": float(loss.detach()),

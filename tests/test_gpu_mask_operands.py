@@ -10,6 +10,7 @@ import torch
 
 from tests.parity_utils import (compare_step, drop_relu_kink_points, make_case, run_cuda_step, run_oracle_step,
                                 sort_case_morton)
+from tests.test_gpu_replicas import grade_run
 from tests.test_gpu_rounds import TILE, _far, _tiles_per_round
 
 pytestmark = pytest.mark.gpu
@@ -46,18 +47,21 @@ def _dec(case, key):
 
 
 def _grade(case, frozen=False, kink_eps=2e-6):
-    """Every training flavour against the oracle on the points whose decoder pre-activations are farther than kink_eps
+    """Every training flavour against the oracle, and element by element against the fp64 bounds
+    (test_gpu_replicas.grade_run), on the points whose decoder pre-activations are farther than kink_eps
     from zero (tests/parity_utils.drop_relu_kink_points); returns the runs as {name: result}."""
     case, _ = drop_relu_kink_points(case, kink_eps)
     want = run_oracle_step(case)
     if frozen:
         want = dict(want); want["dec_grads"] = {}
-    runs = {}
+    runs, ref = {}, None
     for name, kw in (("per-point", {}), ("grouped", {"morton_ordered": True})):
         runs[name] = run_cuda_step(case, DEV, freeze_decoder=frozen, **kw)
         print(name, compare_step(runs[name], want))
+        ref = grade_run(case, runs[name], "mask operands", ref=ref, **kw)
     runs["tf32x1"] = run_cuda_step(case, DEV, freeze_decoder=frozen, tf32x1=True)
     print("tf32x1", compare_step(runs["tf32x1"], want, **TF32X1))
+    grade_run(case, runs["tf32x1"], "mask operands", tf32x1=True)
     return runs
 
 

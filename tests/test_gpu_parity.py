@@ -8,6 +8,7 @@ import torch
 
 from tests.parity_utils import (DEC_KEYS, GOLDEN_NAMES, build_cuda_models, compare_step, load_eikonal_golden, load_golden,
                                 make_case, run_cuda_step, run_oracle_step, sort_case_morton)
+from tests.test_gpu_replicas import grade_run
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -57,9 +58,13 @@ def test_grouped_scatter_matches_oracle(levels, poly, weighted, reduction, order
     if ordered:
         case = sort_case_morton(case)
     want = run_oracle_step(case)
-    print(compare_step(run_cuda_step(case, DEV, morton_ordered=True), want))
+    got = run_cuda_step(case, DEV, morton_ordered=True)
+    print(compare_step(got, want))
+    ref = grade_run(case, got, f"grouped scatter L={levels} ordered={ordered}", morton_ordered=True)
     want_f = dict(want); want_f["dec_grads"] = {}
-    print(compare_step(run_cuda_step(case, DEV, morton_ordered=True, freeze_decoder=True), want_f))
+    got = run_cuda_step(case, DEV, morton_ordered=True, freeze_decoder=True)
+    print(compare_step(got, want_f))
+    grade_run(case, got, f"grouped scatter L={levels} ordered={ordered} frozen", morton_ordered=True, ref=ref)
 
 
 @pytest.mark.parametrize("ordered,weighted,reduction,frozen", [(True, False, "mean", False), (False, True, "sum", False),
@@ -87,8 +92,11 @@ def test_all_miss_tiles_match_oracle(ordered, weighted, reduction, frozen):
         assert bool(missed_everywhere[k:k + far.shape[0]].all())
     if frozen:
         want = dict(want); want["dec_grads"] = {}
+    ref = None
     for flag in (False, True):
-        print(compare_step(run_cuda_step(case, DEV, morton_ordered=flag, freeze_decoder=frozen), want))
+        got = run_cuda_step(case, DEV, morton_ordered=flag, freeze_decoder=frozen)
+        print(compare_step(got, want))
+        ref = grade_run(case, got, f"all-miss tiles ordered={ordered}", morton_ordered=flag, ref=ref)
 
 
 def test_all_miss_batch():
@@ -112,7 +120,9 @@ def test_grouped_scatter_dense_runs():
     case["label"] = rng.uniform(-0.05, 0.05, size=coord.shape[0]).astype(np.float32)
     case["weight"] = np.ones(coord.shape[0], dtype=np.float32)
     case = sort_case_morton(case)
-    print(compare_step(run_cuda_step(case, DEV, morton_ordered=True), run_oracle_step(case)))
+    got = run_cuda_step(case, DEV, morton_ordered=True)
+    print(compare_step(got, run_oracle_step(case)))
+    grade_run(case, got, "dense runs", morton_ordered=True)
 
 
 @pytest.mark.parametrize("n_batch", [0, 1, 15, 16, 17, 255])

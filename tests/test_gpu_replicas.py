@@ -42,10 +42,14 @@ its error E_j:
 Points within twice the forward error of a ReLU kink are dropped from the fused cases: there a correct fp32 kernel may take
 the other branch.  `compare_step` (2e-4 of the level maximum) runs as a second check, and each case prints its worst
 error / bound.
+The decoder gradients of every step are graded element by element too, by the model of tests/decoder_bound.py; the
+grouped kernel's table rows count the adds that land on them (one per (tile, node) of a grouped tile, one per (point,
+corner) of a scattered one: error_bound.grouped_counts) instead of the (point, corner) terms.
 The eikonal paths extend this model (blend-weight derivatives, g, gamma and the eikonal scatter): tests/eikonal_bound.py.
 The pieces both use (eps_mm, the fp32 blend, the decoder passes, the kink filter, the grading loop) live in
 tests/error_bound.py.
 """
+import copy
 import ctypes as C
 
 import numpy as np
@@ -54,12 +58,14 @@ import torch
 
 from oracle import shine_oracle as orc
 from tests import sdf_diff_oracle as sdo
-from tests.error_bound import C_SLACK, U, drop_kinks, eps_mm, grade_tables, subset
+from tests.decoder_bound import DecoderRef, kernel_depth
+from tests.error_bound import C_SLACK, U, drop_kinks, eps_mm, grade_tables, grouped_counts, subset
 from tests.error_bound import abs_feature as _abs_feature
 from tests.error_bound import blend as _blend
 from tests.error_bound import decoder_passes as _decoder_passes
 from tests.error_bound import oracle64 as _oracle64
-from tests.parity_utils import build_cuda_models, compare_step, make_case, oracle_from_case, sort_case_morton
+from tests.parity_utils import (FROZEN_SENTINEL, build_cuda_models, compare_step, make_case, oracle_from_case,
+                                sort_case_morton)
 from tests.test_gpu_sdf_diff import _scale
 
 DEV = "cuda:0"
@@ -129,12 +135,14 @@ class Ref:
     """fp64 oracle step of a case (or the fp64 query backward of a given dfeat), with S, k and T per row.
     loss_type: the step's loss; sdf_l1 needs `pred`, the kernel's pred of the step being graded (module docstring)."""
 
-    def __init__(self, case, dfeat=None, tf32x1=False, grouped=False, loss_type="sdf_bce", pred=None):
+    def __init__(self, case, dfeat=None, tf32x1=False, grouped=False, loss_type="sdf_bce", pred=None, replicas=None):
         c = case["cfg"]
         o, dec = _oracle64(case)
         coord = torch.from_numpy(case["coord"])
         n, L, F = coord.shape[0], c["tree_level_feat"], c["feature_dim"]
         self.n, self.tables, self.slack = n, case["tables"], C_SLACK + (eps_mm(16) / U if grouped else 0)
+        self.dec = None
+        env = torch.zeros(n, F, dtype=torch.float64)
         if dfeat is None:
             label = torch.from_numpy(case["label"]).double()
             weight = torch.from_numpy(case["weight"]).double()
@@ -170,6 +178,18 @@ class Ref:
                 else:
                     dg = 6 * U * g.abs()
                 E = dp["D"] * (dp["ebwd"] * g.abs() + dg)[:, None]
+                # kink points (kept only by the tile-layout tests): |dL/dpred| of the kernel at most gmax, dfeat within
+                # the envelope with the uncertain units live, E = 2 x envelope (tests/decoder_bound.py)
+                s_l = weight.abs() / n
+                gmax = s_l / scale * (1 + 6 * U) if loss_type == "sdf_l1" else g.abs() + dg     # dg from the kink P
+                kink = dp["kink"]
+                if bool(kink.any()):
+                    W1a, W2a, w3a = (dd[k].abs() for k in ("layers.0.weight", "layers.1.weight", "lout.weight"))
+                    Dhi = (dp["m1_hi"] * ((dp["m2_hi"] * w3a) @ W2a)) @ W1a
+                    env = torch.where(kink[:, None], Dhi * gmax[:, None] * (1 + 1e-5), env)
+                    E = torch.where(kink[:, None], 2 * env, E)
+                self.dec = DecoderRef(feat, dp, dd, g.detach(), dg, gmax, tf32x1, grouped)
+                self.feat64, self.g64, self.dec64 = feat.detach(), g.detach(), dd     # for per-tile contributions
             self.P = dp["P"].numpy()
             self.kink = dp["kink"].numpy()
             self.kinks = int(dp["kink"].sum())
@@ -182,25 +202,55 @@ class Ref:
             self.P, self.kink, self.kinks = None, np.zeros(n, dtype=bool), 0
         self.dfeat = dfeat64.detach().numpy()
         pts = torch.arange(n).repeat_interleave(8)
-        self.S, self.k, self.T = [None] * L, [None] * L, [None] * L
+        self.S, self.k, self.T, self._ix = [None] * L, [None] * L, [None] * L, [None] * L
         for i, (ix, w) in enumerate(_blend(o, coord)):
             kk = L - 1 - i
             rows = self.want[kk].shape[0]
             hit = ix >= 0
             r, wj, pj = ix[hit], w[hit][:, None], pts[hit]
-            self.S[kk] = torch.zeros(rows, F, dtype=torch.float64).index_add_(0, r, wj * dfeat64.abs()[pj]).numpy()
+            mag = torch.maximum(dfeat64.detach().abs(), env)
+            self.S[kk] = torch.zeros(rows, F, dtype=torch.float64).index_add_(0, r, wj * mag[pj]).numpy()
             self.T[kk] = torch.zeros(rows, F, dtype=torch.float64).index_add_(0, r, wj * E[pj]).numpy()
+            self._ix[kk] = ix.numpy().reshape(n, 8)
             self.k[kk] = torch.bincount(r, minlength=rows).numpy()
+        self._k_points = self.k
+        if grouped:
+            self.k = self._grouped_k(replicas)
+
+    def _grouped_k(self, replicas):
+        """k_u of the grouped kernel (error_bound.grouped_counts), plus the R - 1 adds of the replica fold."""
+        out = []
+        for kk, ix in enumerate(self._ix):
+            kg = grouped_counts(ix, self.want[kk].shape[0])
+            out.append(kg + np.where(kg > 0, (1 if replicas is None else replicas[kk]) - 1, 0))
+        return out
+
+    def for_kernel(self, grouped):
+        """The same reference graded for the grouped kernel at R = 1 (its k_u, EPS_MM(16), two-product dW2) or for the
+        per-point kernels."""
+        out = copy.copy(self)
+        out.slack = C_SLACK + (eps_mm(16) / U if grouped else 0)
+        out.k = self._grouped_k(None) if grouped else self._k_points
+        if self.dec is not None:
+            out.dec = copy.copy(self.dec)
+            out.dec.grouped = grouped
+        return out
 
     def grade(self, got_tables, what, pred=None):
         """Every element of every level (trash row excluded) against its bound -> worst error / bound."""
         bounds = [(k[:, None] + self.slack) * U * S + T for S, k, T in zip(self.S, self.k, self.T)]
         worst = grade_tables(got_tables, self.want, bounds, self.k, self.S, what, "replica bounds")
-        if pred is not None:
+        if pred is not None:      # every point, kink points with their wider P (error_bound.decoder_passes)
             e = np.abs(np.asarray(pred, dtype=np.float64) - self.pred)
             assert (e <= self.P).all(), f"{what}: pred outside its bound at {int((e > self.P).sum())} points"
             print(f"[replica bounds] {what}: pred worst {float((e / self.P).max()):.3f} of the bound")
         return worst
+
+    def grade_decoder(self, dec_grads, what, chunks=1):
+        """Every decoder-gradient element against the bound of tests/decoder_bound.py at the kernel's depth for this batch."""
+        sms = torch.cuda.get_device_properties(0).multi_processor_count if torch.cuda.is_available() else None
+        depth = kernel_depth(self.n, chunks, sms) if sms else kernel_depth(self.n, chunks)
+        return self.dec.grade(dec_grads, depth, what)
 
     def compare(self, got_tables, pred, loss, dec_grads, tf32x1=False):
         """compare_step on the same step (fp32-graded quantities: loss, pred, decoder gradients)."""
@@ -210,6 +260,22 @@ class Ref:
                 "table_grads": self.want, "dec_grads": {k: self.step["dec_grads"][k] for k in dec_grads}}
         kw = dict(pred_atol=5e-3, pred_rtol=5e-3, grad_rel=3e-2) if tf32x1 else {}
         return compare_step(got, want, **kw)
+
+
+def grade_run(case, got, what, loss_type="sdf_bce", morton_ordered=False, tf32x1=False, ref=None):
+    """The per-element grade of one step's result (the dict of parity_utils.run_cuda_step / test_gpu_sdf_diff._cuda_step):
+    pred, every table-gradient element (the grouped kernel's k_u where the Morton flag picks it: up to 4 levels, 3xTF32)
+    and every decoder-gradient element unless the decoder was frozen.  ref: a Ref of the case to reuse (not for sdf_l1,
+    whose reference follows the kernel's pred).  -> the Ref."""
+    grouped = morton_ordered and case["cfg"]["tree_level_feat"] <= 4 and not tf32x1
+    if ref is None:
+        ref = Ref(case, tf32x1=tf32x1, loss_type=loss_type, pred=got["pred"])
+    graded = ref.for_kernel(grouped)
+    what = f"{what} {'grouped' if grouped else 'per-point'} {loss_type}"
+    graded.grade(got["table_grads"], what, got["pred"])
+    if got["dec_grads"]:
+        graded.grade_decoder(got["dec_grads"], what)
+    return ref
 
 
 # ---- running the kernels -------------------------------------------------------------------------------------------------
@@ -227,29 +293,49 @@ def trainer(case, freeze=False, main_loss_type="sdf_bce", **kw):
 
 
 def train_step(tr, case, morton_ordered=None):
+    """One step; a frozen decoder's gradient segment is filled with a sentinel first and must come back bit for bit."""
     coord, label, weight = _dev(case)
     tr.zero_grad()
+    if not tr._dec_trainable:
+        tr.dec_flat.fill_(FROZEN_SENTINEL)
+        before = tr.dec_flat.clone()
     pred = torch.empty(coord.shape[0], device=DEV)
     loss = float(tr.forward_backward(coord, label, weight, pred_out=pred, morton_ordered=morton_ordered))
     torch.cuda.synchronize()
+    if not tr._dec_trainable:
+        assert torch.equal(tr.dec_flat.view(torch.int32), before.view(torch.int32)), \
+            "a frozen decoder's gradient buffer was written"
     tables = [g.detach().cpu().numpy().copy() for g in tr.table_grads]
-    dec = {k: g.detach().cpu().numpy().copy() for k, g in zip(("layers.0.weight", "layers.0.bias", "layers.1.weight",
-                                                                "layers.1.bias", "lout.weight", "lout.bias"), tr.dec_grads)
-           if g is not None and tr._dec_trainable}
-    return tables, pred.cpu().numpy(), loss, dec
+    return tables, pred.cpu().numpy(), loss, dec_grads(tr)
 
 
-def check_step(tr, spy, case, ref, what, tf32x1=False, morton_ordered=None, grouped=False):
-    """One trainer step: R per level as expected, every element within its bound, compare_step, scratch all zero.
-    ref None: the Ref of the trainer's loss, built after the step from the pred it returned."""
+def dec_grads(tr):
+    return {k: g.detach().cpu().numpy().copy() for k, g in zip(("layers.0.weight", "layers.0.bias", "layers.1.weight",
+                                                                 "layers.1.bias", "lout.weight", "lout.bias"), tr.dec_grads)
+            if g is not None and tr._dec_trainable}
+
+
+def check_step(tr, spy, case, ref, what, tf32x1=False, morton_ordered=None, grouped=False, replicas=True):
+    """One trainer step: R per level as expected, compare_step, every element within its bound (tables, pred and decoder
+    gradients), scratch all zero.  ref None: the Ref of the trainer's loss, built after the step from the pred it
+    returned.  replicas=False: a step that runs at R = 1 (no replica fold)."""
     tables, pred, loss, dec = train_step(tr, case, morton_ordered)
     if ref is None:
-        ref = Ref(case, tf32x1=tf32x1, grouped=grouped, loss_type=tr.main_loss_type, pred=pred)
+        ref = Ref(case, tf32x1=tf32x1, grouped=grouped, loss_type=tr.main_loss_type, pred=pred,
+                  replicas=expected_replicas(case["tables"], case["coord"].shape[0]) if replicas else None)
     what = f"{what} {tr.main_loss_type}"
-    spy.expect(expected_replicas(case["tables"], ref.n), what)
-    worst = ref.grade(tables, what, pred)
+    if replicas:
+        spy.expect(expected_replicas(case["tables"], ref.n), what)
+    else:       # no fold with R > 1, and no replica scratch ever allocated
+        assert all(max(r) == 1 for r in spy.calls), f"{what}: the step ran with replicas {spy.calls}"
+        assert not tr.octree._grad_scratch, f"{what}: replica scratch was allocated"
+        spy.calls.clear()
     print(what, ref.compare(tables, pred, loss, dec, tf32x1))
-    assert_scratch_zero(tr.octree, what)
+    worst = ref.grade(tables, what, pred)
+    if tr._dec_trainable:
+        ref.grade_decoder(dec, what)
+    if replicas:
+        assert_scratch_zero(tr.octree, what)
     return worst
 
 
@@ -347,6 +433,79 @@ def test_grouped_kernel_with_replicas(ordered, loss_type, force):
     tr.grouped_replicas = True
     check_step(tr, spy, case, None, f"grouped ordered={ordered} (kinks dropped: {dropped})", morton_ordered=True,
                grouped=True)
+
+
+def _far_tiles(case, tiles, at, seed, weight=None):
+    """The case with `tiles` tiles of points outside every node (zero tiles) inserted at tile `at`; weight: their weight
+    (0: their dL/dpred is exactly 0), None: random weights in [0.5, 1.5)."""
+    rng = np.random.default_rng(seed)
+    m = 16 * tiles
+    far = {"coord": rng.uniform(0.6, 0.9, size=(m, 3)).astype(np.float32),
+           "label": rng.uniform(-0.2, 0.2, size=m).astype(np.float32),
+           "weight": (rng.uniform(0.5, 1.5, size=m) if weight is None else np.full(m, weight)).astype(np.float32)}
+    out = dict(case)
+    for k in ("coord", "label", "weight"):
+        out[k] = np.ascontiguousarray(np.concatenate((case[k][:16 * at], far[k], case[k][16 * at:])))
+    return out
+
+
+def _grouped_layout(layout, seed):
+    """Morton-ordered batches for the grouped kernel at R = 1 (module docstring of the grouped cases below)."""
+    from tests.test_gpu_rounds import _tiles_per_round
+    per_round = _tiles_per_round()
+    if layout == "zero-block":                  # one round: block 0 holds tiles 0-7, all zero tiles
+        case = sort_case_morton(drop_kinks(make_case(n_points=2500, n_batch=(per_round // 2 - 16) * 16, feat_levels=4,
+                                                     seed=seed, weighted=True))[0])
+        return _far_tiles(case, 8, 0, seed)
+    case = sort_case_morton(drop_kinks(make_case(n_points=2500, n_batch=2 * per_round * 16 + 40, feat_levels=4,
+                                                 seed=seed, weighted=True))[0])
+    if layout == "scattered":                   # 64 tiles in the order drawn: more than kMaxGroupedRuns nodes per tile
+        rng = np.random.default_rng(seed)
+        sl = np.arange(16 * per_round, 16 * (per_round + 64))
+        perm = np.arange(case["coord"].shape[0])
+        perm[sl] = rng.permutation(sl)
+        case = subset(case, perm)
+        return _far_tiles(case, 24, per_round // 2, seed)
+    # zero-sum: block 0's tiles 0-7 are zero tiles of weight 0 (its dL/dpred sum is exactly 0), more zero tiles later
+    return _far_tiles(_far_tiles(case, 40, per_round + 3, seed), 8, 0, seed + 1, weight=0.0)
+
+
+@gpu
+@pytest.mark.parametrize("layout,loss_type", [pytest.param(lo, "sdf_bce", id=lo) for lo in ("scattered", "zero-block",
+                                                                                               "zero-sum")] +
+                         [pytest.param("scattered", lt, id=f"scattered-{lt}") for lt in DIFF_LOSSES])
+def test_grouped_kernel_at_one_replica(layout, loss_type):
+    """The Morton-ordered kernel as the batch loop runs it, at R = 1: batches over more than two grid-stride rounds with
+    a stretch of scattered tiles (more than kMaxGroupedRuns nodes on a level: per-point scatter inside the grouped kernel)
+    and zero tiles in mid-batch; one round whose block 0 holds only zero tiles; and a block whose zero-tile dL/dpred sum is
+    exactly 0 (weight 0), which skips its virtual backward tile."""
+    from tests.error_bound import oracle64
+    case = with_weights(_grouped_layout(layout, 500 + len(layout)), loss_type, 7)
+    o, _ = oracle64(case)
+    idx = o.get_indices(torch.from_numpy(case["coord"]))
+    runs = [grouped_counts(ix.numpy().reshape(-1, 8), 1 + int(ix.max())).sum() for ix in idx]
+    # the layout really is what it claims: zero tiles (every point misses every level) where they were put
+    n = case["coord"].shape[0]
+    miss = np.logical_and.reduce([(ix.numpy().reshape(n, -1) < 0).all(1) for ix in idx])
+    zero = np.concatenate((miss, np.ones(-n % 16, bool))).reshape(-1, 16).all(1)
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    if layout == "zero-block":
+        assert zero[:8].all() and not zero[8:].all(), "block 0 does not hold only zero tiles"
+        assert zero.shape[0] <= 8 * sms, "more than one round: block 0 would get more tiles"
+    elif layout == "zero-sum":
+        assert zero[:8].all() and not case["weight"][:128].any(), "block 0's zero tiles do not sum to exactly 0"
+        assert zero[8:].sum() >= 40 and np.abs(case["weight"][16 * 8:][np.repeat(zero[8:], 16)[:n - 128]]).min() > 0
+    else:
+        assert zero[1:-1].sum() >= 24, "no zero tiles in mid-batch"
+    print(f"[grouped R=1] {layout}: {int(zero.sum())} zero tiles of {zero.shape[0]}")
+    if layout == "scattered":
+        leaf = idx[0].numpy().reshape(-1, 8)[:, 0]
+        node = np.concatenate((leaf, np.full(-leaf.shape[0] % 16, -1))).reshape(-1, 16)
+        nruns = [len(set(r[r >= 0].tolist())) for r in node]
+        assert max(nruns) > 6, "no scattered tile"
+        print(f"[grouped R=1] {layout}: {sum(x > 6 for x in nruns)} scattered tiles of {len(nruns)}; adds per level {runs}")
+    tr, spy = trainer(case, morton_ordered=True, main_loss_type=loss_type)
+    check_step(tr, spy, case, None, f"grouped R=1 {layout}", morton_ordered=True, grouped=True, replicas=False)
 
 
 @gpu
@@ -510,6 +669,7 @@ def test_step_from_host_chunks_with_different_replica_counts(force):
         print(f"[replicas] {what}: R per level of the chunks {want}")
         ref = Ref(c, loss_type=loss_type, pred=pred)
         ref.grade([g.detach().cpu().numpy() for g in tr.table_grads], what)
+        ref.grade_decoder(dec_grads(tr), what, chunks=3)
         assert_scratch_zero(tr.octree, what)
 
 
@@ -529,6 +689,7 @@ def test_capture_step_replays_on_changed_data(force):
         graph = tr.capture_step(coord, label, weight, exchange=False)
         spy.expect(expected_replicas(a["tables"], n), f"capture {loss_type}")
         refs["A"].grade([g.detach().cpu().numpy() for g in tr.table_grads], f"capture warm-up on A {loss_type}")
+        refs["A"].grade_decoder(dec_grads(tr), f"capture warm-up on A {loss_type}")
         for name in ("B", "A", "B"):
             src = _dev(b if name == "B" else a)
             for dst, s in zip((coord, label, weight), src):
@@ -536,6 +697,7 @@ def test_capture_step_replays_on_changed_data(force):
             graph.replay()
             torch.cuda.synchronize()
             refs[name].grade([g.detach().cpu().numpy() for g in tr.table_grads], f"replay on {name} {loss_type}")
+            refs[name].grade_decoder(dec_grads(tr), f"replay on {name} {loss_type}")
             assert_scratch_zero(tr.octree, f"replay on {name} {loss_type}")
 
 

@@ -9,6 +9,7 @@ import torch
 
 from tests import test_gpu_sdf_diff as sdd
 from tests.parity_utils import compare_step, make_case, run_cuda_step, run_oracle_step, sort_case_morton
+from tests.test_gpu_replicas import grade_run
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -62,15 +63,18 @@ def _spans_rounds(case, k=2):
 
 
 def _check(case, frozen=False, loss_type="sdf_bce", zero_labels=None):
-    """Both kernel flavours against the oracle.  sdf_l1 / sdf_l2 go through test_gpu_sdf_diff's step and fp64 oracle (the
+    """Both kernel flavours against the oracle, and element by element against the fp64 bounds (test_gpu_replicas.grade_run).  sdf_l1 / sdf_l2 go through test_gpu_sdf_diff's step and fp64 oracle (the
     L1 sign of the kernel's pred where it is within the pred tolerance of the label).  zero_labels (sdf_l1): indices of
     samples that get the pred the kernel returned for them as label, an exact zero difference inside the zero-tile sum."""
     if loss_type == "sdf_bce":
         want = run_oracle_step(case)
         if frozen:
             want = dict(want); want["dec_grads"] = {}
+        ref = None
         for grouped in (False, True):
-            print(compare_step(run_cuda_step(case, DEV, morton_ordered=grouped, freeze_decoder=frozen), want))
+            got = run_cuda_step(case, DEV, morton_ordered=grouped, freeze_decoder=frozen)
+            print(compare_step(got, want))
+            ref = grade_run(case, got, "rounds", morton_ordered=grouped, ref=ref)
         return
     for grouped in (False, True):
         kw = dict(morton_ordered=grouped, freeze_decoder=frozen)
@@ -83,6 +87,7 @@ def _check(case, frozen=False, loss_type="sdf_bce", zero_labels=None):
             assert np.array_equal(got["pred"][zero_labels], c["label"][zero_labels])
         want = sdd._drop_frozen(sdd._oracle(c, loss_type, got["pred"]), frozen)
         print(loss_type, "grouped" if grouped else "per-point", compare_step(got, want))
+        grade_run(c, got, "rounds", loss_type, morton_ordered=grouped)
 
 
 DIFF_LOSSES = ("sdf_l1", "sdf_l2")

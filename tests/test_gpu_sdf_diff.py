@@ -7,8 +7,8 @@ import pytest
 import torch
 
 from tests import sdf_diff_oracle as sdo
-from tests.parity_utils import (GOLDEN_DIR, build_cuda_models, compare_step, drop_relu_kink_points, make_case,
-                                make_config, oracle_from_case, sort_case_morton)
+from tests.parity_utils import (GOLDEN_DIR, build_cuda_models, check_frozen_grads, compare_step, drop_relu_kink_points,
+                                fill_frozen_grads, make_case, make_config, oracle_from_case, sort_case_morton)
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -35,6 +35,7 @@ def _cuda_step(case, loss_type, **kw):
     from shine_mapping_b200.fused import sdf_diff_step
     freeze = kw.pop("freeze_decoder", False)
     cfg, octree, dec = build_cuda_models(case, DEV, freeze_decoder=freeze)
+    frozen = fill_frozen_grads(dec) if freeze else None
     coord, label, weight = (torch.from_numpy(np.ascontiguousarray(case[k])).to(DEV) for k in ("coord", "label", "weight"))
     indices = [t.cpu().numpy() for t in octree.get_indices(coord)]
     feature = octree.query_feature(coord)
@@ -42,6 +43,8 @@ def _cuda_step(case, loss_type, **kw):
                                return_pred=True, **kw)
     loss.backward()
     torch.cuda.synchronize()
+    if frozen is not None:
+        check_frozen_grads(dec, frozen)
     named = dict(dec.named_parameters())
     return {"indices": indices, "feature": feature.detach().cpu().numpy(), "pred": pred.cpu().numpy(),
             "loss": float(loss.detach()), "table_grads": [p.grad.cpu().numpy() for p in octree.hier_features],
