@@ -543,6 +543,29 @@ int shine_nn_build(const double* points, int64_t n, void* tree, int64_t tree_byt
 int shine_nn_query(const void* tree, int64_t n, const double* queries, int64_t m, double radius2, double* dist,
                    int32_t* index, void* scratch, int64_t scratch_bytes, void* stream);
 
+/* ---- scan-to-map registration: one Gauss-Newton system of a scan against the SDF map (odometry.py) ------------------
+ * For every point p_i of points (device fp32 [n,3], sensor frame, scaled coordinates) and the pose T (host fp64, 4x4
+ * row-major, translation scaled; row 3 is not read), with R and t rounded to fp32:
+ *   q = R p + t              fp32, per row ((R0 x + R1 y) + R2 z) + t, every operation rounded on its own;
+ *   r = sigma pred(q)        pred as shine_sdf_infer computes it (fp32 FMA chains here), sigma = sigma_sigmoid: the SDF;
+ *   g = sigma dpred/dq       back through the ReLU masks to the feature, then through the blend weights
+ *                            (shine_query_coord_grad's derivatives);
+ *   valid                    q's voxel exists at lv[0]; other points contribute nothing;
+ *   Jr = [g, q x g]          the Jacobian of r for a left-multiplied twist (rho, phi), in fp64 from the fp32 q and g;
+ *   w = (k^2 / (k^2 + r^2))^2  Geman-McClure weight in fp64, k = kappa (scaled units).
+ * out (device fp64 [SHINE_REGISTER_OUT]) = the 21 entries of sum w Jr^T Jr (upper triangle, row-major: (0,0), (0,1) ..
+ * (0,5), (1,1) ..), the 6 of sum w Jr^T r, sum w r^2 and the number of valid points.  Per-thread fp64 sums, block
+ * partials into scratch (device, 8-byte aligned, >= SHINE_REGISTER_SCRATCH_BYTES), a second launch adds them in a fixed
+ * order: the result does not change from run to run.  n = 0 writes zeros.  NULL pointers, n < 0, a non-positive or
+ * non-finite kappa or sigma, a non-finite pose entry and a short scratch are SHINE_ERR_INVALID_ARG; a decoder other than
+ * 8 -> 32 -> 32 -> 1 is SHINE_ERR_UNSUPPORTED; none of them launches. */
+#define SHINE_REGISTER_OUT 29
+#define SHINE_REGISTER_MAX_BLOCKS 1024
+#define SHINE_REGISTER_SCRATCH_BYTES (SHINE_REGISTER_MAX_BLOCKS * SHINE_REGISTER_OUT * 8)
+int shine_register_normal_eq(const shine_octree* oct, const shine_decoder* dec, const float* points, int64_t n,
+                             const double* pose, float sigma, double kappa, double* out, void* scratch,
+                             int64_t scratch_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -23,6 +23,8 @@ FLAG_TF32X1 = 4
 FLAG_MORTON_ORDERED = 16
 FLAG_LOSS_L2 = 32
 ERR_CAPACITY = -3
+REGISTER_OUT = 29
+REGISTER_SCRATCH_BYTES = 1024 * REGISTER_OUT * 8
 
 
 class ShineLevel(C.Structure):
@@ -187,6 +189,8 @@ SYMBOLS = {
     "shine_nn_scratch_bytes": (C.c_int64, [_i64]),
     "shine_nn_build": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _i64, _vp]),
     "shine_nn_query": (C.c_int, [_vp, _i64, _vp, _i64, C.c_double, _vp, _vp, _vp, _i64, _vp]),
+    "shine_register_normal_eq": (C.c_int, [_OCT, _DEC, _vp, _i64, C.POINTER(C.c_double), _f32, C.c_double, _vp, _vp,
+                                           _i64, _vp]),
 }
 
 _lib = None

@@ -20,6 +20,7 @@ from __future__ import annotations
 
 import ctypes as C
 import math
+import os
 
 import numpy as np
 import torch
@@ -437,3 +438,36 @@ def build_scene_map(config: SHINEConfig, octree, n_azimuth: int, n_frames: int =
         pool.append(coord, label, weight)
         pool.map_bbx = _mesher.surface_bbx(coord, weight, config.scale, getattr(pool, "map_bbx", None))   # for bbx meshing
     return pool
+
+
+def drive_poses(n_frames: int, step_m: float = 1.5, sway_m: float = 1.0, yaw_amp: float = 0.15) -> list:
+    """World poses (4x4 fp64, metres) of a smooth drive along the street: x = step_m f, y = sway_m sin(0.3 f),
+    yaw = yaw_amp sin(0.3 f) (at most 0.3 yaw_amp rad per frame).  Frame 0 is the identity."""
+    poses = []
+    for f in range(n_frames):
+        yaw = yaw_amp * math.sin(0.3 * f)
+        T = np.eye(4)
+        T[:3, :3] = [[math.cos(yaw), -math.sin(yaw), 0.0], [math.sin(yaw), math.cos(yaw), 0.0], [0.0, 0.0, 1.0]]
+        T[:3, 3] = (step_m * f, sway_m * math.sin(0.3 * f), 0.0)
+        poses.append(T)
+    return poses
+
+
+def write_drive(root: str, n_frames: int = 20, step_m: float = 1.5, n_azimuth: int = 512, max_range: float = 40.0) -> dict:
+    """A LiDAR sequence of the analytic street seen along `drive_poses`: root/scans/{f}.bin (KITTI float32 x y z i, sensor
+    frame) and root/poses.txt (KITTI rows of the world poses, for a calib_path of "").  -> dict(pc_path, pose_path,
+    poses) with the world poses."""
+    os.makedirs(os.path.join(root, "scans"), exist_ok=True)
+    poses = drive_poses(n_frames, step_m)
+    dirs = lidar_directions(n_azimuth).double()
+    rows = []
+    for f, W in enumerate(poses):
+        hits = raycast_scene(torch.tensor(W[:3, 3]), (torch.tensor(W[:3, :3]) @ dirs.T).T.float(), default_boxes(),
+                             min_range=1.0, max_range=max_range).double().numpy()
+        local = (hits - W[:3, 3]) @ W[:3, :3]
+        rec = np.concatenate((local.astype(np.float32), np.ones((len(local), 1), np.float32)), 1)
+        rec.tofile(os.path.join(root, "scans", f"{f}.bin"))
+        rows.append(" ".join(repr(float(v)) for v in W[:3].reshape(-1)))
+    with open(os.path.join(root, "poses.txt"), "w") as fh:
+        fh.write("\n".join(rows) + "\n")
+    return dict(pc_path=os.path.join(root, "scans"), pose_path=os.path.join(root, "poses.txt"), poses=poses)
