@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define SHINE_ABI_VERSION 4
+#define SHINE_ABI_VERSION 5
 #define SHINE_MAX_LEVELS 8
 #define SHINE_HASH_SLOT_BYTES 64
 
@@ -40,18 +40,20 @@ extern "C" {
 #define SHINE_ERR_UNSUPPORTED (-2)
 #define SHINE_ERR_CAPACITY (-3)   /* an output buffer was too small; what fitted was written */
 
-/* flags of shine_sdf_* calls; shine_sdf_infer, shine_sdf_bce_fwd and shine_sdf_bce_step return SHINE_ERR_UNSUPPORTED
- * for any other bit (ABI version 3 also defined bit 8) */
+/* flags of shine_sdf_* calls; each call names the bits it accepts and returns SHINE_ERR_UNSUPPORTED for any other bit
+ * (ABI version 3 also defined bit 8) */
 #define SHINE_FLAG_REDUCTION_SUM 1u   /* loss_reduction == "sum" (shine_incre.py:77-78); default mean   */
 #define SHINE_FLAG_WEIGHTED 2u        /* loss_weight_on (utils/loss.py:18-19): per-sample weight applied */
 #define SHINE_FLAG_TF32X1 4u          /* decoder contractions in plain TF32 (default: 3xTF32 ~ fp32)     */
-#define SHINE_FLAG_MORTON_ORDERED 16u  /* shine_sdf_bce_step: the batch is in Morton order of its coordinates (the order the
+#define SHINE_FLAG_MORTON_ORDERED 16u  /* shine_sdf_step: the batch is in Morton order of its coordinates (the order the
                                          Morton-sorted sample pool hands batches out in).  A hint, never a requirement:
                                          neighbouring points then share nodes, and the step sums the gradients of each run of
                                          equal node on the tensor cores before ONE red per corner row (results equal up to
                                          fp32 summation order); on an unordered batch the flag only costs time           */
-#define SHINE_FLAG_LOSS_L2 32u         /* shine_sdf_diff_*: sdf_diff_loss with l2_loss=True (main_loss_type sdf_l2); without
-                                         it the loss is L1 (sdf_l1).  The other shine_sdf_* calls refuse the bit          */
+#define SHINE_FLAG_LOSS_L2 32u         /* the point-wise loss of shine_sdf_fwd / _step / _eikonal_step: sdf_diff_loss with
+                                         l2_loss=True (main_loss_type sdf_l2; shine_batch.py:171-179)                     */
+#define SHINE_FLAG_LOSS_L1 64u         /* the same with l2_loss=False (sdf_l1).  Neither loss bit: sdf_bce_loss (sdf_bce);
+                                         both: SHINE_ERR_UNSUPPORTED                                                      */
 
 /* One featured level of the FeatureOctree (model/feature_octree.py:46-63). */
 typedef struct shine_level {
@@ -138,35 +140,36 @@ int shine_query_tangent_bwd(const shine_octree* oct, const float* coord, int64_t
 int shine_sdf_infer(const shine_octree* oct, const shine_decoder* dec, const float* coord, int64_t n,
                     float* out_pred, uint8_t* out_mask, int32_t mask_level, uint32_t flags, void* stream);
 
-/* query_feature -> Decoder.sdf -> sdf_bce_loss (utils/loss.py:17-24), forward only.
- * label [n], weight [n] or NULL, sigma = sigma_sigmoid (shine_batch.py:87).
- * out_loss [1] fp32 is ACCUMULATED (+=): caller zeroes it.  loss_scale multiplies every per-point term
- * (1/N_global for "mean", 1 for "sum"). */
+/* query_feature -> Decoder.sdf -> the point-wise loss (shine_batch.py:171-179), forward only.  The loss bits of flags
+ * pick the loss; with z = sigmoid(label / sigma) and d = (pred - label) / scale (metres):
+ *   sdf_bce (no loss bit)   sdf_bce_loss  (utils/loss.py:17-24)  L = sum w (max(pred, 0) - pred z + log(1 + exp(-|pred|)))
+ *                           with w = |weight| under SHINE_FLAG_WEIGHTED, else 1
+ *   sdf_l1 (LOSS_L1)        sdf_diff_loss (utils/loss.py:6-14)   L = sum |weight| |d|
+ *   sdf_l2 (LOSS_L2)        sdf_diff_loss, l2_loss=True          L = sum |weight| d^2
+ * label [n]; weight [n], or NULL for sdf_bce without SHINE_FLAG_WEIGHTED; sigma = sigma_sigmoid (shine_batch.py:87),
+ * > 0 for sdf_bce; scale = config.scale (1 / world_size), positive and finite for sdf_l1 / sdf_l2.  Each loss ignores the
+ * other's parameter.  out_loss [1] fp32 is ACCUMULATED (+=): caller zeroes it.  loss_scale multiplies every per-point
+ * term: 1/N_global for "mean" and for sdf_l1 / sdf_l2 (the reference's count), 1 for "sum".
+ * flags: sdf_bce SHINE_FLAG_REDUCTION_SUM | WEIGHTED | TF32X1 | MORTON_ORDERED (the reduction is loss_scale's, the order
+ * a hint of the step's); sdf_l1 / sdf_l2 only SHINE_FLAG_TF32X1 besides the loss bit (sdf_diff_loss always weighs by
+ * |weight| and divides by the count).  Any other bit is SHINE_ERR_UNSUPPORTED, checked first. */
+int shine_sdf_fwd(const shine_octree* oct, const shine_decoder* dec, const float* coord, const float* label,
+                  const float* weight, int64_t n, float sigma, float scale, float loss_scale, float* out_pred,
+                  float* out_loss, uint32_t flags, void* stream);
+
+/* The whole training step shine_batch.py:123-209 in ONE pass: forward, loss (as shine_sdf_fwd) and the backward that
+ * scatter-adds into lv[i].feature_grads and dec->g*.  d_loss: device scalar dL/dloss (NULL == 1).
+ * out_pred / out_loss may be NULL (pure backward == "recompute" mode for a separate autograd backward).  flags as
+ * shine_sdf_fwd, and SHINE_FLAG_MORTON_ORDERED with sdf_l1 / sdf_l2 too. */
+int shine_sdf_step(const shine_octree* oct, const shine_decoder* dec, const float* coord, const float* label,
+                   const float* weight, int64_t n, float sigma, float scale, float loss_scale, const float* d_loss,
+                   float* out_pred, float* out_loss, uint32_t flags, void* stream);
+
+/* shine_sdf_fwd with sdf_bce_loss (either loss bit is SHINE_ERR_UNSUPPORTED), under the name and arguments of ABI
+ * version 4, which benchmark scripts bind. */
 int shine_sdf_bce_fwd(const shine_octree* oct, const shine_decoder* dec, const float* coord,
                       const float* label, const float* weight, int64_t n, float sigma, float loss_scale,
                       float* out_pred, float* out_loss, uint32_t flags, void* stream);
-
-/* The whole training step shine_batch.py:123-209 in ONE pass: forward, loss and the backward that
- * scatter-adds into lv[i].feature_grads and dec->g*.  d_loss: device scalar dL/dloss (NULL == 1).
- * out_pred / out_loss may be NULL (pure backward == "recompute" mode for a separate autograd backward). */
-int shine_sdf_bce_step(const shine_octree* oct, const shine_decoder* dec, const float* coord,
-                       const float* label, const float* weight, int64_t n, float sigma, float loss_scale,
-                       const float* d_loss, float* out_pred, float* out_loss, uint32_t flags, void* stream);
-
-/* The same forward and training step with the reference's other point-wise losses, sdf_diff_loss (utils/loss.py:6-14,
- * shine_batch.py:171-179; main_loss_type sdf_l1 / sdf_l2):
- *   diff_m = (pred - label) / scale;   L = sum |weight| |diff_m|   (L1)   or   sum |weight| diff_m^2   (SHINE_FLAG_LOSS_L2)
- * scale = config.scale (1 / world_size), positive and finite; weight [n] is required (its magnitude is always applied);
- * loss_scale multiplies every per-point term (1 / the global batch size, the reference's count).  out_loss is ACCUMULATED
- * (+=).  flags: SHINE_FLAG_TF32X1, SHINE_FLAG_LOSS_L2 and, for the step, SHINE_FLAG_MORTON_ORDERED; any other bit (also
- * REDUCTION_SUM and WEIGHTED, which sdf_diff_loss does not have) is SHINE_ERR_UNSUPPORTED.  Other arguments as in
- * shine_sdf_bce_fwd / shine_sdf_bce_step. */
-int shine_sdf_diff_fwd(const shine_octree* oct, const shine_decoder* dec, const float* coord,
-                       const float* label, const float* weight, int64_t n, float scale, float loss_scale,
-                       float* out_pred, float* out_loss, uint32_t flags, void* stream);
-int shine_sdf_diff_step(const shine_octree* oct, const shine_decoder* dec, const float* coord,
-                        const float* label, const float* weight, int64_t n, float scale, float loss_scale,
-                        const float* d_loss, float* out_pred, float* out_loss, uint32_t flags, void* stream);
 
 /* feature_grads[l] += sum of grad_replicas[l][r]; grad_replicas[l] = 0.  No-op for levels without
  * replicas.  Part of the backward (the reference's index_put_ is one pass, shine_batch.py:209). */
@@ -237,26 +240,23 @@ int shine_octree_corner_rehash(void* corner_slots, uint32_t capacity, const int6
 /* ---- the step with `ekional_loss_on` (config/kitti/kitti_batch.yaml:46) as one kernel ---------------------------------
  * Replaces shine_batch.py:119-142,172-185,208-209 + utils/tools.py:175-185 (autograd.grad(pred, coord, create_graph=True)
  * and the double backward through gather, decoder and loss):
- *   g = sigma * d pred / d coord;   L = sdf_bce_loss(pred, label) + weight_e * mean_{weight > 0} (1 - |g|)^2
+ *   g = sigma * d pred / d coord;   L = point-wise loss(pred, label) + weight_e * mean_{weight > 0} (1 - |g|)^2
+ * The point-wise loss is shine_sdf_fwd's, picked by the same loss bits; sigma = sigma_sigmoid, > 0 whatever the loss.
  * Accumulates dL/d(tables) into lv[i].feature_grads and dL/d(decoder) into dec->g* (both terms).
- *   weight     [n]: sign marks surface (+) / free-space (-) samples (shine_batch.py:137); |weight| multiplies the BCE
- *              term only with SHINE_FLAG_WEIGHTED
+ *   weight     [n]: sign marks surface (+) / free-space (-) samples (shine_batch.py:137); |weight| multiplies the sdf_bce
+ *              term only with SHINE_FLAG_WEIGHTED, the sdf_l1 / sdf_l2 term always
  *   n_surface  device int32: number of samples with weight > 0 (shine_count_positive) in the whole batch; when this call
  *              sees one part of it (a rank's shard, a chunk), the count of the whole batch; 0 -> no eikonal contribution
- *   out_pred [n] / out_grad [n,3] (g) may be NULL; out_loss (+=) BCE part; out_eikonal (+=) the mean, without weight_e */
+ *   out_pred [n] / out_grad [n,3] (g) may be NULL; out_loss (+=) the point-wise part; out_eikonal (+=) the mean, without
+ *              weight_e
+ * flags: sdf_bce SHINE_FLAG_REDUCTION_SUM | WEIGHTED | TF32X1 (the reduction is loss_scale's); sdf_l1 / sdf_l2 only
+ * SHINE_FLAG_TF32X1 besides the loss bit.  TF32X1 is accepted and changes nothing: the kernel is fp32 throughout.  Any
+ * other bit is SHINE_ERR_UNSUPPORTED. */
 int shine_count_positive(const float* values, int64_t n, int32_t* out_count, void* stream);
-int shine_sdf_bce_eikonal_step(const shine_octree* oct, const shine_decoder* dec, const float* coord,
-                               const float* label, const float* weight, int64_t n, float sigma, float loss_scale,
-                               float weight_e, const int32_t* n_surface, float* out_pred, float* out_grad,
-                               float* out_loss, float* out_eikonal, uint32_t flags, void* stream);
-/* The same step with sdf_diff_loss in place of the BCE term (see shine_sdf_diff_step): L = sdf_diff_loss(pred, label) +
- * weight_e * mean_{weight > 0} (1 - |g|)^2, g = sigma * d pred / d coord as above (sigma = sigma_sigmoid, whatever the
- * loss).  |weight| always multiplies the sdf_diff_loss term; flags: SHINE_FLAG_TF32X1 (accepted, the kernel is fp32
- * throughout) and SHINE_FLAG_LOSS_L2, any other bit is SHINE_ERR_UNSUPPORTED.  out_loss (+=) the sdf_diff_loss part. */
-int shine_sdf_diff_eikonal_step(const shine_octree* oct, const shine_decoder* dec, const float* coord,
-                                const float* label, const float* weight, int64_t n, float scale, float sigma,
-                                float loss_scale, float weight_e, const int32_t* n_surface, float* out_pred,
-                                float* out_grad, float* out_loss, float* out_eikonal, uint32_t flags, void* stream);
+int shine_sdf_eikonal_step(const shine_octree* oct, const shine_decoder* dec, const float* coord, const float* label,
+                           const float* weight, int64_t n, float sigma, float scale, float loss_scale, float weight_e,
+                           const int32_t* n_surface, float* out_pred, float* out_grad, float* out_loss,
+                           float* out_eikonal, uint32_t flags, void* stream);
 
 /* ---- continual-learning terms of the incremental loop (BASELINE config 4) ---------------------------------------
  * The reference finds the rows a batch touched with `hierarchical_indices[i].flatten().unique()` (a sort per level

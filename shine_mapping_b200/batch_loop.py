@@ -5,14 +5,14 @@
 Same sequence as the reference loop (T-points of shine_batch.py:107-212 kept as timing keys): build the octree
 from all frames, set up the optimiser, then `iters` x { lr decay -> get_batch -> fwd+loss+bwd -> optimiser },
 checkpoint in the reference's format.  What differs: the body of an iteration is TWO launches (the fused
-`shine_sdf_bce_step` kernel and the multi-tensor Adam kernel, which also re-zeroes the gradients) instead of
+`shine_sdf_step` kernel and the multi-tensor Adam kernel, which also re-zeroes the gradients) instead of
 ~300, and there is no host round trip inside the loop (loss is read back only when logging).
 `main_loss_type` is the reference's point-wise menu (shine_batch.py:171-179): sdf_bce, or sdf_l1 / sdf_l2
-(`sdf_diff_loss`, fused as `shine_sdf_diff_step`), each with or without the eikonal term.
+(`sdf_diff_loss`), the loss bit of the same fused `shine_sdf_step`, each with or without the eikonal term.
 
 Out of scope here (SURVEY.md §2): dataset I/O (open3d), meshing, visualiser, wandb.  `pool` is anything with the
 `get_batch(bs)` contract of LiDARDataset (dataset/lidar_dataset.py:431-448); `synth.build_scene_map` provides one.
-`ekional_loss_on` is one fused kernel (`shine_sdf_bce_eikonal_step` / `shine_sdf_diff_eikonal_step`; the class surface
+`ekional_loss_on` is one fused kernel (`shine_sdf_eikonal_step`; the class surface
 supports the reference's autograd recipe too: query_feature is differentiable w.r.t. the coordinates, twice); normal /
 consistency / semantic / ray losses are rejected explicitly.
 """

@@ -1421,13 +1421,6 @@ __global__ void __launch_bounds__(256) adam_kernel(const __grid_constant__ AdamP
 // host side
 // ------------------------------------------------------------------------------------------------------
 
-int check_decoder(const shine_decoder* d, const shine_octree* o) {
-    if (!d) return SHINE_ERR_INVALID_ARG;
-    if (d->in_dim != kF || d->hidden != kH || d->mlp_level != 2 || o->feature_dim != kF) return SHINE_ERR_UNSUPPORTED;
-    if (!d->w1 || !d->w2 || !d->w3) return SHINE_ERR_INVALID_ARG;
-    return SHINE_OK;
-}
-
 template <int NTF, bool TRAIN, bool DEC_GRAD, int LMAX, bool GROUPED = false, class Src = BatchCoords, int LOSS = kLossBce>
 int launch_fused_t(const StepParams& P, cudaStream_t st, const Src& src = Src()) {
     auto kern = sdf_fused_kernel<NTF, TRAIN, DEC_GRAD, LMAX, GROUPED, Src, LOSS>;
@@ -1480,17 +1473,8 @@ int launch_fused(const StepParams& P, uint32_t flags, cudaStream_t st, const Src
                  : launch_fused_t<3, TRAIN, DEC_GRAD, 8, false, Src, LOSS>(P, st, src);
 }
 
-// the sdf_diff_loss step and forward: the per-sample loss (L1 / L2) picks the kernels
-template <bool TRAIN, bool DEC_GRAD>
-int launch_diff(const StepParams& P, uint32_t flags, cudaStream_t st) {
-    return (flags & SHINE_FLAG_LOSS_L2) ? launch_fused<TRAIN, DEC_GRAD, BatchCoords, kLossL2>(P, flags, st)
-                                        : launch_fused<TRAIN, DEC_GRAD, BatchCoords, kLossL1>(P, flags, st);
-}
-
-// the flag bits of the shine_sdf_* calls: any other bit is SHINE_ERR_UNSUPPORTED, never silently ignored
+// the flag bits of shine_sdf_infer and of the sdf_bce loss: any other bit is SHINE_ERR_UNSUPPORTED, never silently ignored
 constexpr uint32_t kSdfFlags = SHINE_FLAG_REDUCTION_SUM | SHINE_FLAG_WEIGHTED | SHINE_FLAG_TF32X1 | SHINE_FLAG_MORTON_ORDERED;
-// the flag bits of the shine_sdf_diff_* calls: reduction and weighting are fixed by sdf_diff_loss (weighted sum / count)
-constexpr uint32_t kDiffFlags = SHINE_FLAG_TF32X1 | SHINE_FLAG_MORTON_ORDERED | SHINE_FLAG_LOSS_L2;
 
 int fill_params(StepParams& P, const shine_octree* oct, const shine_decoder* dec, const float* coord, int64_t n) {
     if (n < 0 || (n > 0 && !coord)) return SHINE_ERR_INVALID_ARG;
@@ -1500,6 +1484,41 @@ int fill_params(StepParams& P, const shine_octree* oct, const shine_decoder* dec
     P.label = nullptr; P.weight = nullptr; P.d_loss = nullptr; P.pred = nullptr; P.loss = nullptr; P.mask = nullptr;
     P.mask_level = 0; P.sigma = 1.f; P.loss_scale = 1.f; P.weighted = 0; P.scale = 1.f;
     return SHINE_OK;
+}
+
+template <bool TRAIN, bool DEC_GRAD>
+int launch_loss(const StepParams& P, int loss, uint32_t flags, cudaStream_t st) {
+    if (loss == kLossL1) return launch_fused<TRAIN, DEC_GRAD, BatchCoords, kLossL1>(P, flags, st);
+    if (loss == kLossL2) return launch_fused<TRAIN, DEC_GRAD, BatchCoords, kLossL2>(P, flags, st);
+    return launch_fused<TRAIN, DEC_GRAD>(P, flags, st);
+}
+
+// shine_sdf_fwd (train false) and shine_sdf_step: the checks of the loss the flags pick, then one launch
+int sdf_loss_call(bool train, const shine_octree* oct, const shine_decoder* dec, const float* coord, const float* label,
+                  const float* weight, int64_t n, float sigma, float scale, float loss_scale, const float* d_loss,
+                  float* out_pred, float* out_loss, uint32_t flags, cudaStream_t st) {
+    // sdf_diff_loss has no reduction or weighting flag: it always weighs by |weight| and divides by the count
+    const int loss = sdf_loss_of(flags, kSdfFlags, SHINE_FLAG_TF32X1 | (train ? SHINE_FLAG_MORTON_ORDERED : 0u));
+    if (loss < 0) return SHINE_ERR_UNSUPPORTED;
+    int rc = check_octree(oct, train);
+    if (rc) return rc;
+    bool dec_grad = false;
+    rc = check_decoder(dec, oct, train ? &dec_grad : nullptr);
+    if (rc) return rc;
+    if (n > 0 && !label) return SHINE_ERR_INVALID_ARG;
+    if (loss == kLossBce ? ((flags & SHINE_FLAG_WEIGHTED) && !weight) || !(sigma > 0.f) : !weight || !valid_scale(scale))
+        return SHINE_ERR_INVALID_ARG;
+    StepParams P;
+    rc = fill_params(P, oct, dec, coord, n);
+    if (rc) return rc;
+    if (n == 0) return SHINE_OK;
+    if ((rc = check_same_device(oct, coord))) return rc;
+    DeviceGuard guard(oct->lv[0].features);
+    P.label = label; P.weight = weight; P.d_loss = d_loss; P.pred = out_pred; P.loss = out_loss;
+    P.sigma = sigma; P.scale = scale; P.loss_scale = loss_scale;
+    P.weighted = (loss != kLossBce || (flags & SHINE_FLAG_WEIGHTED)) ? 1 : 0;   // sdf_l1 / sdf_l2: shine_batch.py:172 |weight|
+    if (!train) return launch_loss<false, false>(P, loss, flags, st);
+    return dec_grad ? launch_loss<true, true>(P, loss, flags, st) : launch_loss<true, false>(P, loss, flags, st);
 }
 
 template <int LP>
@@ -1671,94 +1690,25 @@ int shine_sdf_infer(const shine_octree* oct, const shine_decoder* dec, const flo
     return launch_fused<false, false>(P, flags, (cudaStream_t)stream);
 }
 
+int shine_sdf_fwd(const shine_octree* oct, const shine_decoder* dec, const float* coord, const float* label,
+                  const float* weight, int64_t n, float sigma, float scale, float loss_scale, float* out_pred,
+                  float* out_loss, uint32_t flags, void* stream) {
+    return sdf_loss_call(false, oct, dec, coord, label, weight, n, sigma, scale, loss_scale, nullptr, out_pred, out_loss,
+                         flags, (cudaStream_t)stream);
+}
+
+int shine_sdf_step(const shine_octree* oct, const shine_decoder* dec, const float* coord, const float* label,
+                   const float* weight, int64_t n, float sigma, float scale, float loss_scale, const float* d_loss,
+                   float* out_pred, float* out_loss, uint32_t flags, void* stream) {
+    return sdf_loss_call(true, oct, dec, coord, label, weight, n, sigma, scale, loss_scale, d_loss, out_pred, out_loss,
+                         flags, (cudaStream_t)stream);
+}
+
 int shine_sdf_bce_fwd(const shine_octree* oct, const shine_decoder* dec, const float* coord, const float* label,
                       const float* weight, int64_t n, float sigma, float loss_scale, float* out_pred, float* out_loss,
                       uint32_t flags, void* stream) {
-    if (flags & ~kSdfFlags) return SHINE_ERR_UNSUPPORTED;
-    int rc = check_octree(oct, false);
-    if (rc) return rc;
-    rc = check_decoder(dec, oct);
-    if (rc) return rc;
-    if (n > 0 && !label) return SHINE_ERR_INVALID_ARG;
-    if ((flags & SHINE_FLAG_WEIGHTED) && !weight) return SHINE_ERR_INVALID_ARG;
-    if (!(sigma > 0.f)) return SHINE_ERR_INVALID_ARG;
-    StepParams P;
-    rc = fill_params(P, oct, dec, coord, n);
-    if (rc) return rc;
-    if (n == 0) return SHINE_OK;
-    if ((rc = check_same_device(oct, coord))) return rc;
-    DeviceGuard guard(oct->lv[0].features);
-    P.label = label; P.weight = weight; P.weighted = (flags & SHINE_FLAG_WEIGHTED) ? 1 : 0;
-    P.sigma = sigma; P.loss_scale = loss_scale; P.pred = out_pred; P.loss = out_loss;
-    return launch_fused<false, false>(P, flags, (cudaStream_t)stream);
-}
-
-int shine_sdf_bce_step(const shine_octree* oct, const shine_decoder* dec, const float* coord, const float* label,
-                       const float* weight, int64_t n, float sigma, float loss_scale, const float* d_loss,
-                       float* out_pred, float* out_loss, uint32_t flags, void* stream) {
-    if (flags & ~kSdfFlags) return SHINE_ERR_UNSUPPORTED;
-    int rc = check_octree(oct, true);
-    if (rc) return rc;
-    rc = check_decoder(dec, oct);
-    if (rc) return rc;
-    if (n > 0 && !label) return SHINE_ERR_INVALID_ARG;
-    if ((flags & SHINE_FLAG_WEIGHTED) && !weight) return SHINE_ERR_INVALID_ARG;
-    if (!(sigma > 0.f)) return SHINE_ERR_INVALID_ARG;
-    const bool dec_grad = dec->gw1 || dec->gw2 || dec->gw3;
-    if (dec_grad && !(dec->gw1 && dec->gw2 && dec->gw3)) return SHINE_ERR_INVALID_ARG;
-    StepParams P;
-    rc = fill_params(P, oct, dec, coord, n);
-    if (rc) return rc;
-    if (n == 0) return SHINE_OK;
-    if ((rc = check_same_device(oct, coord))) return rc;
-    DeviceGuard guard(oct->lv[0].features);
-    P.label = label; P.weight = weight; P.weighted = (flags & SHINE_FLAG_WEIGHTED) ? 1 : 0;
-    P.sigma = sigma; P.loss_scale = loss_scale; P.d_loss = d_loss; P.pred = out_pred; P.loss = out_loss;
-    return dec_grad ? launch_fused<true, true>(P, flags, (cudaStream_t)stream)
-                    : launch_fused<true, false>(P, flags, (cudaStream_t)stream);
-}
-
-int shine_sdf_diff_fwd(const shine_octree* oct, const shine_decoder* dec, const float* coord, const float* label,
-                       const float* weight, int64_t n, float scale, float loss_scale, float* out_pred, float* out_loss,
-                       uint32_t flags, void* stream) {
-    if (flags & ~(kDiffFlags & ~SHINE_FLAG_MORTON_ORDERED)) return SHINE_ERR_UNSUPPORTED;
-    int rc = check_octree(oct, false);
-    if (rc) return rc;
-    rc = check_decoder(dec, oct);
-    if (rc) return rc;
-    if (!weight || (n > 0 && !label) || !valid_scale(scale)) return SHINE_ERR_INVALID_ARG;
-    StepParams P;
-    rc = fill_params(P, oct, dec, coord, n);
-    if (rc) return rc;
-    if (n == 0) return SHINE_OK;
-    if ((rc = check_same_device(oct, coord))) return rc;
-    DeviceGuard guard(oct->lv[0].features);
-    P.label = label; P.weight = weight; P.weighted = 1;          // shine_batch.py:172 |weight|, always applied
-    P.scale = scale; P.loss_scale = loss_scale; P.pred = out_pred; P.loss = out_loss;
-    return launch_diff<false, false>(P, flags, (cudaStream_t)stream);
-}
-
-int shine_sdf_diff_step(const shine_octree* oct, const shine_decoder* dec, const float* coord, const float* label,
-                        const float* weight, int64_t n, float scale, float loss_scale, const float* d_loss,
-                        float* out_pred, float* out_loss, uint32_t flags, void* stream) {
-    if (flags & ~kDiffFlags) return SHINE_ERR_UNSUPPORTED;
-    int rc = check_octree(oct, true);
-    if (rc) return rc;
-    rc = check_decoder(dec, oct);
-    if (rc) return rc;
-    if (!weight || (n > 0 && !label) || !valid_scale(scale)) return SHINE_ERR_INVALID_ARG;
-    const bool dec_grad = dec->gw1 || dec->gw2 || dec->gw3;
-    if (dec_grad && !(dec->gw1 && dec->gw2 && dec->gw3)) return SHINE_ERR_INVALID_ARG;
-    StepParams P;
-    rc = fill_params(P, oct, dec, coord, n);
-    if (rc) return rc;
-    if (n == 0) return SHINE_OK;
-    if ((rc = check_same_device(oct, coord))) return rc;
-    DeviceGuard guard(oct->lv[0].features);
-    P.label = label; P.weight = weight; P.weighted = 1;
-    P.scale = scale; P.loss_scale = loss_scale; P.d_loss = d_loss; P.pred = out_pred; P.loss = out_loss;
-    return dec_grad ? launch_diff<true, true>(P, flags, (cudaStream_t)stream)
-                    : launch_diff<true, false>(P, flags, (cudaStream_t)stream);
+    if (flags & (SHINE_FLAG_LOSS_L1 | SHINE_FLAG_LOSS_L2)) return SHINE_ERR_UNSUPPORTED;
+    return shine_sdf_fwd(oct, dec, coord, label, weight, n, sigma, 1.f, loss_scale, out_pred, out_loss, flags, stream);
 }
 
 int shine_reduce_grad_replicas(const shine_octree* oct, void* stream) {

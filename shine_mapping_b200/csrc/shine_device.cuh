@@ -473,6 +473,19 @@ inline int check_same_device(const shine_octree* o, const void* batch_ptr) {
     return (d >= 0 && d != device_of(o->lv[0].features)) ? SHINE_ERR_INVALID_ARG : SHINE_OK;
 }
 
+// the decoder of the fused kernels: F -> 32 -> 32 -> 1 with F = 8.  With dec_grad: its gradient buffers gw1, gw2, gw3 are
+// all set or all NULL (a frozen decoder), and *dec_grad says which.
+inline int check_decoder(const shine_decoder* d, const shine_octree* o, bool* dec_grad = nullptr) {
+    if (!d) return SHINE_ERR_INVALID_ARG;
+    if (d->in_dim != kF || d->hidden != kH || d->mlp_level != 2 || o->feature_dim != kF) return SHINE_ERR_UNSUPPORTED;
+    if (!d->w1 || !d->w2 || !d->w3) return SHINE_ERR_INVALID_ARG;
+    if (dec_grad) {
+        *dec_grad = d->gw1 || d->gw2 || d->gw3;
+        if (*dec_grad && !(d->gw1 && d->gw2 && d->gw3)) return SHINE_ERR_INVALID_ARG;
+    }
+    return SHINE_OK;
+}
+
 // The per-sample loss of the training kernels, a template parameter: sdf_bce_loss (utils/loss.py:17-24), or sdf_diff_loss
 // (utils/loss.py:6-14) with l2_loss False (L1) or True (L2).
 enum SdfLoss : int { kLossBce = 0, kLossL1 = 1, kLossL2 = 2 };
@@ -494,7 +507,16 @@ __device__ __forceinline__ void diff_point(float pv, float lb, float scale, floa
     }
 }
 
-// the sdf_diff_loss entries: the scale a caller passes must be a positive finite number
+// sdf_l1 / sdf_l2: the scale a caller passes must be a positive finite number
 inline bool valid_scale(float scale) { return scale > 0.f && scale <= 3.402823466e38f; }
+
+// The loss the loss bits of a shine_sdf_fwd / _step / _eikonal_step flag word pick (neither: sdf_bce), or -1 when the call
+// refuses the word: both loss bits, or a bit outside those it accepts with that loss (bce_flags / diff_flags).
+inline int sdf_loss_of(uint32_t flags, uint32_t bce_flags, uint32_t diff_flags) {
+    const uint32_t bits = flags & (SHINE_FLAG_LOSS_L1 | SHINE_FLAG_LOSS_L2);
+    if (bits == (SHINE_FLAG_LOSS_L1 | SHINE_FLAG_LOSS_L2)) return -1;
+    const int loss = bits == SHINE_FLAG_LOSS_L1 ? kLossL1 : bits == SHINE_FLAG_LOSS_L2 ? kLossL2 : kLossBce;
+    return (flags & ~(bits | (loss == kLossBce ? bce_flags : diff_flags))) ? -1 : loss;
+}
 
 }  // namespace

@@ -419,57 +419,32 @@ int shine_count_positive(const float* values, int64_t n, int32_t* out_count, voi
     return (int)cudaGetLastError();
 }
 
-int shine_sdf_bce_eikonal_step(const shine_octree* oct, const shine_decoder* dec, const float* coord, const float* label,
-                               const float* weight, int64_t n, float sigma, float loss_scale, float weight_e,
-                               const int32_t* n_surface, float* out_pred, float* out_grad, float* out_loss,
-                               float* out_eikonal, uint32_t flags, void* stream) {
+int shine_sdf_eikonal_step(const shine_octree* oct, const shine_decoder* dec, const float* coord, const float* label,
+                           const float* weight, int64_t n, float sigma, float scale, float loss_scale, float weight_e,
+                           const int32_t* n_surface, float* out_pred, float* out_grad, float* out_loss,
+                           float* out_eikonal, uint32_t flags, void* stream) {
+    // REDUCTION_SUM is accepted with sdf_bce and changes nothing here: the reduction comes in loss_scale
+    const int loss = sdf_loss_of(flags, SHINE_FLAG_REDUCTION_SUM | SHINE_FLAG_WEIGHTED | SHINE_FLAG_TF32X1,
+                                 SHINE_FLAG_TF32X1);
+    if (loss < 0) return SHINE_ERR_UNSUPPORTED;
     int rc = check_octree(oct, true);
     if (rc) return rc;
-    if (!dec) return SHINE_ERR_INVALID_ARG;
-    if (dec->in_dim != kF || dec->hidden != kH || dec->mlp_level != 2 || oct->feature_dim != kF) return SHINE_ERR_UNSUPPORTED;
-    if (!dec->w1 || !dec->w2 || !dec->w3) return SHINE_ERR_INVALID_ARG;
+    bool dec_grad = false;
+    if ((rc = check_decoder(dec, oct, &dec_grad))) return rc;
     if (n < 0 || (n > 0 && (!coord || !label || !weight || !n_surface))) return SHINE_ERR_INVALID_ARG;
-    if (!(sigma > 0.f)) return SHINE_ERR_INVALID_ARG;
-    const bool dec_grad = dec->gw1 || dec->gw2 || dec->gw3;
-    if (dec_grad && !(dec->gw1 && dec->gw2 && dec->gw3)) return SHINE_ERR_INVALID_ARG;
+    if (!(sigma > 0.f) || (loss != kLossBce && (!weight || !valid_scale(scale)))) return SHINE_ERR_INVALID_ARG;
     if (n == 0) return SHINE_OK;
     if ((rc = check_same_device(oct, coord))) return rc;
     DeviceGuard guard(oct->lv[0].features);
     EikParams P;
     P.oct = *oct; P.dec = *dec; P.coord = coord; P.label = label; P.weight = weight; P.n_surface = n_surface;
     P.pred = out_pred; P.grad_out = out_grad; P.loss = out_loss; P.eikonal = out_eikonal; P.n = n;
-    P.sigma = sigma; P.loss_scale = loss_scale; P.weight_e = weight_e;
-    P.weighted = (flags & SHINE_FLAG_WEIGHTED) ? 1 : 0;
-    return dec_grad ? launch_eikonal<true>(P, (cudaStream_t)stream) : launch_eikonal<false>(P, (cudaStream_t)stream);
-}
-
-int shine_sdf_diff_eikonal_step(const shine_octree* oct, const shine_decoder* dec, const float* coord, const float* label,
-                                const float* weight, int64_t n, float scale, float sigma, float loss_scale, float weight_e,
-                                const int32_t* n_surface, float* out_pred, float* out_grad, float* out_loss,
-                                float* out_eikonal, uint32_t flags, void* stream) {
-    if (flags & ~(SHINE_FLAG_TF32X1 | SHINE_FLAG_LOSS_L2)) return SHINE_ERR_UNSUPPORTED;
-    int rc = check_octree(oct, true);
-    if (rc) return rc;
-    if (!dec) return SHINE_ERR_INVALID_ARG;
-    if (dec->in_dim != kF || dec->hidden != kH || dec->mlp_level != 2 || oct->feature_dim != kF) return SHINE_ERR_UNSUPPORTED;
-    if (!dec->w1 || !dec->w2 || !dec->w3) return SHINE_ERR_INVALID_ARG;
-    if (!weight || n < 0 || (n > 0 && (!coord || !label || !n_surface))) return SHINE_ERR_INVALID_ARG;
-    if (!(sigma > 0.f) || !valid_scale(scale)) return SHINE_ERR_INVALID_ARG;
-    const bool dec_grad = dec->gw1 || dec->gw2 || dec->gw3;
-    if (dec_grad && !(dec->gw1 && dec->gw2 && dec->gw3)) return SHINE_ERR_INVALID_ARG;
-    if (n == 0) return SHINE_OK;
-    if ((rc = check_same_device(oct, coord))) return rc;
-    DeviceGuard guard(oct->lv[0].features);
-    EikParams P;
-    P.oct = *oct; P.dec = *dec; P.coord = coord; P.label = label; P.weight = weight; P.n_surface = n_surface;
-    P.pred = out_pred; P.grad_out = out_grad; P.loss = out_loss; P.eikonal = out_eikonal; P.n = n;
-    P.sigma = sigma; P.loss_scale = loss_scale; P.weight_e = weight_e;
-    P.weighted = 1;                                       // shine_batch.py:172 |weight|, always applied
-    P.scale = scale;
+    P.sigma = sigma; P.scale = scale; P.loss_scale = loss_scale; P.weight_e = weight_e;
+    P.weighted = (loss != kLossBce || (flags & SHINE_FLAG_WEIGHTED)) ? 1 : 0;   // sdf_l1 / sdf_l2: shine_batch.py:172 |weight|
     const cudaStream_t st = (cudaStream_t)stream;
-    if (flags & SHINE_FLAG_LOSS_L2)
-        return dec_grad ? launch_eikonal<true, kLossL2>(P, st) : launch_eikonal<false, kLossL2>(P, st);
-    return dec_grad ? launch_eikonal<true, kLossL1>(P, st) : launch_eikonal<false, kLossL1>(P, st);
+    if (loss == kLossL1) return dec_grad ? launch_eikonal<true, kLossL1>(P, st) : launch_eikonal<false, kLossL1>(P, st);
+    if (loss == kLossL2) return dec_grad ? launch_eikonal<true, kLossL2>(P, st) : launch_eikonal<false, kLossL2>(P, st);
+    return dec_grad ? launch_eikonal<true>(P, st) : launch_eikonal<false>(P, st);
 }
 
 }  // extern "C"

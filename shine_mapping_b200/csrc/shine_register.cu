@@ -220,8 +220,7 @@ int shine_register_normal_eq(const shine_octree* oct, const shine_decoder* dec, 
     if (!oct || !dec || !pose || !out || n < 0 || (n > 0 && !points)) return SHINE_ERR_INVALID_ARG;
     int rc = check_octree(oct, false);
     if (rc) return rc;
-    if (dec->in_dim != kF || dec->hidden != kH || dec->mlp_level != 2 || oct->feature_dim != kF) return SHINE_ERR_UNSUPPORTED;
-    if (!dec->w1 || !dec->w2 || !dec->w3) return SHINE_ERR_INVALID_ARG;
+    if ((rc = check_decoder(dec, oct))) return rc;
     if (!(sigma > 0.f) || !is_finite(sigma) || !(kappa > 0.0) || !is_finite(kappa)) return SHINE_ERR_INVALID_ARG;
     for (int i = 0; i < 12; ++i)
         if (!is_finite(pose[i])) return SHINE_ERR_INVALID_ARG;

@@ -5,7 +5,7 @@ One flat fp32 gradient buffer holds every table level and the decoder (each segm
   * zeroing the gradients is ONE memset (or free: fused into the Adam kernel),
   * the data-parallel exchange is ONE NCCL all-reduce over NVLink (decoder 1 377 floats + table rows),
   * `param.grad` of every parameter is a view into it, so stock torch optimizers still work.
-`forward_backward()` = one `shine_sdf_bce_step` launch (`shine_sdf_diff_step` with main_loss_type sdf_l1 / sdf_l2);
+`forward_backward()` = one `shine_sdf_step` launch with the loss of main_loss_type (sdf_bce, sdf_l1 or sdf_l2);
 `optimizer_step()` = one `shine_adam_step` launch with the
 reference's grouping (utils/tools.py:57-83: Adam betas (0.9, 0.99), eps 1e-15, weight decay on the decoder only,
 per-level lr scaled leaf -> coarse by lr_level_reduce_ratio).
@@ -27,10 +27,10 @@ def _align4(n: int) -> int:
     return (n + 3) & ~3
 
 
-def diff_loss_flags(main_loss_type: str):
-    """main_loss_type -> None for sdf_bce, else the loss bit of the shine_sdf_diff_* calls (sdf_l1: 0, sdf_l2:
-    FLAG_LOSS_L2; shine_batch.py:176-179)."""
-    kinds = {"sdf_bce": None, "sdf_l1": 0, "sdf_l2": _abi.FLAG_LOSS_L2}
+def loss_flags(main_loss_type: str) -> int:
+    """main_loss_type -> the loss bit of the shine_sdf_* calls (sdf_bce: 0, sdf_l1: FLAG_LOSS_L1, sdf_l2: FLAG_LOSS_L2;
+    shine_batch.py:171-179)."""
+    kinds = {"sdf_bce": 0, "sdf_l1": _abi.FLAG_LOSS_L1, "sdf_l2": _abi.FLAG_LOSS_L2}
     if main_loss_type not in kinds:
         raise NotImplementedError(f"main_loss_type {main_loss_type!r}: the trainer has {sorted(kinds)}")
     return kinds[main_loss_type]
@@ -64,7 +64,7 @@ class SdfTrainer:
         self._sig = None
         self.sigma = config.sigma_sigmoid
         self.main_loss_type = config.main_loss_type if main_loss_type is None else main_loss_type
-        self._diff = diff_loss_flags(self.main_loss_type)   # None: sdf_bce
+        self._loss_bit = loss_flags(self.main_loss_type)   # 0: sdf_bce
         self._sync()
 
     # ---- flat buffers --------------------------------------------------------------------------------------
@@ -126,6 +126,15 @@ class SdfTrainer:
 
     # ---- the hot path --------------------------------------------------------------------------------------
 
+    def _loss_args(self, n, n_norm, weighted):
+        """(flags, loss_scale) of the point-wise loss: sdf_bce follows loss_reduction and `weighted`; sdf_diff_loss is
+        always weighted and divided by the batch size, whatever loss_reduction says."""
+        if self._loss_bit:
+            return self._loss_bit, 1.0 / float(n_norm if n_norm else n)
+        if self.config.loss_reduction == "sum":
+            return _abi.FLAG_REDUCTION_SUM | (_abi.FLAG_WEIGHTED if weighted else 0), 1.0
+        return _abi.FLAG_WEIGHTED if weighted else 0, 1.0 / float(n_norm if n_norm else n)
+
     def forward_backward(self, coord, sdf_label, weight=None, n_norm=None, pred_out=None, accumulate_loss=False,
                          weighted=None, mid_event=None, morton_ordered=None):
         """One fused launch: loss value (device scalar, accumulated into self.loss which is zeroed here) and
@@ -138,16 +147,14 @@ class SdfTrainer:
         self._sync()
         cfg = self.config
         n = coord.shape[0]
-        diff = self._diff
-        if diff is not None and weight is None:
+        if self._loss_bit and weight is None:
             raise ValueError(f"main_loss_type {self.main_loss_type} needs the per-sample weight tensor")
         weighted = bool(cfg.loss_weight_on) if weighted is None else bool(weighted)
         if weighted and weight is None:
             raise ValueError("loss_weight_on needs the per-sample weight tensor")
-        flags = (_abi.FLAG_REDUCTION_SUM if cfg.loss_reduction == "sum" else 0) | \
-                (_abi.FLAG_WEIGHTED if weighted else 0) | (_abi.FLAG_TF32X1 if self.tf32x1 else 0) | \
-                (_abi.FLAG_MORTON_ORDERED if (self.morton_ordered if morton_ordered is None else morton_ordered) else 0)
-        scale = 1.0 if cfg.loss_reduction == "sum" else 1.0 / float(n_norm if n_norm else n)
+        flags, loss_scale = self._loss_args(n, n_norm, weighted)
+        flags |= (_abi.FLAG_TF32X1 if self.tf32x1 else 0) | \
+            (_abi.FLAG_MORTON_ORDERED if (self.morton_ordered if morton_ordered is None else morton_ordered) else 0)
         # gradient replicas spread same-row atomics of unordered batches; the grouped scatter of ordered batches issues one
         # red per run and row, so it goes straight to the gradient table (and there is no fold kernel)
         replicas = self.use_replicas and (self.grouped_replicas or not (flags & _abi.FLAG_MORTON_ORDERED))
@@ -156,17 +163,10 @@ class SdfTrainer:
         if not accumulate_loss and not self._loss_clean:
             self.loss.zero_()
         self._loss_clean = False
-        if diff is None:
-            _abi.check(_abi.lib().shine_sdf_bce_step(
-                C.byref(od), C.byref(dd), _abi.ptr(coord), _abi.ptr(sdf_label),
-                _abi.ptr(weight) if weighted else None, n, float(self.sigma), scale, None,
-                _abi.ptr(pred_out), _abi.ptr(self.loss), flags, _abi.stream_ptr(coord.device)), "shine_sdf_bce_step")
-        else:   # sdf_diff_loss: always weighted, divided by the batch size whatever loss_reduction says
-            flags = diff | (flags & (_abi.FLAG_TF32X1 | _abi.FLAG_MORTON_ORDERED))
-            _abi.check(_abi.lib().shine_sdf_diff_step(
-                C.byref(od), C.byref(dd), _abi.ptr(coord), _abi.ptr(sdf_label), _abi.ptr(weight), n, float(cfg.scale),
-                1.0 / float(n_norm if n_norm else n), None, _abi.ptr(pred_out), _abi.ptr(self.loss), flags,
-                _abi.stream_ptr(coord.device)), "shine_sdf_diff_step")
+        _abi.check(_abi.lib().shine_sdf_step(
+            C.byref(od), C.byref(dd), _abi.ptr(coord), _abi.ptr(sdf_label), _abi.ptr(weight), n, float(self.sigma),
+            float(cfg.scale), loss_scale, None, _abi.ptr(pred_out), _abi.ptr(self.loss), flags,
+            _abi.stream_ptr(coord.device)), "shine_sdf_step")
         if mid_event is not None:          # lets a profiler time the fused kernel and the replica fold separately
             mid_event.record()
         if replicas:
@@ -176,10 +176,10 @@ class SdfTrainer:
     def forward_backward_eikonal(self, coord, sdf_label, weight, n_norm=None, pred_out=None, grad_out=None,
                                  n_surface=None):
         """The step with `ekional_loss_on` (reference shine_batch.py:119-142,172-185,208-209) as ONE launch
-        (`shine_sdf_bce_eikonal_step`): BCE + weight_e * mean over surface samples of (1 - |sigma d pred/d coord|)^2,
+        (`shine_sdf_eikonal_step`): BCE + weight_e * mean over surface samples of (1 - |sigma d pred/d coord|)^2,
         gradients of both terms accumulated into the flat buffer.  -> (bce loss, eikonal mean) device scalars;
         the loop's total loss is bce + config.weight_e * eikonal.  With main_loss_type sdf_l1 / sdf_l2 the first term is
-        sdf_diff_loss (`shine_sdf_diff_eikonal_step`) and the first scalar its value.
+        sdf_diff_loss and the first scalar its value.
         n_surface: denominator of the eikonal mean, the analogue of n_norm: the number of surface samples (weight > 0) in
         the GLOBAL batch when this call sees one part of it.  None = counted on the device from this batch and, when the
         trainer runs on several ranks, summed over them, so that the per-rank eikonal values and gradients add up to those
@@ -188,9 +188,7 @@ class SdfTrainer:
         cfg = self.config
         n = coord.shape[0]
         dev = coord.device
-        weighted = bool(cfg.loss_weight_on)
-        flags = (_abi.FLAG_REDUCTION_SUM if cfg.loss_reduction == "sum" else 0) | (_abi.FLAG_WEIGHTED if weighted else 0)
-        scale = 1.0 if cfg.loss_reduction == "sum" else 1.0 / float(n_norm if n_norm else n)
+        flags, loss_scale = self._loss_args(n, n_norm, bool(cfg.loss_weight_on))
         aux = getattr(self, "_eik_aux", None)
         if aux is None or aux[0].device != dev:
             aux = (torch.zeros(1, dtype=torch.int32, device=dev), torch.zeros(1, dtype=torch.float32, device=dev))
@@ -212,18 +210,10 @@ class SdfTrainer:
                 total = count.float()                 # exact below 2^24 samples; the collectives here sum fp32
                 self._all_reduce(total)
                 count.copy_(total.round())
-        diff = self._diff
-        if diff is None:
-            _abi.check(lib.shine_sdf_bce_eikonal_step(
-                C.byref(od), C.byref(dd), _abi.ptr(coord), _abi.ptr(sdf_label), _abi.ptr(weight), n, float(self.sigma), scale,
-                float(cfg.weight_e), _abi.ptr(count), _abi.ptr(pred_out), _abi.ptr(grad_out), _abi.ptr(self.loss),
-                _abi.ptr(eik), flags, st), "shine_sdf_bce_eikonal_step")
-        else:
-            _abi.check(lib.shine_sdf_diff_eikonal_step(
-                C.byref(od), C.byref(dd), _abi.ptr(coord), _abi.ptr(sdf_label), _abi.ptr(weight), n, float(cfg.scale),
-                float(self.sigma), 1.0 / float(n_norm if n_norm else n), float(cfg.weight_e), _abi.ptr(count),
-                _abi.ptr(pred_out), _abi.ptr(grad_out), _abi.ptr(self.loss), _abi.ptr(eik), diff, st),
-                "shine_sdf_diff_eikonal_step")
+        _abi.check(lib.shine_sdf_eikonal_step(
+            C.byref(od), C.byref(dd), _abi.ptr(coord), _abi.ptr(sdf_label), _abi.ptr(weight), n, float(self.sigma),
+            float(cfg.scale), loss_scale, float(cfg.weight_e), _abi.ptr(count), _abi.ptr(pred_out), _abi.ptr(grad_out),
+            _abi.ptr(self.loss), _abi.ptr(eik), flags, st), "shine_sdf_eikonal_step")
         return self.loss, eik.view(())
 
     def _all_reduce(self, buf):
@@ -352,7 +342,7 @@ class SdfTrainer:
 
     def _uses_weight(self) -> bool:
         """Whether the steps read the per-sample weights: sdf_bce with loss_weight_on, sdf_l1 / sdf_l2 always."""
-        return bool(self.config.loss_weight_on) or self._diff is not None
+        return bool(self.config.loss_weight_on) or self._loss_bit != 0
 
     # ---- pipelined host-buffer entry ------------------------------------------------------------------------
 

@@ -105,7 +105,7 @@ FUSED_CASES = [   # loss, frozen, levels, poly, scale, bias, weighted, reduction
 @pytest.mark.parametrize("loss_type,frozen,levels,poly,scale,bias,weighted,reduction,n,ordered,seed", FUSED_CASES)
 def test_fused_eikonal_step_per_element(loss_type, frozen, levels, poly, scale, bias, weighted, reduction, n, ordered,
                                         seed):
-    """shine_sdf_bce_eikonal_step / shine_sdf_diff_eikonal_step (DEC_GRAD x {BCE, sdf_l1, sdf_l2}): pred, g, the loss and
+    """shine_sdf_eikonal_step (DEC_GRAD x {BCE, sdf_l1, sdf_l2}): pred, g, the loss and
     eikonal scalars and every table-gradient element within their bounds, at weight_e = 0.1 and at a dominant weight_e."""
     case = _case(levels, poly, seed, scale, weighted or loss_type != "sdf_bce", reduction, bias, n, ordered)
     case, dropped = clean_case(case, loss_type)

@@ -436,7 +436,7 @@ def _fused_eikonal(case, weight_e):
     pytest.param(4, True, True, "mean", 300.0, 60016, False, False, True, True, 164, id="n60016-x300"),
 ])
 def test_fused_eikonal_step_matches_oracle(levels, poly, weighted, reduction, scale, n, ordered, frozen, bias, outs, seed):
-    """ONE launch (shine_sdf_bce_eikonal_step) against the oracle's autograd double backward, for every configuration
+    """ONE launch (shine_sdf_eikonal_step) against the oracle's autograd double backward, for every configuration
     the kernel takes: 1..8 levels, poly / linear interpolation, weighted BCE with mean / sum, the frozen-decoder
     instantiation (table gradients only), a decoder without biases, table scale 1 and x300, tile tails, the grid-stride
     loop, a Morton-ordered batch (lanes of a warp hit the same rows), pred_out / grad_out passed or not."""
@@ -454,7 +454,7 @@ DIFF_LOSSES = ("sdf_l1", "sdf_l2")
 
 
 def _diff_eikonal_runs(case, loss_type, frozen=False, outs=True):
-    """The fused sdf_l1 / sdf_l2 + eikonal step (shine_sdf_diff_eikonal_step) at weight_e = 0.1, 0 and W = _eik_weight(case,
+    """The fused sdf_l1 / sdf_l2 + eikonal step (shine_sdf_eikonal_step) at weight_e = 0.1, 0 and W = _eik_weight(case,
     oracle), graded by _check_eikonal with the floor at most 0.1 of its bar.  The L1 oracle takes the kernel's sign near
     the label from a run with pred_out (the kernel's pred does not depend on the outputs asked for, so runs without
     them are graded against the same oracle).  -> (runs, oracle, report line with N, surface count and eikonal share)."""
@@ -495,7 +495,7 @@ DIFF_EIKONAL_CASES = [   # levels, poly, scale, n, ordered, frozen, bias, outs, 
 @pytest.mark.parametrize("loss_type", DIFF_LOSSES)
 @pytest.mark.parametrize("levels,poly,scale,n,ordered,frozen,bias,outs,seed", DIFF_EIKONAL_CASES)
 def test_fused_sdf_diff_eikonal_step_matches_oracle(loss_type, levels, poly, scale, n, ordered, frozen, bias, outs, seed):
-    """ONE launch of shine_sdf_diff_eikonal_step against the oracle's double backward, on the configurations of
+    """ONE launch of shine_sdf_eikonal_step against the oracle's double backward, on the configurations of
     test_fused_eikonal_step_matches_oracle that apply to sdf_diff_loss (always |w|, always the mean): 1..8 levels, poly /
     linear interpolation, the frozen-decoder instantiation, a decoder without biases, a Morton-ordered batch, tables
     x1 and x300, tile tails, the grid-stride loop, pred_out / grad_out passed or not."""

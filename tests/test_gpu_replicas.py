@@ -788,29 +788,29 @@ def test_fold_kernel_is_bit_exact(r, built_lib):
 # ---- ABI rejections (no GPU: the descriptor checks run before any device call) -------------------------------------------------
 
 def _abi_call(lib, name, desc):
+    """name: an entry, or "entry:main_loss_type" for the shine_sdf_* steps"""
     from shine_mapping_b200 import _abi
+    from shine_mapping_b200.trainer import loss_flags
     dec = _abi.ShineDecoder()
     dec.w1 = dec.w2 = dec.w3 = 0x1000
     dec.in_dim, dec.hidden, dec.mlp_level = 8, 32, 2
     o = C.byref(desc)
-    if name == "shine_sdf_bce_step":
-        return lib.shine_sdf_bce_step(o, C.byref(dec), None, None, None, 0, 1.0, 1.0, None, None, None, 0, None)
-    if name == "shine_sdf_bce_eikonal_step":
-        return lib.shine_sdf_bce_eikonal_step(o, C.byref(dec), None, None, None, 0, 1.0, 1.0, 0.1, None, None, None, None,
-                                              None, 0, None)
-    # the sdf_diff_loss entries need their weights and a valid scale even for an empty batch
-    if name == "shine_sdf_diff_step":
-        return lib.shine_sdf_diff_step(o, C.byref(dec), None, None, 0x3000, 0, 0.01, 1.0, None, None, None, 0, None)
-    if name == "shine_sdf_diff_eikonal_step":
-        return lib.shine_sdf_diff_eikonal_step(o, C.byref(dec), None, None, 0x3000, 0, 0.01, 1.0, 1.0, 0.1, None, None,
-                                               None, None, None, 0, None)
-    if name == "shine_query_bwd":
+    entry, _, loss = name.partition(":")
+    if entry == "shine_query_bwd":
         return lib.shine_query_bwd(o, None, 0, None, None)
-    return lib.shine_reduce_grad_replicas(o, None)
+    if entry == "shine_reduce_grad_replicas":
+        return lib.shine_reduce_grad_replicas(o, None)
+    # sdf_l1 / sdf_l2 need their weights and a valid scale even for an empty batch
+    weight, scale = (None, 1.0) if loss == "sdf_bce" else (0x3000, 0.01)
+    if entry == "shine_sdf_step":
+        return lib.shine_sdf_step(o, C.byref(dec), None, None, weight, 0, 1.0, scale, 1.0, None, None, None,
+                                  loss_flags(loss), None)
+    return lib.shine_sdf_eikonal_step(o, C.byref(dec), None, None, weight, 0, 1.0, scale, 1.0, 0.1, None, None, None, None,
+                                      None, loss_flags(loss), None)
 
-
-@pytest.mark.parametrize("name", ["shine_sdf_bce_step", "shine_query_bwd", "shine_reduce_grad_replicas",
-                                  "shine_sdf_bce_eikonal_step", "shine_sdf_diff_step", "shine_sdf_diff_eikonal_step"])
+@pytest.mark.parametrize("name", ["shine_sdf_step:sdf_bce", "shine_query_bwd", "shine_reduce_grad_replicas",
+                                  "shine_sdf_eikonal_step:sdf_bce", "shine_sdf_step:sdf_l1", "shine_sdf_step:sdf_l2",
+                                  "shine_sdf_eikonal_step:sdf_l1", "shine_sdf_eikonal_step:sdf_l2"])
 def test_abi_replica_checks(name, built_lib):
     """R must be a power of two up to 64 with a scratch pointer; R = 0 and 1 need no scratch.  Placeholder pointers and an
     empty batch: an accepted descriptor returns OK without touching the device."""

@@ -11,15 +11,15 @@ import torch
 from tests.parity_utils import GOLDEN_NAMES, ROOT, load_golden, make_case, make_config, oracle_from_case
 
 
-def test_library_exports_every_declared_symbol_at_abi_v4(built_lib):
+def test_library_exports_every_declared_symbol(built_lib):
     from shine_mapping_b200 import _abi
     header = open(os.path.join(ROOT, "include", "shine_b200.h")).read()
     declared = set(re.findall(r"\b(shine_[a-z0-9_]+)\s*\(", header))
     assert declared == set(_abi.SYMBOLS), declared ^ set(_abi.SYMBOLS)
     for name in declared:
         assert getattr(built_lib, name) is not None
-    # 4: the shine_sdf_* calls reject flag bits they do not know (ABI version 3 also defined bit 8)
-    assert built_lib.shine_abi_version() == _abi.ABI_VERSION == 4
+    # 5: one shine_sdf_fwd / _step / _eikonal_step for every point-wise loss, chosen by flag (4 had one call per loss)
+    assert built_lib.shine_abi_version() == _abi.ABI_VERSION == 5
     assert built_lib.shine_error_string(-2).decode().startswith("shine_b200: unsupported")
 
 
@@ -64,9 +64,10 @@ def test_abi_argument_checks_need_no_gpu(built_lib):
     assert built_lib.shine_octree_frame_nodes(C.byref(plan), None, 0, None) == -1
 
 
-def test_sdf_calls_reject_unknown_flag_bits(built_lib):
+def test_sdf_bce_calls_reject_unknown_flag_bits(built_lib):
     """A flag bit outside REDUCTION_SUM | WEIGHTED | TF32X1 | MORTON_ORDERED is SHINE_ERR_UNSUPPORTED, checked before
-    anything else: a caller still setting bit 8, which ABI version 3 defined, gets an error, not another kernel."""
+    anything else: a caller still setting bit 8, which ABI version 3 defined, gets an error, not another kernel.
+    shine_sdf_fwd / shine_sdf_step run sdf_bce here (no loss bit)."""
     import ctypes as C
     from shine_mapping_b200 import _abi
     oct_, dec = C.byref(_abi.ShineOctree()), C.byref(_abi.ShineDecoder())      # num_levels == 0: an invalid octree
@@ -74,8 +75,10 @@ def test_sdf_calls_reject_unknown_flag_bits(built_lib):
         "shine_sdf_infer": lambda f: built_lib.shine_sdf_infer(oct_, dec, None, 0, None, None, 0, f, None),
         "shine_sdf_bce_fwd": lambda f: built_lib.shine_sdf_bce_fwd(oct_, dec, None, None, None, 0, 1.0, 1.0, None, None,
                                                                    f, None),
-        "shine_sdf_bce_step": lambda f: built_lib.shine_sdf_bce_step(oct_, dec, None, None, None, 0, 1.0, 1.0, None, None,
-                                                                     None, f, None),
+        "shine_sdf_fwd": lambda f: built_lib.shine_sdf_fwd(oct_, dec, None, None, None, 0, 1.0, 1.0, 1.0, None, None, f,
+                                                           None),
+        "shine_sdf_step": lambda f: built_lib.shine_sdf_step(oct_, dec, None, None, None, 0, 1.0, 1.0, 1.0, None, None,
+                                                             None, f, None),
     }
     known = _abi.FLAG_REDUCTION_SUM | _abi.FLAG_WEIGHTED | _abi.FLAG_TF32X1 | _abi.FLAG_MORTON_ORDERED
     for name, call in calls.items():

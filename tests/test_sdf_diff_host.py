@@ -1,6 +1,6 @@
 """CPU tests of training with the reference's sdf_l1 / sdf_l2 losses: the fp64 oracle against goldens minted from the
-reference (oracle/make_sdf_diff_golden.py), the C-ABI argument checks of the shine_sdf_diff_* entries, and which loops
-accept which main_loss_type."""
+reference (oracle/make_sdf_diff_golden.py), the C-ABI argument checks of the shine_sdf_* entries with the sdf_l1 / sdf_l2
+loss bits, and which loops accept which main_loss_type."""
 import ctypes as C
 import os
 
@@ -98,44 +98,65 @@ def _fake_descriptors():
 
 
 def _calls(lib, o, d, p):
-    """entry -> f(weight, scale, flags)"""
+    """entry -> f(weight, scale, flags), sigma = 0.01"""
     oc, dc = C.byref(o), C.byref(d)
     cnt = C.c_int32(0)
     return {
-        "shine_sdf_diff_fwd": lambda w, s, f: lib.shine_sdf_diff_fwd(oc, dc, None, None, w, 0, s, 1.0, None, None, f, None),
-        "shine_sdf_diff_step": lambda w, s, f: lib.shine_sdf_diff_step(oc, dc, None, None, w, 0, s, 1.0, None, None, None,
-                                                                       f, None),
-        "shine_sdf_diff_eikonal_step": lambda w, s, f: lib.shine_sdf_diff_eikonal_step(
-            oc, dc, None, None, w, 0, s, 0.01, 1.0, 0.1, C.addressof(cnt), None, None, None, None, f, None),
+        "shine_sdf_fwd": lambda w, s, f: lib.shine_sdf_fwd(oc, dc, None, None, w, 0, 0.01, s, 1.0, None, None, f, None),
+        "shine_sdf_step": lambda w, s, f: lib.shine_sdf_step(oc, dc, None, None, w, 0, 0.01, s, 1.0, None, None, None, f,
+                                                             None),
+        "shine_sdf_eikonal_step": lambda w, s, f: lib.shine_sdf_eikonal_step(
+            oc, dc, None, None, w, 0, 0.01, s, 1.0, 0.1, C.addressof(cnt), None, None, None, None, f, None),
     }
 
 
-def test_diff_entries_are_exported(built_lib):
+def test_loss_selected_entries_are_exported(built_lib):
     from shine_mapping_b200 import _abi
-    for name in ("shine_sdf_diff_fwd", "shine_sdf_diff_step", "shine_sdf_diff_eikonal_step"):
+    for name in ("shine_sdf_fwd", "shine_sdf_step", "shine_sdf_eikonal_step"):
         assert name in _abi.SYMBOLS and getattr(built_lib, name) is not None
-    assert _abi.FLAG_LOSS_L2 == 32
+    assert (_abi.FLAG_LOSS_L2, _abi.FLAG_LOSS_L1) == (32, 64)
 
 
-def test_diff_entries_check_flags_weight_and_scale(built_lib):
+def test_l1_l2_entries_check_flags_weight_and_scale(built_lib):
     from shine_mapping_b200 import _abi
     buf, o, d, p = _fake_descriptors()
-    accepted = {"shine_sdf_diff_fwd": _abi.FLAG_TF32X1 | _abi.FLAG_LOSS_L2,
-                "shine_sdf_diff_step": _abi.FLAG_TF32X1 | _abi.FLAG_LOSS_L2 | _abi.FLAG_MORTON_ORDERED,
-                "shine_sdf_diff_eikonal_step": _abi.FLAG_TF32X1 | _abi.FLAG_LOSS_L2}
-    for name, call in _calls(built_lib, o, d, p).items():
-        ok = accepted[name]
-        for f in (0, _abi.FLAG_LOSS_L2, ok):
-            assert call(p, 0.01, f) == 0, (name, f)                       # n = 0: valid arguments, nothing launched
-        for bit in range(32):
-            if not (1 << bit) & ok:   # REDUCTION_SUM, WEIGHTED, the retired bit 8, MORTON_ORDERED on the forward-only calls
-                assert call(p, 0.01, 1 << bit) == -2, (name, bit)
-        assert call(None, 0.01, 0) == -1, name                           # the weight is required
-        for bad in (0.0, -0.01, float("inf"), float("nan")):
-            assert call(p, bad, 0) == -1, (name, bad)
-    # the BCE entries keep refusing the new bit
+    for loss in (_abi.FLAG_LOSS_L1, _abi.FLAG_LOSS_L2):
+        accepted = {"shine_sdf_fwd": _abi.FLAG_TF32X1 | loss,
+                    "shine_sdf_step": _abi.FLAG_TF32X1 | loss | _abi.FLAG_MORTON_ORDERED,
+                    "shine_sdf_eikonal_step": _abi.FLAG_TF32X1 | loss}
+        for name, call in _calls(built_lib, o, d, p).items():
+            ok = accepted[name]
+            for f in (loss, ok):
+                assert call(p, 0.01, f) == 0, (name, loss, f)                 # n = 0: valid arguments, nothing launched
+            # REDUCTION_SUM, WEIGHTED, the retired bit 8, the other loss bit, MORTON_ORDERED on the forward-only calls
+            for bit in range(32):
+                if not (1 << bit) & ok:
+                    assert call(p, 0.01, loss | 1 << bit) == -2, (name, loss, bit)
+            assert call(None, 0.01, loss) == -1, (name, loss)                # the weight is required
+            for bad in (0.0, -0.01, float("inf"), float("nan")):
+                assert call(p, bad, loss) == -1, (name, loss, bad)
+
+
+def test_loss_bits_and_the_bce_flags(built_lib):
+    """Both loss bits are refused by every entry; the BCE eikonal step refuses the bits it does not know (REDUCTION_SUM
+    is accepted: the reduction comes in loss_scale); shine_sdf_bce_fwd refuses either loss bit."""
+    from shine_mapping_b200 import _abi
+    buf, o, d, p = _fake_descriptors()
+    calls = _calls(built_lib, o, d, p)
+    both = _abi.FLAG_LOSS_L1 | _abi.FLAG_LOSS_L2
+    for name, call in calls.items():
+        assert call(p, 0.01, both) == -2, name
+        assert call(p, 0.01, both | _abi.FLAG_TF32X1) == -2, name
+    eik = calls["shine_sdf_eikonal_step"]
+    ok = _abi.FLAG_REDUCTION_SUM | _abi.FLAG_WEIGHTED | _abi.FLAG_TF32X1
+    assert eik(p, 0.01, ok) == 0
+    for bit in range(32):
+        if not (1 << bit) & (ok | both):                # MORTON_ORDERED, the retired bit 8, ...
+            assert eik(p, 0.01, 1 << bit) == -2, bit
     oc, dc = C.byref(o), C.byref(d)
-    assert built_lib.shine_sdf_bce_step(oc, dc, None, None, None, 0, 1.0, 1.0, None, None, None, _abi.FLAG_LOSS_L2, None) == -2
+    for bit in (_abi.FLAG_LOSS_L1, _abi.FLAG_LOSS_L2):
+        assert built_lib.shine_sdf_bce_fwd(oc, dc, None, None, None, 0, 1.0, 1.0, None, None, bit, None) == -2, bit
+    assert built_lib.shine_sdf_bce_fwd(oc, dc, None, None, None, 0, 1.0, 1.0, None, None, 0, None) == 0
 
 
 def test_sdf_diff_step_refuses_cpu_tensors(built_lib):
@@ -150,9 +171,9 @@ def test_sdf_diff_step_refuses_cpu_tensors(built_lib):
         sdf_diff_step(octree, dec, coord, torch.zeros(4), None, cfg.scale)
 
 
-def test_batch_loop_accepts_the_point_losses_and_the_incremental_loop_does_not():
+def test_loss_flags_and_which_loops_accept_which_loss():
     from shine_mapping_b200.batch_loop import BATCH_LOSSES, check_supported
-    from shine_mapping_b200.trainer import diff_loss_flags
+    from shine_mapping_b200.trainer import loss_flags
     from shine_mapping_b200 import _abi
     cfg = make_config(2)
     for loss in ("sdf_bce", "sdf_l1", "sdf_l2"):
@@ -161,9 +182,9 @@ def test_batch_loop_accepts_the_point_losses_and_the_incremental_loop_does_not()
         if loss != "sdf_bce":
             with pytest.raises(NotImplementedError):
                 check_supported(cfg, main_losses=("sdf_bce",))            # incre_loop's check
-    assert [diff_loss_flags(t) for t in BATCH_LOSSES] == [None, 0, _abi.FLAG_LOSS_L2]
+    assert [loss_flags(t) for t in BATCH_LOSSES] == [0, _abi.FLAG_LOSS_L1, _abi.FLAG_LOSS_L2]
     with pytest.raises(NotImplementedError):
-        diff_loss_flags("dr")
+        loss_flags("dr")
     for loss in ("dr", "dr_neus", "sdf_huber"):
         cfg.main_loss_type = loss
         with pytest.raises(NotImplementedError):

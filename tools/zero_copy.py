@@ -20,8 +20,8 @@ def zero_copy_step(c_h, l_h):
     tr.zero_grad()
     od = tr.octree._descriptor(None, tr.table_grads, n_points=n)
     dd = tr.decoder.c_descriptor(tr.dec_grads)
-    _abi.check(lib.shine_sdf_bce_step(C.byref(od), C.byref(dd), C.c_void_p(c_h.data_ptr()), C.c_void_p(l_h.data_ptr()), None, n,
-                                      float(tr.sigma), 1.0 / n, None, None, _abi.ptr(tr.loss), 0, st), "step")
+    _abi.check(lib.shine_sdf_step(C.byref(od), C.byref(dd), C.c_void_p(c_h.data_ptr()), C.c_void_p(l_h.data_ptr()), None, n,
+                                  float(tr.sigma), 1.0, 1.0 / n, None, None, _abi.ptr(tr.loss), 0, st), "step")
     tr.octree._reduce_replicas(od, dev)
     return float(tr.loss.item())
 
