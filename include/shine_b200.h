@@ -566,6 +566,19 @@ int shine_register_normal_eq(const shine_octree* oct, const shine_decoder* dec, 
                              const double* pose, float sigma, double kappa, double* out, void* scratch,
                              int64_t scratch_bytes, void* stream);
 
+/* The same normal equations at num_poses poses of one scan (a grid search, several Gauss-Newton starts): poses is host
+ * fp64 [num_poses, 16] (each as pose above), out device fp64 [num_poses, SHINE_REGISTER_OUT].  Row k equals, bit for
+ * bit, what shine_register_normal_eq returns at pose k: the same per-point work, block count and fold order, with the
+ * pose as the grid's second dimension.  scratch (device, 8-byte aligned) holds every pose's block partials:
+ * shine_register_scratch_bytes(n, num_poses) bytes, that is min(ceil(n / 256), SHINE_REGISTER_MAX_BLOCKS) * num_poses *
+ * SHINE_REGISTER_OUT * 8.  num_poses <= 0 or above INT32_MAX, a NULL poses or out, a non-finite entry of any pose, a short
+ * scratch and the checks of shine_register_normal_eq are refused as there, before any launch.  shine_register_scratch_bytes
+ * returns -1 for n < 0 or such a num_poses. */
+int64_t shine_register_scratch_bytes(int64_t n, int64_t num_poses);
+int shine_register_normal_eq_poses(const shine_octree* oct, const shine_decoder* dec, const float* points, int64_t n,
+                                   const double* poses, int64_t num_poses, float sigma, double kappa, double* out,
+                                   void* scratch, int64_t scratch_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -190,6 +190,9 @@ SYMBOLS = {
     "shine_nn_query": (C.c_int, [_vp, _i64, _vp, _i64, C.c_double, _vp, _vp, _vp, _i64, _vp]),
     "shine_register_normal_eq": (C.c_int, [_OCT, _DEC, _vp, _i64, C.POINTER(C.c_double), _f32, C.c_double, _vp, _vp,
                                            _i64, _vp]),
+    "shine_register_scratch_bytes": (C.c_int64, [_i64, _i64]),
+    "shine_register_normal_eq_poses": (C.c_int, [_OCT, _DEC, _vp, _i64, C.POINTER(C.c_double), _i64, _f32, C.c_double,
+                                                 _vp, _vp, _i64, _vp]),
 }
 
 _lib = None

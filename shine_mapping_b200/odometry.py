@@ -5,6 +5,7 @@ residuals of its points (scan-to-implicit-map odometry).  For a pose T and the s
 its Jacobian for a left-multiplied twist xi = (rho, phi) is [g_i, (T p_i) x g_i], g_i the SDF gradient.
 `shine_register_normal_eq` (csrc/shine_register.cu) forms the robust (Geman-McClure) normal equations of one iterate in
 one pass over the scan; the 6x6 system is solved here in fp64, one 29-double read per iteration.
+`shine_register_normal_eq_poses` forms them at many poses in one call (the coarse grid, the weak-direction search).
 
 * `se3_exp` / `se3_log` — the SE(3) exponential and logarithm in fp64, twist (rho, phi).
 * `ScanToMapRegistration` — the normal equations and the Gauss-Newton loop.
@@ -119,6 +120,8 @@ class ScanToMapRegistration:
     GRID_X = np.arange(-8, 9) * 0.25
     GRID_Y = np.arange(-2, 3) * 0.25
     GRID_YAW = np.radians(np.arange(-6, 7) * 1.0)
+    # launch_poses splits a batch of poses so that its block partials stay within this many bytes of scratch
+    SCRATCH_BOUND_BYTES = 64 << 20
 
     def __init__(self, config: SHINEConfig, octree, decoder, kappa_m: float = 0.1, max_iters: int = 30,
                  tol: float = 1e-4, min_valid: int = 100, search_m: float = 2.0, search_step_m: float = 0.1):
@@ -144,6 +147,56 @@ class ScanToMapRegistration:
             _abi.ptr(self.out if out is None else out), _abi.ptr(self.scratch), self.scratch.numel(),
             _abi.stream_ptr(self.device)),
             "shine_register_normal_eq")
+
+    def launch_poses(self, points: torch.Tensor, poses_scaled: np.ndarray, kappa_scaled: float, out: torch.Tensor) -> None:
+        """The normal equations at K poses (fp64 [K,4,4], translation in scaled units) into out (fp64 [K,29]; no host
+        read): shine_register_normal_eq_poses, whose row k equals `launch` at pose k bit for bit.  The poses go in
+        batches whose block partials fit SCRATCH_BOUND_BYTES (a 10^6-point scan needs 237 KB per pose, so the 1105
+        candidates of the coarse grid take 4 calls; a 3*10^4-point scan takes one).
+
+        A subclass that replaces the field by overriding `launch` (a host-side restatement) keeps working: when `launch`
+        is overridden, this calls it once per pose into the rows of out."""
+        poses = np.ascontiguousarray(poses_scaled, dtype=np.float64).reshape(-1, 16)
+        K = poses.shape[0]
+        if out.dtype != torch.float64 or tuple(out.shape) != (K, _abi.REGISTER_OUT) or not out.is_contiguous():
+            raise ValueError(f"launch_poses writes fp64 [{K}, {_abi.REGISTER_OUT}] rows: out is {out.dtype} "
+                             f"{tuple(out.shape)}{'' if out.is_contiguous() else ', not contiguous'}")
+        if type(self).launch is not ScanToMapRegistration.launch:
+            for k in range(K):
+                self.launch(points, poses[k].reshape(4, 4), kappa_scaled, out[k])
+            return
+        _abi.require_cuda(points, "ScanToMapRegistration")
+        if out.device != points.device:
+            raise ValueError(f"launch_poses: out is on {out.device}, the points on {points.device}")
+        points = points.float().contiguous()
+        n = points.shape[0]
+        lib = _abi.lib()
+        per_pose = max(1, lib.shine_register_scratch_bytes(n, 1))
+        chunk = max(1, min(K, self.SCRATCH_BOUND_BYTES // per_pose))
+        need = lib.shine_register_scratch_bytes(n, chunk)
+        if self.scratch.numel() < need:
+            self.scratch = torch.empty(need, dtype=torch.uint8, device=self.device)
+        od = self.octree._descriptor(None, None)
+        dd = self.decoder.c_descriptor(None)
+        for k0 in range(0, K, chunk):
+            kc = min(chunk, K - k0)
+            buf = (C.c_double * (16 * kc))(*poses[k0:k0 + kc].reshape(-1).tolist())
+            _abi.check(lib.shine_register_normal_eq_poses(
+                C.byref(od), C.byref(dd), _abi.ptr(points), n, buf, kc, self.sigma, float(kappa_scaled),
+                _abi.ptr(out[k0:k0 + kc]), _abi.ptr(self.scratch), self.scratch.numel(), _abi.stream_ptr(self.device)),
+                "shine_register_normal_eq_poses")
+
+    def _scaled(self, poses) -> np.ndarray:
+        P = np.array(poses, dtype=np.float64).reshape(-1, 4, 4)
+        P[:, :3, 3] *= self.scale
+        return P
+
+    def normal_equations_at(self, points: torch.Tensor, poses, kappa_m: float | None = None) -> list:
+        """[(H, b, cost, count)] at each of the poses (metres), one launch_poses and one read."""
+        P = self._scaled(poses)
+        out = torch.empty(P.shape[0], _abi.REGISTER_OUT, dtype=torch.float64, device=self.device)
+        self.launch_poses(points, P, (self.kappa_m if kappa_m is None else kappa_m) * self.scale, out)
+        return [unpack_normal_equations(row) for row in out.cpu().numpy()]
 
     def normal_equations(self, points: torch.Tensor, pose: np.ndarray, kappa_m: float | None = None) -> tuple:
         """(H, b, cost, count) of the scan at `pose` (metres): H = sum w J^T J, b = sum w J^T r over the points on the
@@ -172,21 +225,23 @@ class ScanToMapRegistration:
         return pose, self.max_iters, False, None
 
     def search_weak_direction(self, points: torch.Tensor, pose: np.ndarray) -> tuple:
-        """The best pose along the weakest translation direction (class docstring) -> (pose, moved)."""
+        """The best pose along the weakest translation direction (class docstring), all candidates in one launch_poses
+        -> (pose, moved)."""
         H, _, _, _ = self.normal_equations(points, pose)
         score0 = float(np.trace(H[:3, :3]))
         v = np.linalg.eigh(H[:3, :3])[1][:, 0]              # eigenvalues ascending
         n = int(round(self.search_m / self.search_step_m))
-        best, best_score = 0.0, score0
-        for k in range(-n, n + 1):
-            if k == 0:
-                continue
+        steps = [k * self.search_step_m for k in range(-n, n + 1) if k != 0]
+        cands = []
+        for d in steps:
             cand = pose.copy()
-            cand[:3, 3] += k * self.search_step_m * v
-            H, _, _, _ = self.normal_equations(points, cand)
+            cand[:3, 3] += d * v
+            cands.append(cand)
+        best, best_score = 0.0, score0
+        for d, (H, _, _, _) in zip(steps, self.normal_equations_at(points, cands)):
             score = float(np.trace(H[:3, :3]))
             if score > best_score:
-                best, best_score = k * self.search_step_m, score
+                best, best_score = d, score
         if best_score <= score0 * (1.0 + 1e-3):
             return pose, False
         out = pose.copy()
@@ -195,7 +250,7 @@ class ScanToMapRegistration:
 
     def coarse_search(self, points: torch.Tensor, pose: np.ndarray) -> np.ndarray:
         """The candidate of the grid around pose (GRID_X x GRID_Y x GRID_YAW) with the largest inlier score sum w |g|^2
-        at twice kappa: one launch per candidate into its own row, one read for all of them."""
+        at twice kappa: one launch_poses into one row per candidate, one read for all of them."""
         cands = []
         for yaw in self.GRID_YAW:
             c, s_ = math.cos(yaw), math.sin(yaw)
@@ -207,10 +262,7 @@ class ScanToMapRegistration:
                     T[:3, 3] = pose[:3, 3] + (dx, dy, 0.0)
                     cands.append(T)
         outs = torch.empty(len(cands), _abi.REGISTER_OUT, dtype=torch.float64, device=self.device)
-        for k, T in enumerate(cands):
-            Ts = T.copy()
-            Ts[:3, 3] *= self.scale
-            self.launch(points, Ts, 2.0 * self.kappa_m * self.scale, outs[k])
+        self.launch_poses(points, self._scaled(cands), 2.0 * self.kappa_m * self.scale, outs)
         score = (outs[:, 0] + outs[:, 6] + outs[:, 11]).cpu().numpy()        # H(0,0) + H(1,1) + H(2,2)
         return cands[int(np.argmax(score))]
 
