@@ -371,8 +371,13 @@ struct SmemPlan {
     static constexpr int GSCALE = B3 + 1;              // [1] (+2 pad) dL/dpred scale: read per tile, not held in a register
     static constexpr int kDecGradFloats = kH * kF + kH + kH * kH + kH + kH + 1;   // 1377 (a warp's partial goes to its staging area)
     static constexpr int ZSUM = B3 + 4;                // [8] the warps' dL/dpred sums of their zero tiles (zero-tile shortcut)
-    static constexpr int kZsumFloats = 8 * 5 * kTile;  // more than the 8 sums need: the offsets below and the block's
+    static constexpr int H1Z = ZSUM + 8;               // [32] h1(0) = relu(b1)     } the gradient g0 of Decoder.sdf(0) per unit
+    static constexpr int H2Z = H1Z + kH;               // [32] h2(0)                } dL/dpred, in fp32 (zero_tile_gradient)
+    static constexpr int D2Z = H2Z + kH;               // [32] db2 = w3 * [a2(0) > 0]
+    static constexpr int DB1Z = D2Z + kH;              // [32] db1 = (W2^T db2) * [b1 > 0]
+    static constexpr int kZsumFloats = 8 * 5 * kTile;  // more than the sums and g0 need: the offsets below and the block's
                                                        // shared-memory footprint were timed with this size
+    static_assert(DB1Z + kH <= ZSUM + kZsumFloats, "g0 fits the zero-tile corner");
     static constexpr int STAGE = ZSUM + kZsumFloats;   // per-warp staging of one tile, in mma fragment order (below)
     static constexpr int SB2 = 0;                      // h1:  B fragments of dW2, [k-step 2][n-tile 4][32 lanes][2]
     static constexpr int SU = SB2;                     // GROUPED: h1 as A fragments of T = (dp h1)^T M2 (rows = layer-1
@@ -392,6 +397,36 @@ struct SmemPlan {
     // [m-tile 2][n-tile 4][32 lanes][4]
     static constexpr int kW2Part = kH * kH;
 };
+
+// The zero-tile shortcut's closed form (sdf_fused_kernel).  A point with features 0 has h1 = relu(b1) and a2 = W2 h1 + b2,
+// so the gradient of Decoder.sdf(0) is  dW1 = 0, db1 = (W2^T db2) * [b1 > 0], dW2 = db2 h1^T, db2 = w3 * [a2 > 0],
+// dw3 = relu(a2), db3 = 1.  One warp (lane = unit) writes its vectors to SmemPlan::H1Z .. DB1Z in plain fp32.
+__device__ __forceinline__ void zero_tile_gradient(float* smem, const float* __restrict__ w2, int lane) {
+    const float h1 = fmaxf(smem[SmemPlan::B1 + lane], 0.f);
+    float a2 = smem[SmemPlan::B2 + lane];
+#pragma unroll
+    for (int k = 0; k < kH; ++k) a2 = fmaf(__ldg(w2 + lane * kH + k), __shfl_sync(kFull, h1, k), a2);
+    const float d2 = a2 > 0.f ? smem[SmemPlan::W3 + lane] : 0.f;
+    float db1 = 0.f;
+#pragma unroll
+    for (int n = 0; n < kH; ++n) db1 = fmaf(__ldg(w2 + n * kH + lane), __shfl_sync(kFull, d2, n), db1);
+    smem[SmemPlan::H1Z + lane] = h1;
+    smem[SmemPlan::H2Z + lane] = fmaxf(a2, 0.f);
+    smem[SmemPlan::D2Z + lane] = d2;
+    smem[SmemPlan::DB1Z + lane] = h1 > 0.f ? db1 : 0.f;
+}
+// The block's dL/dpred sum over its zero tiles (the warps' sums are in SmemPlan::ZSUM, after a block barrier).  A block
+// with zero tiles then also gets g0 (one more barrier); a block without any leaves g0 unwritten and must not read it.
+__device__ __forceinline__ float zero_tile_sum_and_gradient(float* smem, const float* __restrict__ w2, int warp, int lane) {
+    float s = 0.f;
+#pragma unroll
+    for (int w = 0; w < 8; ++w) s += smem[SmemPlan::ZSUM + w];
+    if (s != 0.f) {                 // block-uniform
+        if (warp == 0) zero_tile_gradient(smem, w2, lane);
+        __syncthreads();
+    }
+    return s;
+}
 
 // ---- voxel-grouped scatter (GROUPED kernels: batches in Morton order) ---------------------------------------------
 // In a Morton-ordered batch the 16 points of a tile fall into a few groups of equal node per level.  The per-group gradient
@@ -658,13 +693,18 @@ sdf_fused_kernel(const __grid_constant__ StepParams P, const __grid_constant__ S
     prefetch_inputs(warp_global);
 
     // Zero-tile shortcut.  A point that misses every level has the feature vector 0, so every such point gets the
-    // SAME prediction pred0 = Decoder.sdf(0), and its decoder gradients are dL/dpred times the gradients of that one forward:
-    // linear in dL/dpred.  In a Morton-ordered batch free-space samples fill whole tiles (35 % of the C2 tiles): such a tile
-    // only walks the hash, evaluates its loss terms against pred0 and adds its dL/dpred to a sum.  Pass 0 of the loop below
-    // is one virtual tile (no points: features 0) run through the forward to get pred0; after the block's real tiles, warp 0
-    // runs one more virtual tile whose first point carries the block's dL/dpred sum through the ordinary backward.
-    int phase = 0;                          // 0: virtual forward, 1: this warp's tiles, 2: virtual backward (warp 0)
-    bool advance = false, last_pass = false;
+    // SAME prediction pred0 = Decoder.sdf(0), and its decoder gradients are dL/dpred times the gradient g0 of that one
+    // forward: linear in dL/dpred.  In a Morton-ordered batch free-space samples fill whole tiles (35 % of the C2 tiles):
+    // such a tile only walks the hash, evaluates its loss terms against pred0 and adds its dL/dpred to a sum.  Pass 0 of
+    // the loop below is one virtual tile (no points: features 0) run through the forward to get pred0; the epilogue adds
+    // the block's dL/dpred sum times g0 in closed form (zero_tile_gradient).
+    int phase = 0;                          // 0: virtual forward, 1: this warp's tiles
+    bool advance = false;
+    // Inference kernels only: an exit flag that never becomes true (phase is never 2).  The loop had a third pass (a virtual backward tile, now
+    // the closed form above) that ended it through this flag; without its test ptxas lays the inference loop out anew
+    // and spills inside it (<3,0,0,4,BatchCoords>: 52 B).  With it their SASS is the one they had.  The training kernels
+    // do better without it (the grouped kernel spills nothing).
+    bool infer_exit = false;
     float pred0 = 0.f, zsum = 0.f;
     // one sample's loss term li (the caller weights it) and dL/dpred dp (weighted and scaled)
     auto loss_point = [&](float pv, float lb, float wg, float& li, float& dp) {
@@ -686,28 +726,11 @@ sdf_fused_kernel(const __grid_constant__ StepParams P, const __grid_constant__ S
         }
     };
     for (int seq = warp_global;; seq = advance ? seq + warp_stride : seq) {
-        if (last_pass) break;
+        if (!TRAIN && infer_exit) break;
         const int tile = seq;
-        if (phase == 1 && seq >= P.num_tiles) {
-            if constexpr (DEC_GRAD) {
-                // hand the all-miss dL/dpred sums of the block's warps to warp 0 (every warp passes here exactly once)
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) zsum += __shfl_xor_sync(kFull, zsum, o);
-                if (lane == 0) smem[SmemPlan::ZSUM + warp] = zsum;
-                __syncthreads();
-                if (warp != 0) break;
-                float tot = 0.f;
-#pragma unroll
-                for (int w = 0; w < kWarps; ++w) tot += smem[SmemPlan::ZSUM + w];
-                if (tot == 0.f) break;
-                zsum = tot;
-                phase = 2;
-            } else {
-                break;
-            }
-        }
+        if (phase == 1 && seq >= P.num_tiles) break;
         const bool virt = phase != 1;
-        last_pass = phase == 2;
+        if (!TRAIN) infer_exit = phase == 2;
         advance = !virt;
         const int64_t base = (int64_t)tile * kTile;
         const int64_t myp = base + g + 8 * odd;
@@ -876,7 +899,7 @@ sdf_fused_kernel(const __grid_constant__ StepParams P, const __grid_constant__ S
         }
         if (phase == 1 && __ballot_sync(kFull, hitmask != 0u) == 0u) {
             // no point of this tile sees a node on any level: features 0, prediction pred0, no table gradient; the decoder
-            // gradients follow by linearity from the sum of dL/dpred (virtual backward tile at the end of the block)
+            // gradients follow by linearity from the sum of dL/dpred (g0 in the epilogue)
             if (!TRAIN && P.mask && half == 0 && valid) P.mask[myp] = 0;
             if (P.pred && half == 0 && valid) P.pred[myp] = src.out(pred0);
             if (P.label != nullptr && valid) {
@@ -986,7 +1009,6 @@ sdf_fused_kernel(const __grid_constant__ StepParams P, const __grid_constant__ S
             if (half == 0) loss_acc += wgt * li;
         }
         if (!TRAIN) continue;
-        if (phase == 2) dpo = (g == 0 && odd == 0) ? zsum : 0.f;   // point 0 of the virtual tile carries the block's sum
 
         // ---- backward: MLP dgrad on tensor cores ------------------------------------------------------
         const float dpx = __shfl_xor_sync(kFull, dpo, 1);
@@ -1222,6 +1244,11 @@ sdf_fused_kernel(const __grid_constant__ StepParams P, const __grid_constant__ S
         for (int o = 16; o > 0; o >>= 1) loss_acc += __shfl_xor_sync(kFull, loss_acc, o);
         if (lane == 0 && loss_acc != 0.f) atomicAdd(P.loss, loss_acc * P.loss_scale);
     }
+    if (DEC_GRAD) {       // this warp's dL/dpred sum over its zero tiles: the block adds their sum times g0 below
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) zsum += __shfl_xor_sync(kFull, zsum, o);
+        if (lane == 0) smem[SmemPlan::ZSUM + warp] = zsum;
+    }
     if (DEC_GRAD && GROUPED) {
         // per-warp partials [gw1 256 | gb1 32 | gb2 32 | gw3 32 | gb3 1] in the staging area (each element has exactly one
         // owner lane) and dW2 in its C-fragment image; the block sums the eight partials of each element and issues one
@@ -1245,17 +1272,20 @@ sdf_fused_kernel(const __grid_constant__ StepParams P, const __grid_constant__ S
         for (int o = 16; o > 0; o >>= 1) db3p += __shfl_xor_sync(kFull, db3p, o);
         if (lane == 0) part[oB3] = db3p;
         __syncthreads();
+        const float zs = zero_tile_sum_and_gradient(smem, P.dec.w2, warp, lane);
         for (int i = tid; i < kVec + kH * kH; i += blockDim.x) {
-            float v = 0.f;
+            float v = 0.f, g0 = 0.f;   // g0: this element's gradient of Decoder.sdf(0) (dW1: 0)
             float* dst;
             if (i < kVec) {
 #pragma unroll
                 for (int w = 0; w < kWarps; ++w) v += smem[SmemPlan::STAGE + w * kStage + i];
                 if (i < oB1) dst = P.dec.gw1 + i;
-                else if (i < oB2) dst = P.dec.gb1 ? P.dec.gb1 + (i - oB1) : nullptr;
-                else if (i < oW3) { v *= smem[SmemPlan::W3 + (i - oB2)]; dst = P.dec.gb2 ? P.dec.gb2 + (i - oB2) : nullptr; }
-                else if (i < oB3) dst = P.dec.gw3 + (i - oW3);
-                else dst = P.dec.gb3;
+                else if (i < oB2) { g0 = smem[SmemPlan::DB1Z + (i - oB1)]; dst = P.dec.gb1 ? P.dec.gb1 + (i - oB1) : nullptr; }
+                else if (i < oW3) {
+                    v *= smem[SmemPlan::W3 + (i - oB2)]; g0 = smem[SmemPlan::D2Z + (i - oB2)];
+                    dst = P.dec.gb2 ? P.dec.gb2 + (i - oB2) : nullptr;
+                } else if (i < oB3) { g0 = smem[SmemPlan::H2Z + (i - oW3)]; dst = P.dec.gw3 + (i - oW3); }
+                else { g0 = 1.f; dst = P.dec.gb3; }
             } else {   // dW2[r][c] = w3[r] T[c][r]: fragment (c >> 4, r >> 3), lane 4 (c & 7) + ((r & 7) >> 1), register
                        // 2 ((c >> 3) & 1) + (r & 1)
                 const int e = i - kVec, r = e / kH, c = e % kH;
@@ -1263,8 +1293,10 @@ sdf_fused_kernel(const __grid_constant__ StepParams P, const __grid_constant__ S
 #pragma unroll
                 for (int w = 0; w < kWarps; ++w) v += w2p[(w - warp) * SmemPlan::kW2Part + f];
                 v *= smem[SmemPlan::W3 + r];
+                if (zs != 0.f) g0 = smem[SmemPlan::D2Z + r] * smem[SmemPlan::H1Z + c];
                 dst = P.dec.gw2 + e;
             }
+            if (zs != 0.f) v = fmaf(zs, g0, v);
             if (v != 0.f && dst) atomicAdd(dst, v);
         }
     }
@@ -1305,10 +1337,20 @@ sdf_fused_kernel(const __grid_constant__ StepParams P, const __grid_constant__ S
         for (int o = 16; o > 0; o >>= 1) db3p += __shfl_xor_sync(kFull, db3p, o);
         if (lane == 0) part[oB3] = db3p;
         __syncthreads();
+        const float zs = zero_tile_sum_and_gradient(smem, P.dec.w2, warp, lane);
         for (int i = tid; i < SmemPlan::kDecGradFloats; i += blockDim.x) {
             float v = 0.f;
 #pragma unroll
             for (int w = 0; w < kWarps; ++w) v += smem[SmemPlan::STAGE + w * kStage + i];
+            if (zs != 0.f && i >= oB1) {   // dW1 of a zero tile is 0
+                float g0;
+                if (i < oW2) g0 = smem[SmemPlan::DB1Z + (i - oB1)];
+                else if (i < oB2) g0 = smem[SmemPlan::D2Z + (i - oW2) / kH] * smem[SmemPlan::H1Z + (i - oW2) % kH];
+                else if (i < oW3) g0 = smem[SmemPlan::D2Z + (i - oB2)];
+                else if (i < oB3) g0 = smem[SmemPlan::H2Z + (i - oW3)];
+                else g0 = 1.f;
+                v = fmaf(zs, g0, v);
+            }
             if (v == 0.f) continue;
             float* dst;
             if (i < oB1) dst = P.dec.gw1 + i;
