@@ -579,6 +579,26 @@ int shine_register_normal_eq_poses(const shine_octree* oct, const shine_decoder*
                                    const double* poses, int64_t num_poses, float sigma, double kappa, double* out,
                                    void* scratch, int64_t scratch_bytes, void* stream);
 
+/* ---- ray casting: where rays from one sensor origin first meet the map's zero level set (evaluate.py eval_scans) ----
+ * Ray i goes from origin (host fp32 [3], scaled) towards points[i] (device fp32 [n,3], scaled, map frame).  fp32, every
+ * operation rounded on its own: v = p - o, r = sqrt((vx vx + vy vy) + vz vz), d = v / r, and the lattice
+ *   t_k = t_min + k h,  x_k = o + t_k d,  k = 0 .. K,  K = min(floor((min(r + beyond, t_max) - t_min) / h), 2^24 - 1)
+ * (no sample when K < 0, or r is 0 or not finite).  At each sample m_k = x_k's voxel exists at lv[mask_level] and
+ * s_k = -Decoder.sdf(f(x_k)): the value and mask of shine_mesh_grid (positive in free space, the mesher's mask), here
+ * with an fp32 FMA blend and decoder.  The hit is the first k >= 1 with m_{k-1}, m_k, s_{k-1} > 0 and s_k <= 0; at most
+ * refine_iters bisection steps follow, t_mid = 0.5 (t_a + t_b), ending early when t_mid is not strictly inside the bracket
+ * or x(t_mid) is masked; out_t[i] = t_a + (t_b - t_a) (s_a / (s_a - s_b)) over the final bracket, the hit distance in
+ * scaled units, and out_status[i] = 1.  A miss: out_t[i] = NaN, out_status[i] = 0.  Samples whose cell at the coarsest
+ * featured level holds no node are skipped, with the same result as a march over every sample.  One thread per ray, no
+ * atomics: two launches on the same inputs give the same bits.  n < 0, NULL buffers (n > 0), a non-finite origin, h not
+ * finite and > 0, a non-finite t_min, t_max <= t_min, beyond < 0 or not finite, refine_iters outside
+ * [0, SHINE_RAYCAST_MAX_REFINE] and mask_level outside [0, num_levels) are SHINE_ERR_INVALID_ARG; a decoder other than
+ * 8 -> 32 -> 32 -> 1 is SHINE_ERR_UNSUPPORTED; none of them launches. */
+#define SHINE_RAYCAST_MAX_REFINE 32
+int shine_raycast(const shine_octree* oct, const shine_decoder* dec, const float* origin, const float* points, int64_t n,
+                  float h, float t_min, float beyond, float t_max, int32_t refine_iters, int32_t mask_level,
+                  float* out_t, uint8_t* out_status, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

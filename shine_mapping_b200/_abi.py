@@ -26,6 +26,7 @@ FLAG_LOSS_L1 = 64
 ERR_CAPACITY = -3
 REGISTER_OUT = 29
 REGISTER_SCRATCH_BYTES = 1024 * REGISTER_OUT * 8
+RAYCAST_MAX_REFINE = 32
 
 
 class ShineLevel(C.Structure):
@@ -193,6 +194,8 @@ SYMBOLS = {
     "shine_register_scratch_bytes": (C.c_int64, [_i64, _i64]),
     "shine_register_normal_eq_poses": (C.c_int, [_OCT, _DEC, _vp, _i64, C.POINTER(C.c_double), _i64, _f32, C.c_double,
                                                  _vp, _vp, _i64, _vp]),
+    "shine_raycast": (C.c_int, [_OCT, _DEC, C.POINTER(_f32), _vp, _i64, _f32, _f32, _f32, _f32, _i32, _i32, _vp, _vp,
+                                _vp]),
 }
 
 _lib = None

@@ -6,6 +6,7 @@
                          clouds, nearest neighbours in both directions with the reference's truncation rules.
 * `crop_intersection`  — the ground-truth points near every one of several meshes, written as an fp64 PLY point cloud.
 * `python -m shine_mapping_b200.evaluate PRED GT [...]` / `... crop GT PRED [PRED ...] --out FILE` — the CLI.
+* `... scans CONFIG CHECKPOINT [...]` — a saved map against held-out scans (raycast.py, DESIGN.md §13).
 
 Sampling and nearest neighbours are csrc/shine_eval.cu; the down-sampling is csrc/shine_scan.cu's voxel_down_sample.
 DESIGN.md §9 states the rules and where this differs from the reference.
@@ -15,6 +16,7 @@ from __future__ import annotations
 import argparse
 import csv
 import ctypes as C
+import math
 import os
 import sys
 
@@ -271,9 +273,51 @@ def _crop_parser():
     return ap
 
 
+def _scans_parser():
+    from .rgbd import add_loop_arguments
+    ap = argparse.ArgumentParser(prog="python -m shine_mapping_b200.evaluate scans",
+                                 description="Cast the rays of held-out scans through a saved map and report range errors. "
+                                             "The checkpoint is unpickled: load only files you trust.")
+    ap.add_argument("config")
+    ap.add_argument("checkpoint")
+    add_loop_arguments(ap)
+    ap.set_defaults(scans=False)
+    ap.add_argument("--frames", default=None, metavar="START:STOP[:STEP]",
+                    help="frames to evaluate (default: the ids in [begin_frame, end_frame] that mapping skips)")
+    ap.add_argument("--step-m", type=float, default=None, help="ray sample spacing, m (default: the config's mc_res_m)")
+    ap.add_argument("--beyond-m", type=float, default=1.0, help="search this far past each measured point, m")
+    ap.add_argument("--threshold", type=float, default=0.1, help="a hit within this of the measured range is an inlier, m")
+    ap.add_argument("--refine-iters", type=int, default=None, help="bisection steps of each hit (default 8)")
+    ap.add_argument("--csv", default=None, help="write one row per frame and a total row")
+    ap.add_argument("--points-dir", default=None, metavar="DIR", help="write each frame's hit points, DIR/{frame}.ply")
+    return ap
+
+
 def parse_args(argv):
-    """-> ("crop" | "eval", namespace); invalid values exit through argparse's error."""
+    """-> ("crop" | "scans" | "eval", namespace); invalid values exit through argparse's error."""
     argv = list(argv)
+    if argv and argv[0] == "scans":
+        from .raycast import REFINE_ITERS, parse_frames
+        from .rgbd import check_loop_arguments
+        ap = _scans_parser()
+        args = ap.parse_args(argv[1:])
+        check_loop_arguments(ap, args)
+        if args.frames is not None:
+            try:
+                args.frames = parse_frames(args.frames)
+            except ValueError as e:
+                ap.error(str(e))
+        for name in ("step_m", "threshold"):
+            v = getattr(args, name)
+            if v is not None and not (v > 0 and math.isfinite(v)):
+                ap.error(f"--{name.replace('_', '-')} must be > 0")
+        if not (args.beyond_m >= 0 and math.isfinite(args.beyond_m)):
+            ap.error("--beyond-m must be >= 0")
+        if args.refine_iters is None:
+            args.refine_iters = REFINE_ITERS
+        if not 0 <= args.refine_iters <= _abi.RAYCAST_MAX_REFINE:
+            ap.error(f"--refine-iters must be in [0, {_abi.RAYCAST_MAX_REFINE}]")
+        return "scans", args
     if argv and argv[0] == "crop":
         ap = _crop_parser()
         args = ap.parse_args(argv[1:])
@@ -303,8 +347,62 @@ def write_csv(path: str, metrics: dict) -> None:
         writer.writerow(metrics)
 
 
+def write_scans_csv(path: str, result: dict) -> None:
+    """eval_scans' result: a `frame` column and the metric columns, one row per frame and a `total` row."""
+    from .raycast import METRIC_COLUMNS
+    os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
+    with open(path, "w", newline="") as fh:
+        writer = csv.DictWriter(fh, fieldnames=["frame"] + METRIC_COLUMNS)
+        writer.writeheader()
+        for row in result["frames"]:
+            writer.writerow(row)
+        writer.writerow({"frame": "total", **result["total"]})
+
+
+def _format_metrics(m: dict) -> str:
+    return (f"rays {m['rays']}, hit ratio {m['hit_ratio']:.4f}, |err| mean {m['mean_abs_err_m']:.4f} m, median "
+            f"{m['median_abs_err_m']:.4f} m, rmse {m['rmse_m']:.4f} m, bias {m['bias_m']:+.4f} m, within threshold "
+            f"{m['within_threshold']:.4f}")
+
+
+def main_scans(args) -> int:
+    from .checkpoint import load_checkpoint
+    from .config import SHINEConfig
+    from .decoder import Decoder
+    from .raycast import eval_scans, held_out_frames, scan_frames
+    config = SHINEConfig()
+    config.load(args.config)
+    state, octree = load_checkpoint(args.checkpoint, config, config.device)
+    if octree is None or octree.is_empty():
+        raise SystemExit(f"{args.checkpoint}: the checkpoint holds a decoder but no map (feature_octree): nothing to cast "
+                         "rays through")
+    decoder = Decoder(config)
+    decoder.load_state_dict(state)
+    if args.rgbd:
+        from .rgbd import dataset_from_args
+        dataset = dataset_from_args(config, args)
+    else:
+        from .scans import LiDARDataset
+        dataset = LiDARDataset(config)
+    frames = list(args.frames) if args.frames is not None else held_out_frames(config, dataset.total_pc_count)
+    if not frames:
+        raise SystemExit(f"no held-out frames: every frame in [begin_frame {config.begin_frame}, end_frame "
+                         f"{config.end_frame}] was used for mapping (every_frame {config.every_frame}); choose frames "
+                         "with --frames START:STOP[:STEP]")
+    result = eval_scans(config, octree, decoder, scan_frames(dataset, frames), args.threshold, args.step_m,
+                        args.beyond_m, args.refine_iters, args.points_dir, np.linalg.inv(dataset.begin_pose_inv))
+    for row in result["frames"]:
+        print(f"frame {row['frame']}: {_format_metrics(row)}")
+    print(f"total: {_format_metrics(result['total'])}")
+    if args.csv:
+        write_scans_csv(args.csv, result)
+    return 0
+
+
 def main(argv=None) -> int:
     mode, args = parse_args(sys.argv[1:] if argv is None else argv)
+    if mode == "scans":
+        return main_scans(args)
     if mode == "crop":
         kept = crop_intersection(args.gt, args.pred, args.out, args.dist_thre, args.samples, args.seed)
         print(f"kept {kept.shape[0]} ground-truth points -> {args.out}")
