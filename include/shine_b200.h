@@ -599,6 +599,41 @@ int shine_raycast(const shine_octree* oct, const shine_decoder* dec, const float
                   float h, float t_min, float beyond, float t_max, int32_t refine_iters, int32_t mask_level,
                   float* out_t, uint8_t* out_status, void* stream);
 
+/* ---- rendering: depth, range and normal images of one camera view of the map (render.py) ----------------------------
+ * One ray per pixel (u, v), u = 0 .. width - 1 (column), v = 0 .. height - 1 (row), pixel i = v width + u.  fp32, every
+ * operation rounded on its own.  The camera-frame unit direction c:
+ *   SHINE_CAMERA_PINHOLE:     a = (u - cx) / fx,  b = (v - cy) / fy,  n = sqrt((a a + b b) + 1),  c = (a / n, b / n, 1 / n)
+ *                             (the pixel centre is (u, v), as shine_rgbd_backproject); depth = t c_z.
+ *   SHINE_CAMERA_RANGE_IMAGE: el = el0 - v del,  az = az0 - u daz  (fp32), with, in fp64 rounded once to fp32,
+ *                             el0 = fov_up pi / 180, del = (fov_up - fov_down) pi / 180 / (height - 1) (0 when height = 1),
+ *                             az0 = pi, daz = 2 pi / width: row 0 looks at fov_up, the last row at fov_down, column 0 at
+ *                             azimuth +pi and the azimuth falls with the column.  ce, se, ca, sa = cos and sin of el and az,
+ *                             each evaluated in fp64 and rounded to fp32; c = (ce ca, ce sa, se); depth = t.
+ * pose (host fp32 [12]) is the 3x4 camera-to-map transform, row-major, in scaled map coordinates: the ray's direction is
+ * d = R c, per row ((R0 c0 + R1 c1) + R2 c2), and its origin o the translation.  Along the ray the lattice and the march
+ * are shine_raycast's, with K = min(floor((t_max - t_min) / h), 2^24 - 1) for every pixel (no per-ray endpoint, no beyond).
+ * Outputs (device, NULL: not wanted): out_range [H W] = the hit distance t in scaled units, out_depth [H W] as above,
+ * out_normal [H W 3] = -g / |g| with g = dpred/dq at the hit point x = o + t d (fp32, shine_raycast's sample rounding): the
+ * gradient shine_register_normal_eq forms without sigma, back through the ReLU masks and the blend weights, so that
+ * n is the unit gradient of the march's field -Decoder.sdf (it faces free space); |n| = sqrt((gx gx + gy gy) + gz gz),
+ * then each component is -(g_a / |g|).  out_status [H W] = 1 on a hit.  A miss: NaN range, depth and normal, status 0.
+ * One thread per pixel, no atomics: two launches on the same inputs give the same bits.  NULL cam or pose, width or
+ * height <= 0, width height > 2^31, a non-finite pose entry, an unknown model, a pinhole with non-finite intrinsics or
+ * fx, fy <= 0, a range image with a non-finite FOV or fov_up <= fov_down, a non-finite t_max and shine_raycast's checks of
+ * h, t_min, t_max, refine_iters and mask_level are SHINE_ERR_INVALID_ARG; a decoder other than 8 -> 32 -> 32 -> 1 is
+ * SHINE_ERR_UNSUPPORTED; none of them launches.  No wanted output: SHINE_OK without a launch. */
+#define SHINE_CAMERA_PINHOLE 0
+#define SHINE_CAMERA_RANGE_IMAGE 1
+typedef struct shine_camera {
+    int32_t model;              /* SHINE_CAMERA_PINHOLE or SHINE_CAMERA_RANGE_IMAGE */
+    int32_t width, height;      /* pixels */
+    float fx, fy, cx, cy;       /* pinhole, pixels */
+    float fov_up, fov_down;     /* range image, degrees */
+} shine_camera;
+int shine_render(const shine_octree* oct, const shine_decoder* dec, const shine_camera* cam, const float* pose, float h,
+                 float t_min, float t_max, int32_t refine_iters, int32_t mask_level, float* out_range, float* out_depth,
+                 float* out_normal, uint8_t* out_status, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

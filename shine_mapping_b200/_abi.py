@@ -27,6 +27,8 @@ ERR_CAPACITY = -3
 REGISTER_OUT = 29
 REGISTER_SCRATCH_BYTES = 1024 * REGISTER_OUT * 8
 RAYCAST_MAX_REFINE = 32
+CAMERA_PINHOLE = 0
+CAMERA_RANGE_IMAGE = 1
 
 
 class ShineLevel(C.Structure):
@@ -100,6 +102,11 @@ class ShineBoundaryInverse(C.Structure):
 class ShineSamplePool(C.Structure):
     _fields_ = [("coord", C.c_void_p), ("label", C.c_void_p), ("weight", C.c_void_p), ("size", C.c_int64),
                 ("capacity", C.c_int64)]
+
+
+class ShineCamera(C.Structure):
+    _fields_ = [("model", C.c_int32), ("width", C.c_int32), ("height", C.c_int32), ("fx", C.c_float), ("fy", C.c_float),
+                ("cx", C.c_float), ("cy", C.c_float), ("fov_up", C.c_float), ("fov_down", C.c_float)]
 
 
 class ShineHostPool(C.Structure):
@@ -196,6 +203,8 @@ SYMBOLS = {
                                                  _vp, _vp, _i64, _vp]),
     "shine_raycast": (C.c_int, [_OCT, _DEC, C.POINTER(_f32), _vp, _i64, _f32, _f32, _f32, _f32, _i32, _i32, _vp, _vp,
                                 _vp]),
+    "shine_render": (C.c_int, [_OCT, _DEC, C.POINTER(ShineCamera), C.POINTER(_f32), _f32, _f32, _f32, _i32, _i32, _vp, _vp,
+                               _vp, _vp, _vp]),
 }
 
 _lib = None

@@ -260,6 +260,103 @@ __device__ __forceinline__ bool resolve_sector(const HashSlot* slots, uint32_t m
     return false;
 }
 
+// pred = Decoder.sdf(f(q)) and its input gradient dpred/dq at q = (x, y, z), fp32 (shine_register.cu's normal equations,
+// shine_render's normals):
+//     f = sum_c w_c F_c,  J = df/dq = sum_c F_c (x) grad w_c         (one gather over the 8 x L corner rows)
+//     pred as fp32 FMA chains (decoder in shared memory), masks D1, D2 of the two ReLUs
+//     dq = W1^T D1 W2^T D2 w3 = dpred/df,  grad = J^T dq
+// Returns whether q's voxel exists at lv[0].  With kNeedLeaf, a q without it returns false right after the gather, and
+// pred and grad are not formed.  S holds W1 [32][8], W2 [32][32] (W2[j][n]), its transpose W2T, b1, b2, w3 and b3.
+template <bool kNeedLeaf, class S>
+__device__ __forceinline__ bool sdf_grad_at(const shine_octree& oct, const S& sm, float x, float y, float z, float& pred,
+                                            float (&grad)[3]) {
+    const bool poly = oct.poly_interp != 0;
+    const int L = oct.num_levels;
+    float f[8], J[8][3];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) { f[k] = 0.f; J[k][0] = J[k][1] = J[k][2] = 0.f; }
+    bool valid = false;
+#pragma unroll 1
+    for (int i = 0; i < L; ++i) {
+        const shine_level& lv = oct.lv[i];
+        const HashSlot* slots = reinterpret_cast<const HashSlot*>(lv.hash_slots);
+        const int s = probe_slot(slots, lv.hash_capacity - 1, morton_of(x, y, z, lv.level));
+        if (s < 0) continue;
+        if (i == 0) valid = true;
+        const int4 ia = ldg_i4(slots[s].ids0), ib = ldg_i4(slots[s].ids1);
+        const int ids[8] = {ia.x, ib.x, ia.y, ib.y, ia.z, ib.z, ia.w, ib.w};
+        BlendD b; b.init(x, y, z, lv.level, poly);
+#pragma unroll
+        for (int c = 0; c < 8; ++c) {
+            float row[8];
+            ldg_row8(lv.features + (int64_t)ids[c] * kF, row);
+            const float X = (c & 4) ? b.t[0] : b.u[0], Y = (c & 2) ? b.t[1] : b.u[1], Z = (c & 1) ? b.t[2] : b.u[2];
+            const float w = __fmul_rn(__fmul_rn(X, Y), Z);
+            float dw[3]; b.dw(c, dw);
+#pragma unroll
+            for (int k = 0; k < 8; ++k) {
+                f[k] = fmaf(w, row[k], f[k]);
+                J[k][0] = fmaf(dw[0], row[k], J[k][0]); J[k][1] = fmaf(dw[1], row[k], J[k][1]);
+                J[k][2] = fmaf(dw[2], row[k], J[k][2]);
+            }
+        }
+    }
+    if (kNeedLeaf && !valid) return false;
+
+    // Decoder.sdf forward (model/decoder.py:49-63), fp32 FMA chains
+    float h1[32];
+    uint32_t m1 = 0, m2 = 0;
+#pragma unroll
+    for (int n = 0; n < 32; ++n) {
+        const float4 wa = *reinterpret_cast<const float4*>(sm.W1 + n * 8), wb = *reinterpret_cast<const float4*>(sm.W1 + n * 8 + 4);
+        float a = sm.b1[n];
+        a = fmaf(wa.x, f[0], a); a = fmaf(wa.y, f[1], a); a = fmaf(wa.z, f[2], a); a = fmaf(wa.w, f[3], a);
+        a = fmaf(wb.x, f[4], a); a = fmaf(wb.y, f[5], a); a = fmaf(wb.z, f[6], a); a = fmaf(wb.w, f[7], a);
+        m1 |= (a > 0.f ? 1u : 0u) << n;
+        h1[n] = fmaxf(a, 0.f);
+    }
+    float pr = sm.b3;
+#pragma unroll 1
+    for (int j = 0; j < 32; ++j) {
+        float a = sm.b2[j];
+#pragma unroll
+        for (int n = 0; n < 32; n += 4) {
+            const float4 w = *reinterpret_cast<const float4*>(sm.W2 + j * 32 + n);
+            a = fmaf(w.x, h1[n], a); a = fmaf(w.y, h1[n + 1], a); a = fmaf(w.z, h1[n + 2], a); a = fmaf(w.w, h1[n + 3], a);
+        }
+        m2 |= (a > 0.f ? 1u : 0u) << j;
+        pr = fmaf(fmaxf(a, 0.f), sm.w3[j], pr);
+    }
+
+    // dq = W1^T D1 W2^T D2 w3 = dpred/df, grad = J^T dq
+    float dq[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+#pragma unroll 1
+    for (int n = 0; n < 32; ++n) {
+        if (!((m1 >> n) & 1u)) continue;
+        float a = 0.f;
+#pragma unroll
+        for (int j = 0; j < 32; j += 4) {
+            const float4 w = *reinterpret_cast<const float4*>(sm.W2T + n * 32 + j);
+            a = fmaf(w.x, ((m2 >> j) & 1u) ? sm.w3[j] : 0.f, a);
+            a = fmaf(w.y, ((m2 >> (j + 1)) & 1u) ? sm.w3[j + 1] : 0.f, a);
+            a = fmaf(w.z, ((m2 >> (j + 2)) & 1u) ? sm.w3[j + 2] : 0.f, a);
+            a = fmaf(w.w, ((m2 >> (j + 3)) & 1u) ? sm.w3[j + 3] : 0.f, a);
+        }
+        const float4 wa = *reinterpret_cast<const float4*>(sm.W1 + n * 8), wb = *reinterpret_cast<const float4*>(sm.W1 + n * 8 + 4);
+        dq[0] = fmaf(a, wa.x, dq[0]); dq[1] = fmaf(a, wa.y, dq[1]); dq[2] = fmaf(a, wa.z, dq[2]); dq[3] = fmaf(a, wa.w, dq[3]);
+        dq[4] = fmaf(a, wb.x, dq[4]); dq[5] = fmaf(a, wb.y, dq[5]); dq[6] = fmaf(a, wb.z, dq[6]); dq[7] = fmaf(a, wb.w, dq[7]);
+    }
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+        float s = 0.f;
+#pragma unroll
+        for (int k = 0; k < 8; ++k) s = fmaf(J[k][a], dq[k], s);
+        grad[a] = s;
+    }
+    pred = pr;
+    return valid;
+}
+
 // ------------------------------------------------------------------------------------------------------
 // tensor-core helpers: mma.sync m16n8k8 TF32, fp32 accumulate, optional 3xTF32 error compensation
 // ------------------------------------------------------------------------------------------------------

@@ -72,8 +72,6 @@ __global__ void __launch_bounds__(kRT) register_normal_eq_kernel(const __grid_co
     if (tid == 0) sm.b3 = P.dec.b3 ? P.dec.b3[0] : 0.f;
     __syncthreads();
 
-    const bool poly = P.oct.poly_interp != 0;
-    const int L = P.oct.num_levels;
     const RegPose& T = P.pose[blockIdx.y];
     double acc[kOut];
 #pragma unroll
@@ -88,89 +86,12 @@ __global__ void __launch_bounds__(kRT) register_normal_eq_kernel(const __grid_co
                                         __fmul_rn(T.R[3 * a + 2], pz)), T.t[a]);
         const float x = qv[0], y = qv[1], z = qv[2];
 
-        // ---- gather: f and J = df/dq over the 8 x L corner rows; valid = a hit at lv[0] ---------------------------------
-        float f[8], J[8][3];
-#pragma unroll
-        for (int k = 0; k < 8; ++k) { f[k] = 0.f; J[k][0] = J[k][1] = J[k][2] = 0.f; }
-        bool valid = false;
-#pragma unroll 1
-        for (int i = 0; i < L; ++i) {
-            const shine_level& lv = P.oct.lv[i];
-            const HashSlot* slots = reinterpret_cast<const HashSlot*>(lv.hash_slots);
-            const int s = probe_slot(slots, lv.hash_capacity - 1, morton_of(x, y, z, lv.level));
-            if (s < 0) continue;
-            if (i == 0) valid = true;
-            const int4 ia = ldg_i4(slots[s].ids0), ib = ldg_i4(slots[s].ids1);
-            const int ids[8] = {ia.x, ib.x, ia.y, ib.y, ia.z, ib.z, ia.w, ib.w};
-            BlendD b; b.init(x, y, z, lv.level, poly);
-#pragma unroll
-            for (int c = 0; c < 8; ++c) {
-                float row[8];
-                ldg_row8(lv.features + (int64_t)ids[c] * kF, row);
-                const float X = (c & 4) ? b.t[0] : b.u[0], Y = (c & 2) ? b.t[1] : b.u[1], Z = (c & 1) ? b.t[2] : b.u[2];
-                const float w = __fmul_rn(__fmul_rn(X, Y), Z);
-                float dw[3]; b.dw(c, dw);
-#pragma unroll
-                for (int k = 0; k < 8; ++k) {
-                    f[k] = fmaf(w, row[k], f[k]);
-                    J[k][0] = fmaf(dw[0], row[k], J[k][0]); J[k][1] = fmaf(dw[1], row[k], J[k][1]);
-                    J[k][2] = fmaf(dw[2], row[k], J[k][2]);
-                }
-            }
-        }
-        if (!valid) continue;                // masked: contributes nothing (also to the count)
-
-        // ---- Decoder.sdf forward (model/decoder.py:49-63), fp32 FMA chains ---------------------------------------------------
-        float h1[32];
-        uint32_t m1 = 0, m2 = 0;
-#pragma unroll
-        for (int n = 0; n < 32; ++n) {
-            const float4 wa = *reinterpret_cast<const float4*>(sm.W1 + n * 8), wb = *reinterpret_cast<const float4*>(sm.W1 + n * 8 + 4);
-            float a = sm.b1[n];
-            a = fmaf(wa.x, f[0], a); a = fmaf(wa.y, f[1], a); a = fmaf(wa.z, f[2], a); a = fmaf(wa.w, f[3], a);
-            a = fmaf(wb.x, f[4], a); a = fmaf(wb.y, f[5], a); a = fmaf(wb.z, f[6], a); a = fmaf(wb.w, f[7], a);
-            m1 |= (a > 0.f ? 1u : 0u) << n;
-            h1[n] = fmaxf(a, 0.f);
-        }
-        float pr = sm.b3;
-#pragma unroll 1
-        for (int j = 0; j < 32; ++j) {
-            float a = sm.b2[j];
-#pragma unroll
-            for (int n = 0; n < 32; n += 4) {
-                const float4 w = *reinterpret_cast<const float4*>(sm.W2 + j * 32 + n);
-                a = fmaf(w.x, h1[n], a); a = fmaf(w.y, h1[n + 1], a); a = fmaf(w.z, h1[n + 2], a); a = fmaf(w.w, h1[n + 3], a);
-            }
-            m2 |= (a > 0.f ? 1u : 0u) << j;
-            pr = fmaf(fmaxf(a, 0.f), sm.w3[j], pr);
-        }
-
-        // ---- dq = W1^T D1 W2^T D2 w3 = dpred/df, g = sigma J^T dq ------------------------------------------------------------
-        float dq[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-#pragma unroll 1
-        for (int n = 0; n < 32; ++n) {
-            if (!((m1 >> n) & 1u)) continue;
-            float a = 0.f;
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-                const float4 w = *reinterpret_cast<const float4*>(sm.W2T + n * 32 + j);
-                a = fmaf(w.x, ((m2 >> j) & 1u) ? sm.w3[j] : 0.f, a);
-                a = fmaf(w.y, ((m2 >> (j + 1)) & 1u) ? sm.w3[j + 1] : 0.f, a);
-                a = fmaf(w.z, ((m2 >> (j + 2)) & 1u) ? sm.w3[j + 2] : 0.f, a);
-                a = fmaf(w.w, ((m2 >> (j + 3)) & 1u) ? sm.w3[j + 3] : 0.f, a);
-            }
-            const float4 wa = *reinterpret_cast<const float4*>(sm.W1 + n * 8), wb = *reinterpret_cast<const float4*>(sm.W1 + n * 8 + 4);
-            dq[0] = fmaf(a, wa.x, dq[0]); dq[1] = fmaf(a, wa.y, dq[1]); dq[2] = fmaf(a, wa.z, dq[2]); dq[3] = fmaf(a, wa.w, dq[3]);
-            dq[4] = fmaf(a, wb.x, dq[4]); dq[5] = fmaf(a, wb.y, dq[5]); dq[6] = fmaf(a, wb.z, dq[6]); dq[7] = fmaf(a, wb.w, dq[7]);
-        }
+        // ---- pred and dpred/dq (shine_device.cuh sdf_grad_at); a q outside lv[0] contributes nothing (also to the count)
+        float pr, gs[3];
+        if (!sdf_grad_at<true>(P.oct, sm, x, y, z, pr, gs)) continue;
         float gv[3];
 #pragma unroll
-        for (int a = 0; a < 3; ++a) {
-            float s = 0.f;
-#pragma unroll
-            for (int k = 0; k < 8; ++k) s = fmaf(J[k][a], dq[k], s);
-            gv[a] = P.sigma * s;
-        }
+        for (int a = 0; a < 3; ++a) gv[a] = P.sigma * gs[a];
         const float r = P.sigma * pr;
 
         // ---- fp64 from here: Jr = [g, q x g], Geman-McClure weight, the point's share --------------------------------------

@@ -7,6 +7,8 @@
 * `crop_intersection`  — the ground-truth points near every one of several meshes, written as an fp64 PLY point cloud.
 * `python -m shine_mapping_b200.evaluate PRED GT [...]` / `... crop GT PRED [PRED ...] --out FILE` — the CLI.
 * `... scans CONFIG CHECKPOINT [...]` — a saved map against held-out scans (raycast.py, DESIGN.md §13).
+* `... depth CONFIG CHECKPOINT --rgbd DEPTH_DIR [...]` — depth images rendered from a saved map against the held-out
+                         frames' depth images, with the reference's `eval_depth` metrics (render.py, DESIGN.md §14).
 
 Sampling and nearest neighbours are csrc/shine_eval.cu; the down-sampling is csrc/shine_scan.cu's voxel_down_sample.
 DESIGN.md §9 states the rules and where this differs from the reference.
@@ -293,9 +295,46 @@ def _scans_parser():
     return ap
 
 
+def _depth_parser():
+    from .rgbd import add_loop_arguments
+    ap = argparse.ArgumentParser(prog="python -m shine_mapping_b200.evaluate depth",
+                                 description="Render depth images of a saved map at RGB-D frames' camera poses and score "
+                                             "them against the frames' depth images (eval_depth).  The checkpoint is "
+                                             "unpickled: load only files you trust.")
+    ap.add_argument("config")
+    ap.add_argument("checkpoint")
+    add_loop_arguments(ap)
+    ap.set_defaults(scans=False)
+    ap.add_argument("--frames", default=None, metavar="START:STOP[:STEP]",
+                    help="frames to evaluate (default: the ids in [begin_frame, end_frame] that mapping skips)")
+    ap.add_argument("--step-m", type=float, default=None, help="ray sample spacing, m (default: the config's mc_res_m)")
+    ap.add_argument("--max-range-m", type=float, default=10.0,
+                    help="ray length, m (default 10, the metrics' largest target depth)")
+    ap.add_argument("--csv", default=None, help="write one row per frame and a mean row")
+    ap.add_argument("--out", default=None, metavar="DIR",
+                    help="write the rendered DIR/depth/{frame}.png and DIR/normal/{frame}.png")
+    return ap
+
+
 def parse_args(argv):
-    """-> ("crop" | "scans" | "eval", namespace); invalid values exit through argparse's error."""
+    """-> ("crop" | "scans" | "depth" | "eval", namespace); invalid values exit through argparse's error."""
     argv = list(argv)
+    if argv and argv[0] == "depth":
+        from .raycast import parse_frames
+        from .render import check_view_arguments
+        ap = _depth_parser()
+        args = ap.parse_args(argv[1:])
+        if args.rgbd is None:
+            ap.error("depth evaluation needs RGB-D frames: give --rgbd DEPTH_DIR and --pose-file")
+        from .rgbd import check_loop_arguments
+        check_loop_arguments(ap, args)
+        check_view_arguments(ap, args)
+        if args.frames is not None:
+            try:
+                args.frames = parse_frames(args.frames)
+            except ValueError as e:
+                ap.error(str(e))
+        return "depth", args
     if argv and argv[0] == "scans":
         from .raycast import REFINE_ITERS, parse_frames
         from .rgbd import check_loop_arguments
@@ -365,11 +404,11 @@ def _format_metrics(m: dict) -> str:
             f"{m['within_threshold']:.4f}")
 
 
-def main_scans(args) -> int:
+def load_map_and_dataset(args):
+    """args.config, args.checkpoint and the loops' --rgbd options -> (config, octree, decoder, dataset)."""
     from .checkpoint import load_checkpoint
     from .config import SHINEConfig
     from .decoder import Decoder
-    from .raycast import eval_scans, held_out_frames, scan_frames
     config = SHINEConfig()
     config.load(args.config)
     state, octree = load_checkpoint(args.checkpoint, config, config.device)
@@ -384,11 +423,24 @@ def main_scans(args) -> int:
     else:
         from .scans import LiDARDataset
         dataset = LiDARDataset(config)
-    frames = list(args.frames) if args.frames is not None else held_out_frames(config, dataset.total_pc_count)
+    return config, octree, decoder, dataset
+
+
+def selected_frames(config, dataset, frames) -> list:
+    """--frames, or by default the held-out frames (`raycast.held_out_frames`); none is an error."""
+    from .raycast import held_out_frames
+    frames = list(frames) if frames is not None else held_out_frames(config, dataset.total_pc_count)
     if not frames:
         raise SystemExit(f"no held-out frames: every frame in [begin_frame {config.begin_frame}, end_frame "
                          f"{config.end_frame}] was used for mapping (every_frame {config.every_frame}); choose frames "
                          "with --frames START:STOP[:STEP]")
+    return frames
+
+
+def main_scans(args) -> int:
+    from .raycast import eval_scans, scan_frames
+    config, octree, decoder, dataset = load_map_and_dataset(args)
+    frames = selected_frames(config, dataset, args.frames)
     result = eval_scans(config, octree, decoder, scan_frames(dataset, frames), args.threshold, args.step_m,
                         args.beyond_m, args.refine_iters, args.points_dir, np.linalg.inv(dataset.begin_pose_inv))
     for row in result["frames"]:
@@ -399,10 +451,56 @@ def main_scans(args) -> int:
     return 0
 
 
+def write_depth_csv(path: str, rows: list, mean: dict) -> None:
+    """eval_depth's metrics: a `frame` column, one row per frame and a `mean` row."""
+    from .render import DEPTH_METRICS
+    os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
+    with open(path, "w", newline="") as fh:
+        writer = csv.DictWriter(fh, fieldnames=["frame"] + DEPTH_METRICS)
+        writer.writeheader()
+        for row in rows:
+            writer.writerow(row)
+        writer.writerow({"frame": "mean", **mean})
+
+
+def _format_depth(m: dict) -> str:
+    return ", ".join(f"{k} {m[k]:.4f}" for k in m if k != "frame")
+
+
+def main_depth(args) -> int:
+    from .raycast import map_pose
+    from .render import DEPTH_METRICS, depth_metrics, render_view, write_view
+    from .rgbd import read_depth
+    config, octree, decoder, dataset = load_map_and_dataset(args)
+    frames = selected_frames(config, dataset, args.frames)
+    cam = dataset.camera
+    rows = []
+    for f in frames:
+        if not 0 <= f < dataset.total_pc_count:
+            raise SystemExit(f"frame {f}: the sequence has frames 0 .. {dataset.total_pc_count - 1}")
+        raw = read_depth(os.path.join(dataset.depth_dir, dataset.depth_filenames[f]))
+        if tuple(raw.shape) != (cam.height, cam.width):
+            raise SystemExit(f"frame {f}: the depth image is {raw.shape[1]} x {raw.shape[0]}, the camera "
+                             f"{cam.width} x {cam.height}")
+        target = torch.from_numpy(raw.numpy().astype(np.float64) / cam.depth_scale).to(dataset.device)
+        view = render_view(config, octree, decoder, map_pose(dataset, f), cam, args.max_range_m, args.step_m)
+        rows.append({"frame": f, **depth_metrics(view["depth"], target)})
+        if args.out:
+            write_view(args.out, f, view, cam.depth_scale)
+        print(f"frame {f}: {_format_depth(rows[-1])}")
+    mean = {k: float(np.mean([r[k] for r in rows])) for k in DEPTH_METRICS}
+    print(f"mean: {_format_depth(mean)}")
+    if args.csv:
+        write_depth_csv(args.csv, rows, mean)
+    return 0
+
+
 def main(argv=None) -> int:
     mode, args = parse_args(sys.argv[1:] if argv is None else argv)
     if mode == "scans":
         return main_scans(args)
+    if mode == "depth":
+        return main_depth(args)
     if mode == "crop":
         kept = crop_intersection(args.gt, args.pred, args.out, args.dist_thre, args.samples, args.seed)
         print(f"kept {kept.shape[0]} ground-truth points -> {args.out}")
