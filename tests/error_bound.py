@@ -42,10 +42,11 @@ def blend(o, coord):
 
 
 def abs_feature(o, coord):
+    """sum over levels and corners of |w| |row| (a coordinate outside [-1, 1] can have a negative blend weight)"""
     total = torch.zeros(coord.shape[0], o.feature_dim, dtype=torch.float64)
     for i, (ix, w) in enumerate(blend(o, coord)):
         t = o.hier_features[o.featured_level_num - 1 - i].detach().abs()
-        total += (t[ix] * w[:, None]).reshape(coord.shape[0], 8, -1).sum(1)
+        total += (t[ix] * w.abs()[:, None]).reshape(coord.shape[0], 8, -1).sum(1)
     return total
 
 

@@ -16,6 +16,7 @@ import numpy as np
 import pytest
 import torch
 
+from tests import hash_layout as hl
 from tests.parity_utils import make_config, orc
 
 pytestmark = pytest.mark.gpu
@@ -32,42 +33,10 @@ def _lib(built_lib):
 # host restatements of the device table layout (csrc/shine_device.cuh, csrc/shine_octree_build.cu)
 # ------------------------------------------------------------------------------------------------------------------
 
-_EMPTY = np.uint64(0xFFFFFFFFFFFFFFFF)
-
-
-def _hash_key(k: np.ndarray) -> np.ndarray:
-    """hash_key of shine_device.cuh in uint64 arithmetic (wraps like the device's)."""
-    k = k.astype(np.uint64)
-    k = k ^ (k >> np.uint64(31))
-    k = k * np.uint64(0x9E3779B97F4A7C15)
-    k = k ^ (k >> np.uint64(29))
-    k = k * np.uint64(0xBF58476D1CE4E5B9)
-    k = k ^ (k >> np.uint64(32))
-    return (k & np.uint64(0xFFFFFFFF)).astype(np.int64)
-
-
-def _probe_pos(h0, it, mask):
-    """probe_pos of shine_device.cuh, vectorised over h0 / it."""
-    return np.where(it == 0, h0, np.where(it == 1, h0 ^ 1, ((h0 & ~1) + it) & mask))
-
-
-def _probe_index(h0, s, mask):
-    """inverse of _probe_pos: the probe index at which a key of home h0 sits in slot s"""
-    return np.where(s == h0, 0, np.where(s == (h0 ^ 1), 1, (s - (h0 & ~1)) & mask))
-
-
 def _lex_key(xyz: np.ndarray) -> np.ndarray:
     """lexicographic corner key of shine_octree_build.cu (16 bits per axis, int16 order)"""
     c = xyz.astype(np.int64) & 0xFFFF ^ 0x8000
     return (c[..., 0] << 32) | (c[..., 1] << 16) | c[..., 2]
-
-
-def _decode_node_slots(st):
-    raw = st.hash.cpu().numpy().reshape(st.hash_capacity, 64)
-    return dict(key=raw[:, 0:8].copy().view(np.uint64)[:, 0], node=raw[:, 8:12].copy().view(np.int32)[:, 0],
-                maxdisp=raw[:, 12:16].copy().view(np.int32)[:, 0], ids0=raw[:, 16:32].copy().view(np.int32),
-                key2=raw[:, 32:40].copy().view(np.uint64)[:, 0], maxdisp2=raw[:, 44:48].copy().view(np.int32)[:, 0],
-                ids1=raw[:, 48:64].copy().view(np.int32))
 
 
 def check_device_tables(octree):
@@ -80,31 +49,8 @@ def check_device_tables(octree):
         keys = st.node_keys.cpu().numpy()
         node_ids = st.node_ids.cpu().numpy()
         n, cap = keys.size, st.hash_capacity
-        assert np.unique(keys).size == n
-        mask = cap - 1
-        s = _decode_node_slots(st)
-        occupied = np.flatnonzero(s["key"] != _EMPTY)
-        assert occupied.size == n, (lvl, occupied.size, n)
         assert n < cap and n * spn <= 2 * cap, (lvl, n, cap, spn)           # one empty slot at least, load <= 2/spn
-        slot_keys = s["key"][occupied].astype(np.int64)
-        order = np.argsort(slot_keys)
-        assert np.array_equal(slot_keys[order], np.sort(keys)), f"level {lvl}: slot keys != node_keys"
-        assert np.array_equal(s["key2"][occupied], s["key"][occupied])
-        assert np.array_equal(s["maxdisp"], s["maxdisp2"])
-        slot_of = occupied[order]                                              # slot of the i-th smallest key
-        idx = np.argsort(keys)                                                 # node index of the i-th smallest key
-        slot = np.empty(n, dtype=np.int64)
-        slot[idx] = slot_of
-        assert np.array_equal(s["node"][slot], np.arange(n)), f"level {lvl}: slot ordinal != index in node_keys"
-        assert np.array_equal(s["ids0"][slot], node_ids[:, 0::2])
-        assert np.array_equal(s["ids1"][slot], node_ids[:, 1::2])
-        h0 = _hash_key(keys) & mask
-        it = _probe_index(h0, slot, mask)
-        far = it > 0
-        assert np.all(it[far] <= s["maxdisp"][h0[far]]), f"level {lvl}: key beyond its home's maxdisp"
-        for j in np.flatnonzero(far):                                          # no empty slot before the key on its walk
-            walk = _probe_pos(np.full(it[j], h0[j]), np.arange(it[j]), mask)
-            assert np.all(s["key"][walk] != _EMPTY)
+        hl.check_slots(hl.Slots.decode(st.hash.cpu().numpy()), keys, node_ids, f"level {lvl}")
         # corner table: {lexicographic key, row}, every row once.  Only update() on the GPU builds it (rebuilt there after
         # a move), so a level grown on the CPU path has none until the next GPU frame.
         if st.corner_hash is None:
@@ -120,7 +66,7 @@ def check_device_tables(octree):
         assert np.array_equal(np.sort(got_rows), np.arange(rows))
         assert np.array_equal(ct[used, 0], want[got_rows]), f"level {lvl}: corner slot key != its row's corner"
         # linear probing from the home slot: no empty slot between a key's home and its slot
-        home = _hash_key(ct[used, 0].astype(np.uint64)) & (ccap - 1)
+        home = hl.hash_key(ct[used, 0].astype(np.uint64)) & (ccap - 1)
         empties = np.concatenate(([0], np.cumsum(np.tile(ct[:, 0] == -1, 2))))
         dist = (used - home) & (ccap - 1)
         assert np.all(empties[home + dist] == empties[home]), f"level {lvl}: corner key unreachable from its home slot"
