@@ -4,9 +4,11 @@ tests).  The reference has no multi-GPU code (SURVEY.md §2.2) — this is new d
 * "replicated": tables replicated, the POINT BATCH is sharded (`shard_range`); every per-point gradient already
   carries 1/N_global, so one sum all-reduce of the flat gradient buffer (tables + 1 377 decoder floats) yields
   exactly the single-GPU gradient of the global batch.
-* "spatial" (BASELINE config 5): every rank owns a spatial octree block and the samples that fall inside it; table
-  rows are private to their owner, only the decoder segment is all-reduced.  (Rows on shared block faces would
-  need a boundary exchange; blocks used here are disjoint — see DESIGN.md.)
+* "spatial" (BASELINE config 5): every rank owns a Morton-prefix range of ONE map and the samples that fall inside it.
+  Corner rows on the faces between ranges exist on every rank that holds a node touching them (`partition.BoundaryPlan`);
+  every step their gradients travel with the decoder gradients in ONE exchange ([decoder | boundary rows]: pack ->
+  all-reduce -> unpack through `NcclComm`, or the one-kernel peer-memory `P2PExchange`), which sums them in a fixed rank
+  order so that the duplicates stay bit-identical.  The other rows are private to their rank (DESIGN.md §6).
 """
 from __future__ import annotations
 
@@ -106,12 +108,16 @@ class P2PExchange:
         """In place: dec_flat and the plan's rows of table_grads become the sums over all ranks."""
         C = self._C
         if plan is not None and plan.total_floats > plan.dec_floats:
-            key = tuple(t.data_ptr() for t in table_grads)
+            # the descriptors point at the plan's index tensors and at the tables: rebuilt when either changes (another
+            # plan, a plan moved by .to(), tables re-allocated by octree.update)
+            key = (tuple(t.data_ptr() for t in table_grads),
+                   tuple(t.data_ptr() for ts in (plan.rows, plan.slots, plan.inverse, plan.holders) for t in ts))
             cached = getattr(self, "_desc", None)
-            if cached is None or cached[0] != key:          # building the ctypes structs costs tens of us of Python
-                cached = (key, plan.descriptor(table_grads), plan.inverse_descriptor(), len(table_grads), plan.feature_dim)
+            if cached is None or cached[0] != key or cached[-1] is not plan:   # building the ctypes structs costs tens of us
+                cached = (key, plan.descriptor(table_grads), plan.inverse_descriptor(), len(table_grads), plan.feature_dim,
+                          plan)
                 self._desc = cached
-            _, desc, inv, levels, fdim = cached
+            _, desc, inv, levels, fdim, _ = cached
             arg, iarg = C.byref(desc), C.byref(inv)
         else:
             arg, iarg, levels, fdim = None, None, 0, 8

@@ -36,6 +36,18 @@ def global_oracle_step(cfg, pool, batch, dec):
     return o, key_to_row, res
 
 
+def global_case(cfg, o, batch, dec):
+    """The global batch as a case of tests/parity_utils (the oracle octree `o` reused, unweighted, mean), for the fp64
+    reference `tests.test_gpu_replicas.Ref` and the bound of tests/boundary_oracle.py."""
+    n = batch[0].shape[0]
+    return {"cfg": dict(tree_level_world=cfg.tree_level_world, tree_level_feat=cfg.tree_level_feat,
+                        feature_dim=cfg.feature_dim, poly_int_on=cfg.poly_int_on, leaf_vox_size=cfg.leaf_vox_size,
+                        sigma=float(cfg.sigma_sigmoid), weighted=False, reduction="mean", bias=True),
+            "frames": [], "oracle": o, "tables": [t.detach().numpy().copy() for t in o.hier_features],
+            "dec": {k: v.detach().numpy().copy() for k, v in dec.items()},
+            "coord": batch[0].numpy().copy(), "label": batch[1].numpy().copy(), "weight": np.ones(n, dtype=np.float32)}
+
+
 def rows_in_global(corner_keys: torch.Tensor, key_to_row: dict) -> np.ndarray:
     return np.array([key_to_row[int(k)] for k in corner_keys.tolist()], dtype=np.int64)
 

@@ -9,7 +9,7 @@ import pytest
 import torch
 
 from tests.parity_utils import DEC_KEYS
-from tests.partition_utils import check_rank_against_global, global_oracle_step, global_scene
+from tests.partition_utils import check_rank_against_global, global_case, global_oracle_step, global_scene
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -109,6 +109,33 @@ def _free_port():
         return s.getsockname()[1]
 
 
+def _grade_exchanged(tr, plan, loss, pb, ref, case, sizes, what):
+    """Every table element of this rank and the decoder gradients against the bound of a partitioned step
+    (tests/boundary_oracle.py), the summed loss against its own, and the exchange's result bitwise equal on every rank:
+    decoder segment and every shared corner's rows gathered from all ranks."""
+    import torch.distributed as dist
+    from tests.boundary_oracle import pack_host
+    from tests.test_gpu_replicas import dec_grads
+    torch.cuda.synchronize()
+    tables = [g.detach().cpu().numpy() for g in tr.table_grads]
+    pb.grade_rank(plan.rank, tables, what)
+    ref.dec.grade(dec_grads(tr), pb.decoder_depth(sizes, torch.cuda.get_device_properties(0).multi_processor_count), what)
+    pb.loss_ref(case).grade(loss, what)
+    mine = pack_host(plan, tables)
+    mine[:plan.dec_floats] = tr.dec_flat.detach().cpu().numpy()[:plan.dec_floats]
+    held = np.zeros(plan.total_floats, dtype=bool)
+    held[:plan.dec_floats] = True
+    for lvl, n in enumerate(plan.counts):
+        held[plan.offsets[lvl]:plan.offsets[lvl] + n * plan.feature_dim].reshape(-1, plan.feature_dim)[
+            plan.slots[lvl].cpu().numpy()] = True
+    everyone = [None] * dist.get_world_size()
+    dist.all_gather_object(everyone, (mine, held))
+    for r, (theirs, their_held) in enumerate(everyone):
+        both = held & their_held
+        bad = np.flatnonzero(mine[both].view(np.uint32) != theirs[both].view(np.uint32))
+        assert bad.size == 0, f"{what}: {bad.size} exchanged floats differ from rank {r}'s"
+
+
 def _nccl_worker(rank, world, port, out_dir):
     os.environ.update(RANK=str(rank), WORLD_SIZE=str(world), LOCAL_RANK=str(rank), MASTER_ADDR="127.0.0.1",
                       MASTER_PORT=str(port))
@@ -117,25 +144,39 @@ def _nccl_worker(rank, world, port, out_dir):
     from shine_mapping_b200.partition import BoundaryPlan, coarse_keys, gather_corner_keys, owner_of, partition_pool
     sdist.init_from_env("nccl")
     dev = f"cuda:{rank}"
+    from tests.boundary_oracle import PartitionBound, global_rows
+    from tests.test_gpu_replicas import Ref
     cfg0, pool, batch, dec = global_scene(levels=4, n_azimuth=128, n_frames=3, n_batch=20000)
     o_glob, key_to_row, res_glob = global_oracle_step(cfg0, pool, batch, dec)
     bounds, parts = partition_pool(*pool, cfg0, world)
     cfg, octree, decoder, keys = _build_rank(cfg0, parts[rank], dec, key_to_row, o_glob, dev, rank)
     comm = sdist.NcclComm(rank, world, torch.device(dev))
-    plan = BoundaryPlan(rank, gather_corner_keys(octree), cfg0.feature_dim, 1380).to(dev)
+    all_keys = gather_corner_keys(octree)
+    plan = BoundaryPlan(rank, all_keys, cfg0.feature_dim, 1380).to(dev)
     tr = SdfTrainer(cfg, octree, decoder, shard_mode="spatial", boundary=plan, comm=comm)
     tr.zero_grad()
-    m = owner_of(coarse_keys(batch[0], cfg0.tree_level_world - cfg0.tree_level_feat + 1), bounds) == rank
+    owner = owner_of(coarse_keys(batch[0], cfg0.tree_level_world - cfg0.tree_level_feat + 1), bounds)
+    m = owner == rank
+    # the fp64 step of the global batch and the bound of the per-point kernel on this split (kink points keep their
+    # envelope bound: the batch is the one the fp32 checks use)
+    case = global_case(cfg0, o_glob, batch, dec)
+    ref = Ref(case)
+    points = [np.flatnonzero(owner.numpy() == r) for r in range(world)]
+    rank_rows = [[global_rows(k, key_to_row[kk]) for kk, k in enumerate(ks)] for ks in all_keys]
+    pb = PartitionBound(ref, points, rank_rows, grouped=False)
+    sizes = [p.size for p in points]
     loss = tr.forward_backward(batch[0][m].to(dev), batch[1][m].to(dev), None, n_norm=batch[0].shape[0]).clone()
     tr.all_reduce_grads()                       # pack -> shine_allreduce_decoder_grads (NCCL, C ABI) -> unpack
     comm.all_reduce(loss.view(1))
     torch.cuda.synchronize()
     check_rank_against_global([g.detach().cpu().numpy() for g in tr.table_grads], keys, key_to_row, res_glob)
     _check_decoder_and_loss(tr, float(loss), res_glob)
+    _grade_exchanged(tr, plan, float(loss), pb, ref, case, sizes, f"NCCL rank {rank}")
     # second step through the pipelined host entry with the exchange inside
     h = tr.submit_host_step(batch[0][m].pin_memory(), batch[1][m].pin_memory(), n_norm=batch[0].shape[0], exchange=True)
     h.result()
     check_rank_against_global([g.detach().cpu().numpy() for g in tr.table_grads], keys, key_to_row, res_glob)
+    pb.grade_rank(rank, [g.detach().cpu().numpy() for g in tr.table_grads], f"NCCL host step rank {rank}")
     # the same exchange as ONE NVLink peer-memory kernel (IPC buffers + flags, no NCCL) — three steps in a row so that both
     # buffer parities and the flag hand-over between consecutive steps are exercised
     p2p = sdist.P2PExchange(rank, world, torch.device(dev), plan.total_floats)
@@ -148,6 +189,7 @@ def _nccl_worker(rank, world, port, out_dir):
         torch.cuda.synchronize()
         check_rank_against_global([g.detach().cpu().numpy() for g in tr2.table_grads], keys, key_to_row, res_glob)
         _check_decoder_and_loss(tr2, float(loss2), res_glob)
+        _grade_exchanged(tr2, plan, float(loss2), pb, ref, case, sizes, f"peer memory rank {rank}")
     # the whole step {zero, fused kernel, peer-memory exchange} captured as a CUDA graph and replayed: the exchange keeps
     # its step number on the device, so replays keep the protocol going (four replays: both buffer parities twice)
     cd, ld = batch[0][m].to(dev), batch[1][m].to(dev)
@@ -159,6 +201,7 @@ def _nccl_worker(rank, world, port, out_dir):
         loss3 = tr2.loss.detach().clone()
         comm.all_reduce(loss3.view(1))
         _check_decoder_and_loss(tr2, float(loss3), res_glob)
+        _grade_exchanged(tr2, plan, float(loss3), pb, ref, case, sizes, f"graph replay rank {rank}")
     assert p2p.timeouts() == 0
     open(os.path.join(out_dir, f"ok{rank}"), "w").write("ok")
     dist.barrier()
