@@ -64,17 +64,19 @@ def _scale(case):
 
 # ---- blend weights and their derivatives -----------------------------------------------------------------------------------
 
-def level_geometry(o, coord, exact=False):
+def level_geometry(o, coord, exact=False, levels=None):
     """Per level, bottom-up: dict(level, ix [N, 8] rows (-1: miss), w [N, 8], dw [N, 8, 3], edw [N, 8, 3]) as fp64 numpy.
     coord: fp32 array (exact=False: fp32 weights and factors, dt in fp64 from the fp32 fraction) or an fp64 array of
-    fp32-representable points (exact=True: everything in fp64, edw = 0).  The rows come from the fp32 coordinates."""
+    fp32-representable points (exact=True: everything in fp64, edw = 0).  The rows come from the fp32 coordinates.
+    levels: the world level of each bottom-up position when they are not max_level - i (an oracle of levels that are not
+    consecutive, whose get_indices and interpolat already use them)."""
     c32 = torch.from_numpy(np.asarray(coord, dtype=np.float32))
     idx = o.get_indices(c32)
     poly = o.polynomial_interpolation
     out = []
     for i in range(o.featured_level_num):
         level = o.max_level - i
-        res = 2.0 ** level
+        res = 2.0 ** (level if levels is None else levels[i])
         if exact:
             x = np.asarray(coord, dtype=np.float64)
             cc = res * (x * 0.5 + 0.5)
@@ -82,7 +84,7 @@ def level_geometry(o, coord, exact=False):
             t = 3 * d ** 2 - 2 * d ** 3 if poly else d
             u = 1 - t
         else:
-            cc = (2 ** level) * (c32 * 0.5 + 0.5)           # the oracle's interpolat, op for op
+            cc = res * (c32 * 0.5 + 0.5)                    # the oracle's interpolat, op for op
             d32 = torch.frac(cc)
             t32 = 3 * (d32 ** 2) - 2 * (d32 ** 3) if poly else d32
             d, t, u = d32.double().numpy(), t32.double().numpy(), (1 - t32).double().numpy()

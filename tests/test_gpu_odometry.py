@@ -12,6 +12,7 @@ from shine_mapping_b200 import odometry, synth
 from shine_mapping_b200.trainer import SdfTrainer
 from tests.eikonal_bound import EikRef
 from tests.error_bound import U, grade_values
+from tests.grad_field_bound import sum_depth
 from tests.parity_utils import build_cuda_models, dec_keys, make_case
 
 pytestmark = pytest.mark.gpu
@@ -70,8 +71,8 @@ class RegRef:
     """fp64 values of the 29 outputs and their bounds for points whose q (fp32) the kernel computes bit for bit.
     r = sigma pred with e_r = sigma P + u |r|; Jr = [g, q x g] with e_J = [e_g, |q| x e_g (crosswise)]; w = (k^2 / (k^2 +
     r^2))^2 with e_w = |w'(r)| e_r + 2 e_r^2 / k^2 (|w''| <= 4 / k^2); per point e(w a c) <= e_w |a c| + w (e_a |c| + |a| e_c)
-    (+ second-order terms); the fp64 products and sums add 8 (n + 8) 2^-53 of the sum of |terms|.  `mult` copies of every
-    point (the million-point launch tiles a smaller set)."""
+    (+ second-order terms); the fp64 products add 8 2^-53 and the sums (sum_depth(n) + 2) 2^-53 of the sum of |terms|
+    (tests/grad_field_bound.py).  `mult` copies of every point (the million-point launch tiles a smaller set)."""
 
     def __init__(self, case, q, kappa):
         n = q.shape[0]
@@ -108,7 +109,9 @@ class RegRef:
         bounds = np.concatenate((eH, eb, ec[:, None]), 1)
         total = int(m.sum()) * mult
         want = mult * terms.sum(0)
-        bound = mult * bounds.sum(0) + 8 * (total + 8) * E64 * mult * np.abs(terms).sum(0)
+        # the fp64 tail's own roundings (8 per share) and the kernel's summation depth (tests/grad_field_bound.py)
+        depth = sum_depth(int(keep.shape[0]) * mult) + 8 + 2
+        bound = mult * bounds.sum(0) + depth * E64 * mult * np.abs(terms).sum(0)
         return np.concatenate((want, [total])), np.concatenate((bound, [0.0]))
 
 
