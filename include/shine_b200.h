@@ -579,6 +579,26 @@ int shine_register_normal_eq_poses(const shine_octree* oct, const shine_decoder*
                                    const double* poses, int64_t num_poses, float sigma, double kappa, double* out,
                                    void* scratch, int64_t scratch_bytes, void* stream);
 
+/* The same normal equations for num_items items of many scans at once (scans localized in lock-step): points is one
+ * device fp32 [num_points, 3] array holding every scan, item k is the segment points[seg_begin[k] .. seg_begin[k] +
+ * seg_n[k]) at the pose poses[16 k ..] (host fp64, as above), and out (device fp64 [num_items, SHINE_REGISTER_OUT]) row k
+ * equals, bit for bit, shine_register_normal_eq(points + 3 seg_begin[k], seg_n[k], pose k): item k runs its own
+ * G_k = min(ceil(n_k / 256), SHINE_REGISTER_MAX_BLOCKS) blocks with its own grid-stride, its partials sit at its own
+ * prefix offset of the scratch and its fold adds them in block order.  Items may share a segment; an empty segment gives
+ * a row of zeros.  seg_begin and seg_n are host int64 [num_items]; the items go to the device in the kernel parameters,
+ * at most SHINE_REGISTER_ITEMS_PER_LAUNCH per launch.  scratch (device, 8-byte aligned) holds
+ * shine_register_scans_scratch_bytes(seg_n, num_items) = sum_k G_k * SHINE_REGISTER_OUT * 8 bytes.  Everything
+ * shine_register_normal_eq_poses refuses (with num_points as n), a NULL seg_begin or seg_n, a negative seg_n[k] or
+ * seg_begin[k], and a segment reaching past num_points are SHINE_ERR_INVALID_ARG, before any launch.
+ * shine_register_scans_scratch_bytes returns -1 for a NULL seg_n, a negative entry, or num_items <= 0 or above
+ * INT32_MAX. */
+#define SHINE_REGISTER_ITEMS_PER_LAUNCH 384
+int64_t shine_register_scans_scratch_bytes(const int64_t* seg_n, int64_t num_items);
+int shine_register_normal_eq_scans(const shine_octree* oct, const shine_decoder* dec, const float* points,
+                                   int64_t num_points, const int64_t* seg_begin, const int64_t* seg_n,
+                                   const double* poses, int64_t num_items, float sigma, double kappa, double* out,
+                                   void* scratch, int64_t scratch_bytes, void* stream);
+
 /* ---- ray casting: where rays from one sensor origin first meet the map's zero level set (evaluate.py eval_scans) ----
  * Ray i goes from origin (host fp32 [3], scaled) towards points[i] (device fp32 [n,3], scaled, map frame).  fp32, every
  * operation rounded on its own: v = p - o, r = sqrt((vx vx + vy vy) + vz vz), d = v / r, and the lattice

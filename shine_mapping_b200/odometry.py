@@ -5,10 +5,12 @@ residuals of its points (scan-to-implicit-map odometry).  For a pose T and the s
 its Jacobian for a left-multiplied twist xi = (rho, phi) is [g_i, (T p_i) x g_i], g_i the SDF gradient.
 `shine_register_normal_eq` (csrc/shine_register.cu) forms the robust (Geman-McClure) normal equations of one iterate in
 one pass over the scan; the 6x6 system is solved here in fp64, one 29-double read per iteration.
-`shine_register_normal_eq_poses` forms them at many poses in one call (the coarse grid, the weak-direction search).
+`shine_register_normal_eq_poses` forms them at many poses in one call, and `shine_register_normal_eq_scans` for many
+scans at many poses: `register_scans` runs `register`'s policy for a whole sequence in lock-step (localization in a
+saved map, `localize.py`), one launch and one read per step for all of its scans.
 
 * `se3_exp` / `se3_log` — the SE(3) exponential and logarithm in fp64, twist (rho, phi).
-* `ScanToMapRegistration` — the normal equations and the Gauss-Newton loop.
+* `ScanToMapRegistration` — the normal equations and the Gauss-Newton loop, for one scan or many in lock-step.
 * `OdometryScans` — a frame source for `incre_loop.run_shine_mapping_incremental` that estimates each frame's pose.
 
 The map frame is the first scan's frame.  The loop trains the map frame by frame, so each scan is registered to the map
@@ -120,7 +122,7 @@ class ScanToMapRegistration:
     GRID_X = np.arange(-8, 9) * 0.25
     GRID_Y = np.arange(-2, 3) * 0.25
     GRID_YAW = np.radians(np.arange(-6, 7) * 1.0)
-    # launch_poses splits a batch of poses so that its block partials stay within this many bytes of scratch
+    # launch_poses and launch_items split a batch so that its block partials stay within this many bytes of scratch
     SCRATCH_BOUND_BYTES = 64 << 20
 
     def __init__(self, config: SHINEConfig, octree, decoder, kappa_m: float = 0.1, max_iters: int = 30,
@@ -186,6 +188,57 @@ class ScanToMapRegistration:
                 _abi.ptr(out[k0:k0 + kc]), _abi.ptr(self.scratch), self.scratch.numel(), _abi.stream_ptr(self.device)),
                 "shine_register_normal_eq_poses")
 
+    def launch_items(self, points: torch.Tensor, segments: np.ndarray, poses_scaled: np.ndarray, kappa_scaled: float,
+                     out: torch.Tensor) -> None:
+        """The normal equations of K items into out (fp64 [K,29]; no host read): item k is the scan
+        points[begin_k : begin_k + n_k] (segments int64 [K,2] of (begin, n); points fp32 [N,3] holds every scan) at pose
+        k (fp64 [K,4,4], translation in scaled units).  shine_register_normal_eq_scans, whose row k equals `launch` of
+        that segment at pose k bit for bit.  The items go in batches whose block partials fit SCRATCH_BOUND_BYTES.
+
+        When `launch` is overridden (a host-side restatement of the field), this calls it once per item instead."""
+        seg = np.ascontiguousarray(segments, dtype=np.int64).reshape(-1, 2)
+        poses = np.ascontiguousarray(poses_scaled, dtype=np.float64).reshape(-1, 16)
+        K = poses.shape[0]
+        if seg.shape[0] != K:
+            raise ValueError(f"launch_items: {seg.shape[0]} segments for {K} poses")
+        if out.dtype != torch.float64 or tuple(out.shape) != (K, _abi.REGISTER_OUT) or not out.is_contiguous():
+            raise ValueError(f"launch_items writes fp64 [{K}, {_abi.REGISTER_OUT}] rows: out is {out.dtype} "
+                             f"{tuple(out.shape)}{'' if out.is_contiguous() else ', not contiguous'}")
+        if K == 0:
+            return
+        if type(self).launch is not ScanToMapRegistration.launch:
+            for k in range(K):
+                b, n = int(seg[k, 0]), int(seg[k, 1])
+                self.launch(points[b:b + n], poses[k].reshape(4, 4), kappa_scaled, out[k])
+            return
+        _abi.require_cuda(points, "ScanToMapRegistration")
+        if out.device != points.device:
+            raise ValueError(f"launch_items: out is on {out.device}, the points on {points.device}")
+        points = points.float().contiguous()
+        lib = _abi.lib()
+        per_scan = {n: lib.shine_register_scratch_bytes(n, 1) for n in set(seg[:, 1].tolist())}
+        if min(per_scan.values()) < 0:
+            raise ValueError("launch_items: a segment of negative length")
+        begins = np.ascontiguousarray(seg[:, 0])
+        counts = np.ascontiguousarray(seg[:, 1])
+        od = self.octree._descriptor(None, None)
+        dd = self.decoder.c_descriptor(None)
+        i64p, f64p = C.POINTER(C.c_int64), C.POINTER(C.c_double)
+        k0 = 0
+        while k0 < K:                                   # the longest run of items whose partials fit the bound (>= 1)
+            k1, used = k0 + 1, per_scan[int(counts[k0])]
+            while k1 < K and used + per_scan[int(counts[k1])] <= self.SCRATCH_BOUND_BYTES:
+                used += per_scan[int(counts[k1])]
+                k1 += 1
+            if self.scratch.numel() < used:
+                self.scratch = torch.empty(used, dtype=torch.uint8, device=self.device)
+            _abi.check(lib.shine_register_normal_eq_scans(
+                C.byref(od), C.byref(dd), _abi.ptr(points), points.shape[0], begins[k0:].ctypes.data_as(i64p),
+                counts[k0:].ctypes.data_as(i64p), poses[k0:].ctypes.data_as(f64p), k1 - k0, self.sigma,
+                float(kappa_scaled), _abi.ptr(out[k0:k1]), _abi.ptr(self.scratch), self.scratch.numel(),
+                _abi.stream_ptr(self.device)), "shine_register_normal_eq_scans")
+            k0 = k1
+
     def _scaled(self, poses) -> np.ndarray:
         P = np.array(poses, dtype=np.float64).reshape(-1, 4, 4)
         P[:, :3, 3] *= self.scale
@@ -206,65 +259,164 @@ class ScanToMapRegistration:
         self.launch(points, T, (self.kappa_m if kappa_m is None else kappa_m) * self.scale)
         return unpack_normal_equations(self.out.cpu().numpy())
 
-    def gauss_newton(self, points: torch.Tensor, pose: np.ndarray) -> tuple:
-        """-> (pose, iterations, converged, failure reason or None)."""
-        pose = np.array(pose, dtype=np.float64)
-        for it in range(self.max_iters):
-            wide = it < len(self.WIDE)
-            H, b, cost, count = self.normal_equations(points, pose, self.kappa_m * (self.WIDE[it] if wide else 1.0))
-            if count < self.min_valid:
-                return pose, it + 1, False, f"{count} points on the map (< {self.min_valid})"
-            if not np.all(np.isfinite(H)) or np.linalg.cond(H) > 1e12:
-                return pose, it + 1, False, "singular normal equations"
-            xi = -np.linalg.solve(H, b)
-            step = se3_exp(xi)
-            step[:3, 3] /= self.scale                       # rho was in scaled units
-            pose = step @ pose
-            if not wide and np.linalg.norm(xi[:3]) / self.scale < self.tol and np.linalg.norm(xi[3:]) < self.tol:
-                return pose, it + 1, True, None
-        return pose, self.max_iters, False, None
+    # ---- the policy, for S scans in lock-step ------------------------------------------------------------------------
+    # Each stage takes the scans as segments (begin, n) of one points array, one pose each.  A step of a stage is one
+    # launch_items over the items of every scan still in it and one read; what follows per scan (the condition test,
+    # the solve, the update, the choice of a candidate) is host arithmetic, the same for a scan whatever the others do.
 
-    def search_weak_direction(self, points: torch.Tensor, pose: np.ndarray) -> tuple:
-        """The best pose along the weakest translation direction (class docstring), all candidates in one launch_poses
-        -> (pose, moved)."""
-        H, _, _, _ = self.normal_equations(points, pose)
-        score0 = float(np.trace(H[:3, :3]))
-        v = np.linalg.eigh(H[:3, :3])[1][:, 0]              # eigenvalues ascending
+    def _rows(self, points: torch.Tensor, segments, poses, kappa_m: float) -> np.ndarray:
+        """The 29 values of each item (segment, pose in metres) at kappa_m: one launch_items and one read."""
+        P = self._scaled(poses)
+        out = torch.empty(P.shape[0], _abi.REGISTER_OUT, dtype=torch.float64, device=self.device)
+        self.launch_items(points, segments, P, kappa_m * self.scale, out)
+        return out.cpu().numpy()
+
+    def coarse_scans(self, points: torch.Tensor, segments, poses: list) -> list:
+        """Each scan's candidate of the grid around its pose (GRID_X x GRID_Y x GRID_YAW) with the largest inlier score
+        sum w |g|^2 at twice kappa: the candidates of every scan in one launch_items, one read of their scores."""
+        cands = []
+        for pose in poses:
+            for yaw in self.GRID_YAW:
+                c, s_ = math.cos(yaw), math.sin(yaw)
+                Rz = np.array([[c, -s_, 0.0], [s_, c, 0.0], [0.0, 0.0, 1.0]])
+                for dx in self.GRID_X:
+                    for dy in self.GRID_Y:
+                        T = pose.copy()
+                        T[:3, :3] = Rz @ pose[:3, :3]
+                        T[:3, 3] = pose[:3, 3] + (dx, dy, 0.0)
+                        cands.append(T)
+        per = len(cands) // max(len(poses), 1)
+        outs = torch.empty(len(cands), _abi.REGISTER_OUT, dtype=torch.float64, device=self.device)
+        self.launch_items(points, np.repeat(np.asarray(segments, dtype=np.int64).reshape(-1, 2), per, axis=0),
+                          self._scaled(cands), 2.0 * self.kappa_m * self.scale, outs)
+        score = (outs[:, 0] + outs[:, 6] + outs[:, 11]).cpu().numpy()        # H(0,0) + H(1,1) + H(2,2)
+        return [cands[i * per + int(np.argmax(score[i * per:(i + 1) * per]))] for i in range(len(poses))]
+
+    def gauss_newton_scans(self, points: torch.Tensor, segments, poses: list) -> list:
+        """Gauss-Newton from each pose, iteration i of every scan still running in one step, at the kappa of iteration
+        i -> [(pose, iterations, converged, failure reason or None)] per scan."""
+        segments = np.asarray(segments, dtype=np.int64).reshape(-1, 2)
+        state = [np.array(p, dtype=np.float64) for p in poses]
+        result = [None] * len(state)
+        running = list(range(len(state)))
+        for it in range(self.max_iters):
+            if not running:
+                break
+            wide = it < len(self.WIDE)
+            rows = self._rows(points, segments[running], [state[s] for s in running],
+                              self.kappa_m * (self.WIDE[it] if wide else 1.0))
+            still = []
+            for s, row in zip(running, rows):
+                pose = state[s]
+                H, b, cost, count = unpack_normal_equations(row)
+                if count < self.min_valid:
+                    result[s] = (pose, it + 1, False, f"{count} points on the map (< {self.min_valid})")
+                    continue
+                if not np.all(np.isfinite(H)) or np.linalg.cond(H) > 1e12:
+                    result[s] = (pose, it + 1, False, "singular normal equations")
+                    continue
+                xi = -np.linalg.solve(H, b)
+                step = se3_exp(xi)
+                step[:3, 3] /= self.scale                       # rho was in scaled units
+                pose = step @ pose
+                if not wide and np.linalg.norm(xi[:3]) / self.scale < self.tol and np.linalg.norm(xi[3:]) < self.tol:
+                    result[s] = (pose, it + 1, True, None)
+                    continue
+                state[s] = pose
+                still.append(s)
+            running = still
+        for s in running:
+            result[s] = (state[s], self.max_iters, False, None)
+        return result
+
+    def search_scans(self, points: torch.Tensor, segments, poses: list) -> list:
+        """Each scan's best pose along the weakest translation direction (class docstring): one step for the normal
+        equations at the poses, one for every scan's candidates -> [(pose, moved)] per scan."""
+        if not poses:
+            return []
+        segments = np.asarray(segments, dtype=np.int64).reshape(-1, 2)
         n = int(round(self.search_m / self.search_step_m))
         steps = [k * self.search_step_m for k in range(-n, n + 1) if k != 0]
-        cands = []
-        for d in steps:
-            cand = pose.copy()
-            cand[:3, 3] += d * v
-            cands.append(cand)
-        best, best_score = 0.0, score0
-        for d, (H, _, _, _) in zip(steps, self.normal_equations_at(points, cands)):
-            score = float(np.trace(H[:3, :3]))
-            if score > best_score:
-                best, best_score = d, score
-        if best_score <= score0 * (1.0 + 1e-3):
-            return pose, False
-        out = pose.copy()
-        out[:3, 3] += best * v
-        return out, True
+        score0, dirs, cands = [], [], []
+        for pose, row in zip(poses, self._rows(points, segments, poses, self.kappa_m)):
+            H, _, _, _ = unpack_normal_equations(row)
+            score0.append(float(np.trace(H[:3, :3])))
+            v = np.linalg.eigh(H[:3, :3])[1][:, 0]          # eigenvalues ascending
+            dirs.append(v)
+            for d in steps:
+                cand = pose.copy()
+                cand[:3, 3] += d * v
+                cands.append(cand)
+        rows = self._rows(points, np.repeat(segments, len(steps), axis=0), cands, self.kappa_m) if cands else []
+        result = []
+        for i, pose in enumerate(poses):
+            best, best_score = 0.0, score0[i]
+            for d, row in zip(steps, rows[i * len(steps):(i + 1) * len(steps)]):
+                H, _, _, _ = unpack_normal_equations(row)
+                score = float(np.trace(H[:3, :3]))
+                if score > best_score:
+                    best, best_score = d, score
+            if best_score <= score0[i] * (1.0 + 1e-3):
+                result.append((pose, False))
+                continue
+            out = pose.copy()
+            out[:3, 3] += best * dirs[i]
+            result.append((out, True))
+        return result
+
+    def register_scans(self, scans: list, init_poses: list) -> list:
+        """`register` for S scans in lock-step, stage by stage: the coarse grid of every scan, Gauss-Newton, the
+        weak-direction search, Gauss-Newton again for the scans it moved, the final evaluation.  Every stage runs one
+        kappa for all scans; a scan leaves a stage when it converges or fails.  scans: fp32 [n_s,3] each (as `register`
+        takes them).  -> [(pose, info)] per scan, each equal bit for bit to `register(scans[s], init_poses[s])`."""
+        if len(scans) != len(init_poses):
+            raise ValueError(f"register_scans: {len(scans)} scans, {len(init_poses)} initial poses")
+        if not scans:
+            return []
+        counts = [int(p.shape[0]) for p in scans]
+        points = scans[0] if len(scans) == 1 else torch.cat([p.reshape(-1, 3).float() for p in scans])
+        segments = np.stack([np.cumsum([0] + counts[:-1]), counts], 1).astype(np.int64)
+        init = [np.array(p, dtype=np.float64) for p in init_poses]
+        runs = self.gauss_newton_scans(points, segments, self.coarse_scans(points, segments, init))
+        ok = [s for s, r in enumerate(runs) if r[3] is None]
+        searched = self.search_scans(points, segments[ok], [runs[s][0] for s in ok])
+        moved = [s for s, (_, m) in zip(ok, searched) if m]
+        again = self.gauss_newton_scans(points, segments[moved], [p for p, m in searched if m])
+        for s, (pose, more, converged, reason) in zip(moved, again):
+            runs[s] = (pose, runs[s][1] + more, converged, reason)
+        ok = [s for s, r in enumerate(runs) if r[3] is None]
+        final = self._rows(points, segments[ok], [runs[s][0] for s in ok], self.kappa_m) if ok else []
+        results = []
+        for s, (pose, iters, converged, reason) in enumerate(runs):
+            if reason is not None:
+                results.append((init[s], {"iters": iters, "valid": 0, "rmse_m": float("nan"), "ok": False,
+                                          "converged": False, "reason": reason}))
+                continue
+            _, _, cost, count = unpack_normal_equations(final[ok.index(s)])
+            results.append((pose, {"iters": iters, "valid": count,
+                                   "rmse_m": math.sqrt(cost / count) / self.scale if count else float("nan"),
+                                   "ok": True, "converged": converged}))
+        return results
+
+    # ---- one scan: the S = 1 case of the stages -----------------------------------------------------------------------
+
+    @staticmethod
+    def _whole(points) -> np.ndarray:
+        return np.array([[0, int(points.shape[0])]], dtype=np.int64)
+
+    def gauss_newton(self, points: torch.Tensor, pose: np.ndarray) -> tuple:
+        """-> (pose, iterations, converged, failure reason or None)."""
+        return self.gauss_newton_scans(points, self._whole(points), [np.array(pose, dtype=np.float64)])[0]
+
+    def search_weak_direction(self, points: torch.Tensor, pose: np.ndarray) -> tuple:
+        """The best pose along the weakest translation direction (class docstring), all candidates in one step
+        -> (pose, moved)."""
+        return self.search_scans(points, self._whole(points), [pose])[0]
 
     def coarse_search(self, points: torch.Tensor, pose: np.ndarray) -> np.ndarray:
         """The candidate of the grid around pose (GRID_X x GRID_Y x GRID_YAW) with the largest inlier score sum w |g|^2
-        at twice kappa: one launch_poses into one row per candidate, one read for all of them."""
-        cands = []
-        for yaw in self.GRID_YAW:
-            c, s_ = math.cos(yaw), math.sin(yaw)
-            Rz = np.array([[c, -s_, 0.0], [s_, c, 0.0], [0.0, 0.0, 1.0]])
-            for dx in self.GRID_X:
-                for dy in self.GRID_Y:
-                    T = pose.copy()
-                    T[:3, :3] = Rz @ pose[:3, :3]
-                    T[:3, 3] = pose[:3, 3] + (dx, dy, 0.0)
-                    cands.append(T)
-        outs = torch.empty(len(cands), _abi.REGISTER_OUT, dtype=torch.float64, device=self.device)
-        self.launch_poses(points, self._scaled(cands), 2.0 * self.kappa_m * self.scale, outs)
-        score = (outs[:, 0] + outs[:, 6] + outs[:, 11]).cpu().numpy()        # H(0,0) + H(1,1) + H(2,2)
-        return cands[int(np.argmax(score))]
+        at twice kappa: one step for all candidates."""
+        return self.coarse_scans(points, self._whole(points), [pose])[0]
 
     def register(self, points: torch.Tensor, init_pose: np.ndarray) -> tuple:
         """The coarse grid search, Gauss-Newton from its best candidate, the search along the weakest direction,
@@ -272,20 +424,8 @@ class ScanToMapRegistration:
         (pose, {iters, valid, rmse_m, ok, converged}).  ok=False (with `reason`): too few points on the map or a singular
         system, the initial pose is returned.  converged=False: the last Gauss-Newton run stopped at max_iters without
         meeting tol (the pose is returned, ok stays True).  valid and rmse_m = sqrt(sum w r^2 / valid) (metres) are
-        those of the returned pose."""
-        init = np.array(init_pose, dtype=np.float64)
-        pose, iters, converged, reason = self.gauss_newton(points, self.coarse_search(points, init))
-        if reason is None:
-            pose, moved = self.search_weak_direction(points, pose)
-            if moved:
-                pose, more, converged, reason = self.gauss_newton(points, pose)
-                iters += more
-        if reason is not None:
-            return init, {"iters": iters, "valid": 0, "rmse_m": float("nan"), "ok": False, "converged": False,
-                          "reason": reason}
-        _, _, cost, count = self.normal_equations(points, pose)
-        return pose, {"iters": iters, "valid": count, "rmse_m": math.sqrt(cost / count) / self.scale if count else float("nan"),
-                      "ok": True, "converged": converged}
+        those of the returned pose.  The S = 1 case of `register_scans`."""
+        return self.register_scans([points], [init_pose])[0]
 
 
 # ------------------------------------------------------------------------------------------------------ frame source

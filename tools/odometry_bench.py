@@ -9,8 +9,8 @@
    prints one line: its error against the written pose (translation m, rotation deg), the registration's info and the
    error of the pose after each stage of `register` (the constant-velocity prediction, the best coarse candidate, each
    Gauss-Newton run and the weak-direction search).  The drive runs twice, alternately:
-   with `launch_poses` forced through one `launch` per pose ("per_pose", the registration before the batched entry: the
-   same poses, bit for bit) and as built ("batched").
+   with `launch_items` forced through one `launch` per pose ("per_pose", the registration before the batched entries:
+   the same poses, bit for bit) and as built ("batched").
 2. `shine_register_normal_eq` alone at the scans' point counts on the final map: CUDA events around --reps launches
    (one Gauss-Newton iteration each, without its 29-double read; the interval includes the host's launch cost when the
    host is the slower side), and the two kernels' own durations from a torch.profiler run of the same launches.
@@ -69,25 +69,28 @@ def main(argv=None):
             self.stages = [("prediction", np.array(init))]
             return super().register(points, init)
 
-        def coarse_search(self, points, pose):
-            r = super().coarse_search(points, pose)
-            self.stages.append(("coarse", r))
+        def coarse_scans(self, points, segments, poses):
+            r = super().coarse_scans(points, segments, poses)
+            self.stages.append(("coarse", r[0]))
             return r
 
-        def gauss_newton(self, points, pose):
-            r = super().gauss_newton(points, pose)
-            self.stages.append(("gauss_newton", r[0]))
+        def gauss_newton_scans(self, points, segments, poses):
+            r = super().gauss_newton_scans(points, segments, poses)
+            if r:
+                self.stages.append(("gauss_newton", r[0][0]))
             return r
 
-        def search_weak_direction(self, points, pose):
-            r = super().search_weak_direction(points, pose)
-            self.stages.append(("weak_direction", r[0]))
+        def search_scans(self, points, segments, poses):
+            r = super().search_scans(points, segments, poses)
+            if r:
+                self.stages.append(("weak_direction", r[0][0]))
             return r
 
     class PerPose(Traced):
-        def launch_poses(self, points, poses_scaled, kappa_scaled, out):
+        def launch_items(self, points, segments, poses_scaled, kappa_scaled, out):
             for k, T in enumerate(np.asarray(poses_scaled).reshape(-1, 4, 4)):
-                self.launch(points, T, kappa_scaled, out[k])
+                b, n = (int(v) for v in np.asarray(segments).reshape(-1, 2)[k])
+                self.launch(points[b:b + n], T, kappa_scaled, out[k])
 
     def err(E, W):
         D = np.linalg.inv(W) @ E
